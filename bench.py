@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- Step-1 level-0 ridge throughput (SNPs/s) on synthetic PLINK panels.
 
-  python bench.py --gpus N --steps K --warmup W            # the B200 path (C ABI)
+  python bench.py --gpus N --steps K --warmup W            # the H100 path (C ABI)
+  python bench.py ... --dump-outputs DIR                   # also save what the last timed step computed
   python bench.py --impl reference --steps K --warmup W    # the CPU port of the reference path
 
 One "step" = one full level-0 pass (decode -> Gram -> ridge solves -> out-of-fold predictions
@@ -29,9 +30,9 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 # Hardware queues for the lane streams of a Step-1 handle: with 32 instead of the driver's default 8 the library runs 12 lanes
-# (csrc/rg_api.cu, rg_step1_create; profiles/ab_r2u_connections_lanes.txt).  The variable is read when the CUDA context is
+# (csrc/rg_api.cu, rg_step1_create).  The variable is read when the CUDA context is
 # created, i.e. it has to be in the environment before torch touches the device.  A 32-queue context takes ~1 s longer to
-# create, which a long job does not notice and a 1.3 s from-files run does: that leg's child process gets the default back.
+# create, which a long job does not notice and a short from-files run does: that leg's child process gets the default back.
 _CONN_WAS_SET = "CUDA_DEVICE_MAX_CONNECTIONS" in os.environ
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
@@ -44,7 +45,8 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (dense, 700 W board power): a bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data-sheet"
 
 
 # ----------------------------------------------------------------------------- synthetic data
@@ -77,6 +79,18 @@ def gen_pheno(N, P, C, seed):
     cov = rng.normal(size=(N, C - 1))
     na = rng.random(size=(N, P)) < 0.02
     return Y, cov, na
+
+
+def dump_outputs(d, st, nblocks, traits, N):
+    """What a caller of the timed pass receives, sampled to a few MB: the level-0 predictors W (float64, N x R per block
+    and trait) of the first, middle and last block for the given traits, at a fixed seeded sample of 8192 sample rows.
+    W_block<b>.npy is [len(traits)][rows][R]; traits.npy lists the traits."""
+    os.makedirs(d, exist_ok=True)
+    rows = np.sort(np.random.default_rng(SEED).choice(N, size=min(N, 8192), replace=False))
+    np.save(os.path.join(d, "sample_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(d, "traits.npy"), np.asarray(traits, dtype=np.float64))
+    for b in sorted({0, nblocks // 2, nblocks - 1}):
+        np.save(os.path.join(d, "W_block%04d.npy" % b), np.stack([st.fetch_W(b, p)[rows] for p in traits]))
 
 
 def blocks_of(M, bsize):
@@ -271,7 +285,7 @@ def run_gpu(args):
         import torch.distributed as dist
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     if not torch.cuda.is_available() or capi.lib().rg_device_count() == 0:
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback)")
+        raise SystemExit("bench.py: no CUDA device (the H100 path has no CPU fallback)")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     c = CFG
@@ -361,11 +375,14 @@ def run_gpu(args):
         raise SystemExit("level-0 reported an error (timed pass): " + capi.lib().rg_last_error().decode())
     total_snps = M * args.steps * world
     value = total_snps / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        # sharded (--gpus N > 1): rank 0 holds the W of the traits it owns (p mod world == 0) for every block
+        dump_outputs(args.dump_outputs, st, len(blocks) * world, [p for p in range(P) if owner is None or owner[p] == 0], N)
 
     # ---- per-kernel durations with CUDA events on the launching stream.  The timed region overlaps
     # consecutive blocks on several streams ("lanes"), so a kernel's event-bracketed time there includes
     # time-sharing with other kernels; for the roofline each kernel is ALSO timed alone (single lane).
-    knames = ["bed_relayout", "bed_expand", "l0_stats", "gram_tcgen05", "l0_assemble", "mx_solve", "chol_factor",
+    knames = ["bed_relayout", "bed_expand", "l0_stats", "gram_wgmma", "l0_assemble", "mx_solve", "chol_factor",
               "chol_backsolve", "l0_predict"]
 
     def kernel_times(handle, nsteps):
@@ -442,6 +459,17 @@ def run_gpu(args):
                                "stores to peers ride inside the prediction / standardisation kernels, overlapped with compute"
                                % (P, world, max(owner.count(r) for r in range(world)))}
 
+    cpu_missing = None
+    try:                                            # the CPU baseline needs the checker built from the reference's sources
+        from oracle import ref_eigen
+        ref_eigen.lib()
+    except OSError as e:
+        if not args.no_cpu:
+            cpu_missing = {"value": None, "note": "not measured: %s" % e}
+            args.no_cpu = True
+            print("bench.py: WARNING: the Eigen oracle is not built (%s): no CPU baseline and NO parity check in this run" % e,
+                  file=sys.stderr)
+
     # ---- end to end from files through the C++ driver (rank 0, single GPU run only)
     file_e2e = None
     if world == 1 and not args.no_step2 and not (args.small or args.n_samples or args.blocks or args.n_pheno):
@@ -472,10 +500,10 @@ def run_gpu(args):
             dist.barrier(); dist.destroy_process_group()
         return
     peaks, peak_src = load_peaks()
-    gram_ms, gram_n = kern["gram_tcgen05"]["ms_total"], max(1, kern["gram_tcgen05"]["launches"])
+    gram_ms, gram_n = kern["gram_wgmma"]["ms_total"], max(1, kern["gram_wgmma"]["launches"])
     flops_per_launch = 2.0 * bs * bs * N          # SURVEY 8(d): 2*N*bs per SNP x bs SNPs (reference src/Data.cpp:748)
     ach = flops_per_launch / (gram_ms / gram_n * 1e-3) / 1e12
-    # the Gram runs in e4m3 (exact for hard calls); FP8 dense peak = 2 x the measured BF16 cuBLAS rate
+    # the Gram runs in int8 (exact for hard calls); dense INT8 peak = 2 x the BF16 rate
     peak_bf16 = peaks.get("bf16_tflops") or peaks.get("bf16_tflops_sustained")   # kernel timed alone -> burst figure
     peak = 2.0 * peak_bf16
     ktot = sum(v["ms_total"] for v in kern.values()) or 1.0
@@ -492,8 +520,10 @@ def run_gpu(args):
     F0 = 2.0 * N * bs + 2.0 * N * P * (1 + R) + 4.0 * N * C
     step_tf = value * F0 / 1e12 / world
     peak_sust = 2.0 * (peaks.get("bf16_tflops_sustained") or peak_bf16)
-    traffic, pipe_active = gram_traffic_from_profile()
-    cpu, parity = None, None
+    traffic, pipe_active = None, None               # DRAM traffic needs a hardware-counter capture; not measured
+    cpu, parity = cpu_missing, None
+    if cpu_missing is not None:
+        parity = {"max_rel_err": None, "tol": 1e-9, "checked": False, "what": "NOT CHECKED: " + cpu_missing["note"]}
     if not args.no_cpu:
         rows = [host_panel[s:s + n].numpy() for (s, n) in blocks[: args.cpu_blocks]]
         thr, calib = calibrate_threads(rows[0], N, X, Y, mask, in_an, fsz, lam, neff)
@@ -507,7 +537,7 @@ def run_gpu(args):
             Wg = st.fetch_W(0, p)
             err = max(err, float(np.abs(Wg - W_cpu[p]).max() / np.abs(W_cpu[p]).max()))
         parity = {"max_rel_err": err, "tol": 1e-9, "what": "level-0 predictors W of block 0 (N x %d columns x %d traits) of the "
-                  "timed panel, B200 path vs the Eigen restatement of ridge_level_0" % (R, P)}
+                  "timed panel, H100 path vs the Eigen restatement of ridge_level_0" % (R, P)}
         if not (err < 1e-9):
             raise SystemExit("bench.py: parity check failed on the benchmarked configuration: max rel err %g" % err)
 
@@ -515,7 +545,7 @@ def run_gpu(args):
         "metric": "step1_level0_snps_per_sec", "value": value, "unit": "SNPs/s", "n_gpus": world,
         "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms / args.steps,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "e4m3 Gram + int8 prediction (both exact integer sums) + tf32x3 factorisation + f64 refinement / statistics",
+        "dtype": "int8 Gram + int8 prediction (both exact integer sums) + tf32x3 factorisation + f64 refinement / statistics",
         "data": "synthetic", "config": workload_config() if not (args.small or args.n_samples or args.n_pheno) else {"workload": "NOT the benchmark configuration (smoke / exploration run)", "n_samples": N, "n_snps": M, "n_pheno": P},
         "clocks": clk,
         "e2e": {"value": e2e_val, "unit": "SNPs/s", "ms_per_step": ms_e2e / args.steps,
@@ -523,21 +553,20 @@ def run_gpu(args):
                 "result_read": "every pass: rg_l0_poll_status (8-byte D2H read of the sticky error word, lanes keep running); "
                                "after the last pass, inside the timed region: rg_l0_status (waits for every block)"},
         "gpu_launches": int(launches),
-        "roofline": {"kernel": "gram_fp8_tcgen05_kernel", "bound": "tensor", "achieved": ach, "peak": peak,
+        "roofline": {"kernel": "gram_s8_wgmma_kernel", "bound": "tensor", "achieved": ach, "peak": peak,
                      "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
-                     "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full "
-                                     "(profiles/ncu_r2o_key_kernels.txt, else ncu_r1n_key_kernels.txt); algorithmic bytes = 205 MB of "
+                     "traffic_note": "DRAM bytes of one launch: not measured; algorithmic bytes = 205 MB of "
                                      "Z planes + 47 MB of Gram tiles",
                      "executed_frac": 2.0 * ach / peak, "tensor_pipe_active_ncu": pipe_active,
-                     "peak_basis": "2 x %s bf16 cuBLAS rate (%s TF/s) = dense FP8" % (peak_src, peak_bf16),
+                     "peak_basis": "2 x %s bf16 rate (%s TF/s) = dense INT8" % (peak_src, peak_bf16),
                      "algorithmic_flops_per_launch": flops_per_launch,
                      "timed": "alone (single lane), CUDA events on the launching stream",
                      "note": "kernel executes 2x this (lower triangle of the [G0;Miss] Gram) to handle missing calls exactly"},
         "step_roofline": {"flops_per_snp": F0, "achieved_tflops_per_gpu": step_tf, "peak": peak_sust, "frac": step_tf / peak_sust,
-                          "peak_basis": "2 x %s SUSTAINED bf16 cuBLAS rate = dense FP8, kernel mix timed inside a long step" % peak_src,
+                          "peak_basis": "2 x %s SUSTAINED bf16 rate = dense INT8, kernel mix timed inside a long step" % peak_src,
                           "note": "whole level-0 step (decode, statistics, Gram, solver, predictions) against the tensor "
                                   "roofline of its algorithmic flops; the solver's share is in `solver`"},
-        "solver": {"kernel": "mixed: 3xTF32 tcgen05 factorisation / inverse + FP64 refinement (chol_mixed.cu)" if mixed_blocks else
+        "solver": {"kernel": "mixed: 3xTF32 wgmma factorisation / inverse + FP64 refinement (chol_mixed.cu)" if mixed_blocks else
                              "fp64: DMMA Cholesky + back-substitution (chol.cu)",
                    "ms_per_block_single_lane": chol_ms,
                    "cholesky_equivalent_tflops": chol_tf,
@@ -618,46 +647,17 @@ def file_e2e_leg(host_panel, N, M, bs, P, Yr, cov, na, gpus=1):
         shutil.rmtree(d, ignore_errors=True)
 
 
-def step2_traffic_from_profile(kernels, variants_per_launch):
-    """DRAM bytes per variant (dram__bytes_read.sum + dram__bytes_write.sum of one launch of each named kernel, divided by the
-    variants a launch covers) from the committed ncu --set full summary of the Step-2 kernels (tools/ncu_capture_s2.sh ->
-    profiles/ncu_r2t_step2_kernels.txt; captured at N = 100k: 1000 .bed variants / 400 dosage variants per launch)."""
-    try:
-        blocks = open(os.path.join(ROOT, "profiles", "ncu_r2t_step2_kernels.txt")).read().split("---\n")
-    except OSError:
-        return None, None
-    per = {}
-    for b in blocks:                                   # the LAST captured launch of each kernel (warm handle)
-        name = next((k for k in kernels if k in b), None)
-        if name is None:
-            continue
-        d = {}
-        for line in b.splitlines():
-            t = line.split()
-            if len(t) >= 2:
-                d[t[0]] = t[1]
-        if "dram__bytes_read.sum" in d:
-            per[name] = (float(d["dram__bytes_read.sum"]) + float(d["dram__bytes_write.sum"])) * 1e6 / variants_per_launch
-    if len(per) != len(kernels):
-        return None, None
-    return sum(per.values()), {k: round(v) for k, v in per.items()}
-
-
 def hbm_roofline(rate, bytes_per_variant, what, traffic=(None, None)):
     peaks, src = load_peaks()
     gbs = rate * bytes_per_variant / 1e9
-    out = {"bound": "hbm", "achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
-           "traffic": traffic[0], "algorithmic_bytes_per_variant": bytes_per_variant, "peak_basis": "%s copy bandwidth" % src,
-           "rate_used": "device-resident variants/s x algorithmic bytes per variant (%s)" % what}
-    if traffic[0] is not None:
-        out["traffic_unit"] = "DRAM bytes per variant, all kernels of a block (ncu --set full at N = 100k, profiles/ncu_r2t_step2_kernels.txt)"
-        out["traffic_by_kernel"] = traffic[1]
-    return out
+    return {"bound": "hbm", "achieved": gbs, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": gbs / peaks["hbm_gbs"],
+            "traffic": traffic[0], "algorithmic_bytes_per_variant": bytes_per_variant, "peak_basis": "%s copy bandwidth" % src,
+            "rate_used": "device-resident variants/s x algorithmic bytes per variant (%s)" % what}
 
 
 def s2_tensor_roofline(rate, N, P, C):
     """What really bounds the hard-call Step-2 path: with per-trait masks a variant needs D = 1 + C + 2P + PC exact sums over
-    its N calls (not one pass over N/4 bytes), done as FP8 tensor tiles against 9 radix-30 digit rows per feature column for the
+    its N calls (not one pass over N/4 bytes), done as INT8 tensor tiles against 9 radix-30 digit rows per feature column for the
     three planes g0, g0^2, missing (csrc/s2_kernels.cu, s2_api.cu: digit rows padded to 14 columns per 128-row group)."""
     peaks, src = load_peaks()
     D = 1 + C + 2 * P + P * C
@@ -668,7 +668,7 @@ def s2_tensor_roofline(rate, N, P, C):
     return {"bound": "tensor", "achieved": tf, "peak": peak, "unit": "TFLOP/s", "frac": tf / peak,
             "executed_flops_per_variant": executed, "feature_columns": D, "digit_rows": drows,
             "algorithmic_flops_per_variant": 2.0 * N * D,
-            "peak_basis": "2 x %s sustained bf16 cuBLAS rate = dense FP8" % src,
+            "peak_basis": "2 x %s sustained bf16 rate = dense INT8" % src,
             "note": "the HBM line above is SURVEY 8(d)'s scan bound (N/4 bytes per variant); at %d traits the exact digit-plane "
                     "tiles are the binding resource, not the bytes" % P}
 
@@ -732,8 +732,7 @@ def step2_qt_leg(capi, X, mask, in_an, N, P, C, bs, blocks, host_panel, dev_ptr,
                     "note": "staged = rg_s2_stage copies block b+1 on a copy stream under the kernels of block b; unstaged = "
                             "the block call copies its own rows first"},
             "roofline": hbm_roofline(dev_rate, N / 4.0, "N/4 bytes of 2-bit calls",
-                                     step2_traffic_from_profile(("bed_relayout_kernel", "bed_expand3_fp8_kernel", "gram_fp8_tcgen05_kernel",
-                                                                 "s2_stats_finish_kernel", "s2_finalize_kernel"), 1000) if N == 100_000 else (None, None)),
+                                     (None, None)),
             "tensor_roofline": s2_tensor_roofline(dev_rate, N, P, C),
             "cpu_baseline": cpu,
             "sample": "%d blocks of %d variants, N=%d, %d traits; value = .bed rows resident in HBM, e2e = pinned host rows; "
@@ -946,38 +945,12 @@ def step2_bt_leg(capi, X, in_an, N, C, args, nvar=400, nblocks=4):
             "e2e_compressed_input": inflate,
             "compressed_bytes_per_variant": float(offs[-1]) / nvar,
             "roofline": hbm_roofline(dev_rate, 3.0 * N, "2N probability bytes + N ploidy bytes",
-                                     step2_traffic_from_profile(("dosage_relayout_kernel", "dosage_stats_kernel", "s2_bt_finalize_kernel"), 400)
-                                     if N == 100_000 else (None, None)),
+                                     (None, None)),
             "cpu_baseline": cpu, "firth_fraction": ff,
             "sample": "%d blocks of %d variants, N=%d, 1 binary trait (prevalence 10 %%), score test + approximate Firth for |z| > 1.96; "
                       "value = inflated bytes resident in HBM, e2e = pinned host probability + ploidy bytes (3N B/variant), "
                       "e2e_compressed_input = zlib payloads from host memory, inflated on the device (direct / shared-memory "
                       "window kernel) in front of the same calls" % (nblocks, nvar, N)}
-
-
-def gram_traffic_from_profile():
-    """DRAM bytes per launch and tensor-pipe activity of the Gram kernel from the committed ncu --set full summary
-    (bench.py cannot run under a profiler; the capture command is tools/ncu_capture.sh)."""
-    blocks = []
-    for name in ("ncu_r2o_key_kernels.txt", "ncu_r1n_key_kernels.txt"):      # newest committed capture first
-        try:
-            blocks = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", name)).read().split("---\n")
-            break
-        except OSError:
-            continue
-    for b in blocks:
-        if "gram_fp8_tcgen05_kernel" not in b or "launch__grid_size" not in b:
-            continue
-        d = {}
-        for line in b.splitlines():
-            t = line.split()
-            if len(t) >= 2:
-                d[t[0]] = t[1]
-        if d.get("launch__grid_size") != "360":            # the bs x bs Gram launch (72 tiles x 5 folds), not the statistics tiles
-            continue
-        mb = float(d["dram__bytes_read.sum"]) + float(d["dram__bytes_write.sum"])
-        return mb * 1e6, float(d["sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active"]) / 100.0
-    return None, None
 
 
 def main():
@@ -993,6 +966,9 @@ def main():
     ap.add_argument("--blocks", type=int, default=0, help="profiling only: restrict the pass to the first n blocks")
     ap.add_argument("--n-samples", type=int, default=0, help="exploration only: other sample count, --blocks blocks (default 20)")
     ap.add_argument("--n-pheno", type=int, default=0, help="exploration only: other trait count (configs[4] has 50)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the level-0 predictors of the last timed step as DIR/<name>.npy (seeded sample, < 64 MB; "
+                         "with --gpus N > 1 the traits rank 0 owns)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * rg_b200.h -- C ABI of the B200-native regenie hot path (librg_b200.so).
+ * rg_b200.h -- C ABI of the H100-native regenie hot path (librg_b200.so).
  *
  * The reference (rgcgithub/regenie v4.1.2) has no FFI: its hot path is a sequence of
  * C++ member/free functions called from Data::run_step1 / Data::test_snps_fast.  Each
@@ -19,7 +19,7 @@
  *     handle's CUDA stream and are asynchronous until rg_sync or a call that returns
  *     host data.
  *   - there is NO CPU fallback: every call fails with an error when no CUDA device
- *     (sm_100) is usable.
+ *     (sm_90) is usable.
  */
 #ifndef RG_B200_H
 #define RG_B200_H

@@ -1,9 +1,10 @@
 """Build recipe for the compiled checker under oracle/ (test infrastructure; never the product path).
 
 `oracle/ref_eigen/regenie_ref_eigen.cpp` (our C++ restatement of the reference's level-0 / score-test arithmetic) is
-compiled against the reference's OWN vendored Eigen, where it lies: /root/reference/external_libs/eigen-3.4.0.  Flags
-follow the reference Makefile (:33 `-O3 -ffast-math`, :49 `-fopenmp`).  Outputs go to oracle/_ref/ only (git-ignored,
-shipped to the GPU box with the snapshot; /root/reference does not exist there, so the prebuilt files are used).
+compiled against the reference's OWN vendored Eigen (external_libs/eigen-3.4.0 of a regenie checkout, located by
+RG_REF_EIGEN).  Flags follow the reference Makefile (:33 `-O3 -ffast-math`, :49 `-fopenmp`).  Outputs go to oracle/_ref/
+only (git-ignored).  Without the reference's sources nothing is built: the tests compare against the outputs of these
+libraries stored under tests/golden/, and bench.py skips its CPU baseline.
 
 Also built here: the reference's vendored pgenlib itself (external_libs/pgenlib, plain g++ over its own few sources, no
 cmake / external libraries) behind oracle/ref_pgenlib/pgen_ref_shim.cpp -> oracle/_ref/libpgenlib_ref.so, the reference
@@ -20,11 +21,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(HERE, "_ref")
 SRC = os.path.join(HERE, "ref_eigen", "regenie_ref_eigen.cpp")
-EIGEN = os.environ.get("RG_REF_EIGEN", "/root/reference/external_libs/eigen-3.4.0")
+EIGEN = os.environ.get("RG_REF_EIGEN", os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference", "external_libs", "eigen-3.4.0"))
 LIBS = {"libregenie_ref_eigen.so": [], "libregenie_ref_eigen_avx2.so": ["-mavx2", "-mfma"]}
 
 
-PGENLIB = os.environ.get("RG_REF_PGENLIB", "/root/reference/external_libs/pgenlib")
+PGENLIB = os.environ.get("RG_REF_PGENLIB", os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference", "external_libs", "pgenlib"))
 PGEN_SHIM = os.path.join(HERE, "ref_pgenlib", "pgen_ref_shim.cpp")
 PGEN_LIB = os.path.join(OUT, "libpgenlib_ref.so")
 
@@ -35,9 +36,10 @@ def build_pgenlib(verbose=False):
     import glob
     gxx = shutil.which("g++")
     if not (os.path.isdir(PGENLIB) and gxx):
-        if os.path.exists(PGEN_LIB):
-            return                             # GPU box: the prebuilt checker travels with the snapshot
-        raise RuntimeError("oracle/_ref/libpgenlib_ref.so missing and the reference's pgenlib (%s) is not available" % PGENLIB)
+        if not os.path.exists(PGEN_LIB):
+            print("oracle: %s not built: the reference's pgenlib sources are not at %s (set RG_REF_PGENLIB)"
+                  % (os.path.relpath(PGEN_LIB, os.path.dirname(HERE)), PGENLIB), file=sys.stderr)
+        return
     if os.path.exists(PGEN_LIB) and os.path.getmtime(PGEN_LIB) > max(os.path.getmtime(PGEN_SHIM), os.path.getmtime(__file__)):
         return
     os.makedirs(OUT, exist_ok=True)
@@ -60,9 +62,11 @@ def build(verbose=False):
     for name, extra in LIBS.items():
         lib = os.path.join(OUT, name)
         if not have_src:
-            if os.path.exists(lib):
-                continue                       # GPU box: prebuilt checker travels with the snapshot
-            raise RuntimeError("oracle/_ref/%s missing and the reference's Eigen (%s) is not available to build it" % (name, EIGEN))
+            if not os.path.exists(lib):
+                print("oracle: oracle/_ref/%s not built: the reference's Eigen is not at %s (set RG_REF_EIGEN); the tests "
+                      "use the stored outputs under tests/golden/, bench.py runs without its CPU baseline and parity check"
+                      % (name, EIGEN), file=sys.stderr)
+            continue
         if os.path.exists(lib) and os.path.getmtime(lib) > max(os.path.getmtime(SRC), os.path.getmtime(__file__)):
             continue
         os.makedirs(OUT, exist_ok=True)

@@ -1,7 +1,7 @@
 """In-tree build of librg_b200.so (CUDA kernels + C ABI) and the rgb200 host driver.
 
-nvcc cross-compiles for sm_100a without a GPU; the .so is git-ignored but travels to the GPU
-box with the repo snapshot.  Rebuilds only when a source is newer than its object.
+nvcc cross-compiles for sm_90a (H100) without a GPU; the .so and the objects are build products (git-ignored).
+Rebuilds only when a source is newer than its object.
 """
 import os
 import shutil
@@ -17,8 +17,9 @@ DRIVER = os.path.join(HERE, "rgb200")
 PROBE = os.path.join(HERE, "rgb200_hostprobe")     # CPU-only test hook for the host logic (host/probe/)
 
 NVCC = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    ARCH[0], ARCH[1], "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall,-Wno-unused-function", "--expt-relaxed-constexpr",
     "-I", os.path.join(ROOT, "include"),
 ]
@@ -55,7 +56,7 @@ def headers():
 def build_lib(verbose=False, force=False, extra_flags=()):
     if not os.path.exists(NVCC):
         if os.path.exists(LIB):
-            return LIB          # GPU box without a toolchain problem: use the prebuilt library
+            return LIB          # no toolchain here: use the library built earlier
         raise RuntimeError("nvcc not found and no prebuilt librg_b200.so")
     os.makedirs(OBJ, exist_ok=True)
     objs = []
@@ -66,8 +67,7 @@ def build_lib(verbose=False, force=False, extra_flags=()):
         if force or _newer([src] + hdrs, obj):
             _run([NVCC] + NVCC_FLAGS + list(extra_flags) + ["-c", src, "-o", obj], verbose)
     if force or _newer(objs, LIB):
-        _run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-             "-lcuda" if False else "-lcudart"], verbose)
+        _run([NVCC, "-shared", "-o", LIB] + objs + ARCH + ["-lcudart"], verbose)
     return LIB
 
 

@@ -2,7 +2,7 @@
 
 This is plumbing for tests / bench.py; the product boundary is the C header.  There is no
 CPU fallback: importing works anywhere (so CPU-only checks can verify the exported symbols),
-but every compute entry point raises RgError when no sm_100 device is present.
+but every compute entry point raises RgError when no sm_90 device is present.
 """
 import ctypes as C
 import os

@@ -61,11 +61,10 @@ __global__ void bed_relayout_kernel(const uint8_t* __restrict__ packed, int64_t 
   gp[(int64_t)row * words_per_row + w] = out;
 }
 
-// 2-bit codes -> two operand planes whose bytes are valid in BOTH 8-bit tensor-core formats:
-//   dosage 0 / 1 / 2 -> 0x00 / 0x08 / 0x10  =  2^-6 * (0, 1, 2) as e4m3 (0x08 is the smallest normal)  =  8 * (0, 1, 2) as int8,
-//   missing indicator -> 0x08.
-// The FP8 Gram (kind::f8f6f4) therefore accumulates 2^-12 x the integer Gram - still exact in FP32, a power-of-two scale the
-// epilogue removes (kZScaleGram) - and the INT8 prediction kernel (kind::i8) reads the same bytes as small integers.
+// 2-bit codes -> two int8 operand planes:
+//   dosage 0 / 1 / 2 -> 0x00 / 0x08 / 0x10  =  8 * (0, 1, 2),   missing indicator -> 0x08.
+// The INT8 Gram therefore accumulates 64 x the integer Gram - exact in int32, a power-of-two scale the epilogue removes
+// (kZScaleGram) - and the INT8 prediction kernel reads the same bytes.
 // Byte-permute does the 4-way table lookup: selector nibble k = code of sample k.
 __device__ __forceinline__ uint32_t spread_sel(uint32_t b) {
   return (b & 0x3u) | ((b & 0xCu) << 2) | ((b & 0x30u) << 4) | ((b & 0xC0u) << 6);

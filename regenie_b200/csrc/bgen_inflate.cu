@@ -8,11 +8,9 @@
 // (`probs` [bs][n_file][2], `ploidy_missing` [bs][n_file]), i.e. exactly what host/bgen.cpp produces on the host.
 //
 // The decoder core is verified against zlib on the CPU (tests/test_host_cpu.py: every variant of the reference's BGEN
-// fixtures plus 128 synthetic streams covering stored / fixed / dynamic blocks and the error paths) and on a B200 through
-// the driver (`--gpu-inflate` output is byte-identical to the host-zlib path, tests/test_driver_gpu.py).  Measured
-// (profiles/inflate_bench_r1.txt, N = 100k, 1000 variants per block, H2D of the compressed bytes included): 30 ms per
-// block = 9.9 GB/s of inflated bytes, against 1.9 GB/s for zlib on 32 host threads.  The default stays host zlib until the
-// Step-2 bench leg is switched over.
+// fixtures plus 128 synthetic streams covering stored / fixed / dynamic blocks and the error paths) and on the GPU through
+// the driver (`--gpu-inflate` output is byte-identical to the host-zlib path, tests/test_driver_gpu.py).  The default stays host
+// zlib until the Step-2 bench leg is switched over.
 #include <stdlib.h>
 
 #include "context.cuh"
@@ -52,7 +50,7 @@ bgen_inflate_kernel(const uint8_t* __restrict__ comp, const uint64_t* __restrict
 // Variant with the last 16 KB of every stream's output in shared memory (inflate_zlib_window): matches are ring-to-ring
 // copies and global memory is written in coalesced runs.  Selected with RG_B200_INFLATE=window; verified against zlib on
 // the CPU like the direct variant (tests/test_host_cpu.py, tools/inflate_fuzz.cpp, both lane orders), NOT yet run or timed
-// on a B200 - the direct kernel above stays the default until it has been.
+// on the GPU - the direct kernel above stays the default until it has been.
 constexpr int kWindowWarps = 4;
 constexpr size_t kWindowWarpBytes = rgi::kWinBytes + ((sizeof(rgi::Tables) + 15) / 16) * 16;
 constexpr size_t kWindowSmem = kWindowWarps * kWindowWarpBytes;

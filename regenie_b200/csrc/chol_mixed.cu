@@ -1,5 +1,5 @@
 // Mixed-precision solve of the K*R level-0 ridge systems  (A_f + lambda_r I) x = b_f :
-//   factorisation, triangular inverse and A^-1 in FP32-accurate 3xTF32 arithmetic on the tcgen05 tensor pipe
+//   factorisation, triangular inverse and A^-1 in FP32-accurate 3xTF32 arithmetic on the wgmma tensor pipe
 //   (tf32_gemm.cu), then FP64 iterative refinement  x <- x + X (b - A x)  against the FP64 systems.
 //
 // Reference semantics (src/Step1_Models.cpp:484-494): beta = V (D + lambda I)^-1 V^T (GtY - GtY_f) from one
@@ -8,8 +8,8 @@
 // host re-solves that block in FP64 (rg_api.cu).
 //
 // Why this shape: a right/left-looking FP64 Cholesky of 25 systems of 1024 unknowns is 16 panel steps of latency-bound
-// 25-CTA grids on the DMMA pipe (profiles/ncu_r1n_key_kernels.txt: 7 TF/s).  Here
-//   * the n^3/3 update flops run as 128x128 tcgen05 tiles (3xTF32, FP32 accumulate in TMEM),
+// 25-CTA grids on the DMMA pipe.  Here
+//   * the n^3/3 update flops run as 128x128 wgmma tiles (3xTF32, FP32 accumulate in registers),
 //   * the only serial piece is the 128x128 diagonal tile (FP32, one CTA per system, warp-register Cholesky),
 //   * the substitutions run block-wise against the stored inverses M_k = L_kk^-1 of the diagonal tiles, one CTA per
 //     system streaming L once per sweep (mx_trisolve_kernel); a refinement step is one FP64 residual pass + one such solve.
@@ -393,8 +393,8 @@ mx_residual_fused_kernel(const double* __restrict__ Af, const double* __restrict
 // contraction range, so a sub-tile costs no shuffles and no bank conflicts (the tile is read [c][r], r contiguous).  L is
 // kept as one FP32 plane with BOTH triangles (lower = L, upper = L^T, written by the TRSM tiles' epilogue) and M_k in both
 // orientations, which makes the two sweeps the same code on different triangles.  FP32 throughout - a correction needs
-// few digits - and the result is added to the FP64 solution.  The first version (plain loads, one CTA per system) reached
-// 13 GB/s per SM and 365 us per solve (profiles/launches_r2e_mixed.txt); per-SM TMA streaming is what fixes that.
+// few digits - and the result is added to the FP64 solution.  The first version (plain loads, one CTA per system) was
+// bound by its load latency; per-SM TMA streaming is what fixes that.
 // grid: (nmat), block TS_THREADS = TS_CW consumer warps + 1 producer warp.
 constexpr int TS_STAGES = 6;
 constexpr int TS_SUB = 32;                          // contraction indices per sub-tile
@@ -496,29 +496,16 @@ mx_trisolve_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_constan
     ts_mbar_wait(full_bar + 8 * s, ph);
     const float* t = tiles + (size_t)s * (TS_STAGE_BYTES / 4) + (size_t)(half * TS_CPP) * PT + row;
     const float* y = vec + (size_t)(half * TS_CPP) * TS_VP;
-    // packed FP32 FMAs (fma.rn.f32x2, two right-hand sides per instruction: same roundings as scalar fmaf): this sweep
-    // is issue-bound (profiles/ncu_r2k_*: 2.1 warp instructions per cycle and SM), a c step is 1 + 3 loads and PMAX / 2 FMAs
-    unsigned long long a2[PMAX / 2];
-#pragma unroll
-    for (int p = 0; p < PMAX / 2; ++p) asm("mov.b64 %0, {%1, %2};" : "=l"(a2[p]) : "f"(acc[2 * p]), "f"(acc[2 * p + 1]));
 #pragma unroll
     for (int c = 0; c < TS_CPP; ++c) {
       const float tv = t[(size_t)c * PT];
-      unsigned long long tv2;
-      asm("mov.b64 %0, {%1, %1};" : "=l"(tv2) : "f"(tv));
       const float4 y0 = *reinterpret_cast<const float4*>(y + c * TS_VP);
       const float4 y1 = *reinterpret_cast<const float4*>(y + c * TS_VP + 4);
       const float4 y2 = *reinterpret_cast<const float4*>(y + c * TS_VP + 8);
       const float yy[12] = {y0.x, y0.y, y0.z, y0.w, y1.x, y1.y, y1.z, y1.w, y2.x, y2.y, y2.z, y2.w};
 #pragma unroll
-      for (int p = 0; p < PMAX / 2; ++p) {
-        unsigned long long yp;
-        asm("mov.b64 %0, {%1, %2};" : "=l"(yp) : "f"(yy[2 * p]), "f"(yy[2 * p + 1]));
-        asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a2[p]) : "l"(tv2), "l"(yp));
-      }
+      for (int p = 0; p < PMAX; ++p) acc[p] = fmaf(tv, yy[p], acc[p]);
     }
-#pragma unroll
-    for (int p = 0; p < PMAX / 2; ++p) asm("mov.b64 {%0, %1}, %2;" : "=f"(acc[2 * p]), "=f"(acc[2 * p + 1]) : "l"(a2[p]));
     __syncwarp();
     if (lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(empty_bar + 8 * s) : "memory");
     ++it;
@@ -707,7 +694,7 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
   ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<10, 16>), 220 * 1024);
   RG_CHECK(n <= 2048, "mixed solver: n <= 2048");
   // profiling aid (results are garbage): RG_DBG_SKIP=mxgemm|mxpotrf|mxtri|mxres drops one kernel family of the solver so
-  // its marginal cost under multi-lane overlap can be read off (profiles/ablation_r2_*.txt)
+  // its marginal cost under multi-lane overlap can be read off
   static const char* skip_env = getenv("RG_DBG_SKIP");
   const bool sk_gemm = skip_env && strstr(skip_env, "mxgemm"), sk_potrf = skip_env && strstr(skip_env, "mxpotrf");
   const bool sk_tri = skip_env && strstr(skip_env, "mxtri"), sk_res = skip_env && strstr(skip_env, "mxres");
@@ -716,7 +703,7 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
   Tf32GemmEpilogue e0{};
   e0.n = n; e0.out_mat_stride = (int64_t)n * n;
   static const int l2pf = [] { const char* e = getenv("RG_B200_MX_L2PF"); return e ? std::max(0, std::min(8, atoi(e))) : 0; }();
-  e0.l2_prefetch = l2pf;       // measured: no gain (0 / 3 / 6 chunks ahead: 38.3 / 39.0 / 40.6 ms per step, profiles/ab_r2m_solver_variants.txt)
+  e0.l2_prefetch = l2pf;       // off by default
   // ---- factorisation: left-looking, 128-wide panels
   for (int k = 0; k < nt; ++k) {
     Tf32GemmEpilogue e = e0;

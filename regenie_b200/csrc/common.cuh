@@ -1,4 +1,4 @@
-// Shared declarations for the sm_100a kernels behind include/rg_b200.h.
+// Shared declarations for the sm_90a kernels behind include/rg_b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda.h>

@@ -10,8 +10,7 @@ constexpr int kMaxRidge = 8;
 constexpr int kMaxPhenoTile = 8;
 constexpr int kLimbs = 9;          // radix-30 digits per coefficient (44 bits)
 constexpr int kLimbsI8 = 5;        // radix-254 int8 digits per coefficient of the INT8 prediction kernel (40 bits)
-constexpr int kLimbQI8 = 50;       // outputs per INT8 prediction pass (5 x 50 = 250 <= 256 TMEM columns)
-constexpr int kLimbQ = 56;         // outputs per tensor-core prediction pass (9 x 56 = 504 <= 512 TMEM columns)   // phenotypes per register pass of the LOOCV prediction kernel
+constexpr int kLimbQI8 = 50;       // outputs per INT8 prediction pass (5 x 50 = 250 <= 256 digit rows)   // phenotypes per register pass of the LOOCV prediction kernel
 
 // ---- bed_kernels.cu
 void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int rows_p,
@@ -62,7 +61,7 @@ void launch_l0_fold_reduce(const int32_t* cnt_part, const double* sum_part, int 
 void launch_l0_snp_finalize(const SnpFinalizeArgs& a, cudaStream_t s);
 void launch_l0_assemble(const AssembleArgs& a, const double* rhs, int P, int Ppad, int nmat, cudaStream_t s);
 
-// ---- gram_tcgen05.cu
+// ---- gram_wgmma.cu
 void make_gram_tensor_map(CUtensorMap* tm, const uint8_t* z, int64_t npad, int rows2);
 size_t gram_smem_bytes(int bn = 256);
 // ---- l0_stats_tc.cu: the statistics as extra Gram column tiles
@@ -74,11 +73,11 @@ void launch_l0_stats_finish(const float* T, int ldt, int64_t t_fold_stride, cons
                             int64_t zz_fold_stride, int rows_p, int cpp, int ncol, int K, const double* scale,
                             int32_t* cnt_fold, double* sum_fold, cudaStream_t s);
 void gram_tile_list(int rows2, std::vector<int2>& tiles);
-void launch_gram_tcgen05(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
+void launch_gram_wgmma(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
                          float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256);
-// operand-plane bytes of the Step-1 block (bed_expand_fp8_kernel): dosage d -> 8 d as int8 = 2^-6 d as e4m3
-constexpr float kZScaleGram = 4096.f;     // Z Z^T tiles: both operands carry 2^-6
-constexpr float kZScaleStat = 64.f;       // Z [X|Y]-digit tiles: the digit rows are plain e4m3 integers
+// operand-plane bytes of the Step-1 block (bed_expand_fp8_kernel): dosage d -> 8 d as int8
+constexpr float kZScaleGram = 1.f / 64;   // Z Z^T tiles: both operands carry 8
+constexpr float kZScaleStat = 1.f / 8;    // Z [X|Y]-digit tiles: the digit rows are plain int8 integers
 void launch_gram_reference(const uint8_t* z, int64_t npad, int rows2, int k0, int k1, float* out, int ldo,
                            cudaStream_t s);
 
@@ -92,7 +91,7 @@ size_t chol_inv_elems(int nC, int batch);
 void launch_chol_rows_backsolve(double* cm, int64_t stride, int nC, int row0, int nrows, int batch,
                                 const double* inv, cudaStream_t s);
 
-// ---- tf32_gemm.cu: batched 128x128 "NT" tiles in 3xTF32 on tcgen05 (operands = hi/lo FP32 planes [batch][2][n][n])
+// ---- tf32_gemm.cu: batched 128x128 "NT" tiles in 3xTF32 on wgmma (operands = hi/lo FP32 planes [batch][2][n][n])
 struct Tf32GemmEpilogue {
   int n;                      // matrix dimension = row stride of every output
   int64_t out_mat_stride;     // elements per plane per matrix (n * n)
@@ -181,7 +180,7 @@ void launch_l0_standardize(const double* part, int ntiles, int Qp, int Q, int P,
                            const uint8_t* is_real, cudaStream_t s, const double* const* src = nullptr, int src_col0 = 0);
 int predict_qt();
 
-// ---- predict_tcgen05.cu
+// ---- predict_wgmma.cu
 struct PredictTcArgs {
   int rows_p, C, P, Q, Qp, cpp, col0, ngroups;
   int64_t npad;
@@ -192,18 +191,12 @@ struct PredictTcArgs {
   const uint8_t* mask;
   double* const* W;
   double* part;
-  long long* dbg;            // optional per-CTA clock64 stamps (profiling aid)
   int l2_prefetch = 0;       // INT8 kernel: k-blocks of the genotype planes prefetched into L2 ahead of the ring
 };
 void make_byte_tensor_map(CUtensorMap* tm, const uint8_t* basep, int64_t inner, int64_t rows);
-size_t predict_tc_dig_bytes(int K, int ngroups, int rows_p);
-void launch_l0_gamma_limbs(const double* gam, const double* gmu, int Qp, int Q, int bs, int rows_p, int K,
-                           double* scale, uint8_t* dig, int ngroups, cudaStream_t s);
 int launch_l0_colsum(double* const* W, int64_t npad, int col0, int P, int Q, int Qp, double* part,
                      cudaStream_t s);
-void launch_l0_predict_tcgen05(const CUtensorMap& tmZ, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
-                               cudaStream_t s);
-// INT8 variant (kind::i8): 5 radix-254 digit rows per output, 256 TMEM columns, two CTAs per SM
+// INT8 digits: 5 radix-254 digit rows per output, s8 x s8 -> s32 wgmma
 size_t predict_i8_dig_bytes(int K, int ngroups, int rows_p);
 void launch_l0_gamma_limbs_i8(const double* gam, const double* gmu, int Qp, int Q, int bs, int rows_p, int K,
                               double* scale, uint8_t* dig, int ngroups, cudaStream_t s);

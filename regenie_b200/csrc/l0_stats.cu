@@ -1,5 +1,5 @@
 // f64 sufficient statistics of a genotype block against the covariate basis and phenotypes,
-// and the assembly of the per-fold ridge systems.  Together with gram_tcgen05.cu this
+// and the assembly of the per-fold ridge systems.  Together with gram_wgmma.cu this
 // replaces Data::residualize_genotypes (reference src/Data.cpp:190-228) and the k-fold branch
 // of Data::calc_cv_matrices (src/Data.cpp:735-751) WITHOUT ever materialising the N x bs
 // double matrix: with X orthonormal,  G~ = D^-1 (G - (GX) X^T)  so
@@ -421,7 +421,7 @@ void launch_l0_assemble(const AssembleArgs& a, const double* rhs, int P, int Ppa
 
 void launch_l0_assemble_sym(const AssembleArgs& a, const double* rhs, int P, int Pp, double* bvec, cudaStream_t s) {
   // (a fold-unrolled variant with every per-fold value in registers and one barrier for all transposed tiles measured
-  // SLOWER under lane overlap - 40.8 vs 38.3 ms per step, profiles/ab_r2n_assemble.txt: 128 registers, 2 CTAs per SM)
+  // slower under lane overlap: 128 registers, 2 CTAs per SM)
   dim3 grid(a.nC / 32, a.nC / 32);
   l0_assemble_sym_kernel<<<grid, dim3(32, 8), 0, s>>>(a);
   dim3 g2((unsigned)ceil_div(a.nC, 256), Pp, a.K);

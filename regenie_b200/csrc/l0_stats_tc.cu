@@ -2,21 +2,16 @@
 //
 // The skinny products  G0 [X | Y]  and  Miss [X | Y]  per fold (A_f = G_f X_f and G_f Y_f of l0_stats.cu; the
 // reference's `Gmat * new_cov`, src/Data.cpp:199, and `Gmat * phenotypes`, src/Data.cpp:746) are one more
-// column tile of the same FP8 Gram kernel: the right operand is a fixed digit matrix D built ONCE per run from the
+// column tile of the same INT8 Gram kernel: the right operand is a fixed digit matrix D built ONCE per run from the
 // covariate basis and the phenotypes,
-//   xy[t, c] = (s_c / 15) * sum_l d_l[t, c] 30^-l,   d_l in {-15..15} (exact in e4m3), 9 limbs = 44 bits,
-// so each tensor-core product is an integer <= 30, each fold sum an exact integer < 2^24 in the FP32 TMEM
+//   xy[t, c] = (s_c / 15) * sum_l d_l[t, c] 30^-l,   d_l in {-15..15} (int8), 9 limbs = 44 bits,
+// so each tensor-core product is an integer <= 240 (the planes carry 8), each fold sum an exact integer in the int32
 // accumulators, and the FP64 Horner below reassembles  sum_t g(i,t) xy[t,c]  to ~5e-14 s_c per sample.
 // A column of ones gives sum g0 and the missing count; together with the Gram diagonal (sum g0^2) that is n1, n2, nm.
 // This replaces l0_stats_kernel + l0_fold_reduce_kernel (2.6e9 FP64 FMAs per block) by 22 % more Gram tiles.
 #include "kernels.cuh"
 
 namespace rg {
-
-namespace {
-__device__ __constant__ uint8_t kE4m3IntS[16] = {0x00, 0x38, 0x40, 0x44, 0x48, 0x4A, 0x4C, 0x4E,
-                                                 0x50, 0x51, 0x52, 0x53, 0x54, 0x55, 0x56, 0x57};
-}
 
 // digit rows of xy.  D: [drows][npad] bytes; row (c / 14) * 128 + (c % 14) * 9 + l; ones at row 126.
 // grid: cpp (+1 for the ones row), block 256.
@@ -27,7 +22,7 @@ l0_xy_digits_kernel(const double* __restrict__ xy, int cpp, int ncol, int64_t np
   const int c = blockIdx.x;
   if (c == ncol) {      // ones over the real (non-padding) samples
     uint8_t* row = D + (int64_t)kStatOnesRow * npad;
-    for (int64_t t = threadIdx.x; t < npad; t += 256) row[t] = is_real[t] ? 0x38 : 0x00;
+    for (int64_t t = threadIdx.x; t < npad; t += 256) row[t] = is_real[t] ? 0x01 : 0x00;
     return;
   }
   double mx = 0.0;
@@ -47,7 +42,7 @@ l0_xy_digits_kernel(const double* __restrict__ xy, int cpp, int ncol, int64_t np
     for (int l = 0; l < kLimbs; ++l) {
       const double d = rint(v);
       const int di = (int)d;
-      base[(int64_t)l * npad + t] = (uint8_t)(kE4m3IntS[di < 0 ? -di : di] | (di < 0 ? 0x80 : 0));
+      base[(int64_t)l * npad + t] = (uint8_t)(int8_t)di;
       v = (v - d) * 30.0;
     }
   }

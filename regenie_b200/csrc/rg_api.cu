@@ -68,7 +68,7 @@ static void require_gpu(int device) {
   RG_CHECK(device >= 0 && device < n, "invalid CUDA device ordinal");
   cudaDeviceProp prop;
   RG_CUDA(cudaGetDeviceProperties(&prop, device));
-  RG_CHECK(prop.major == 10, std::string("librg_b200 is built for sm_100a only; device is sm_") +
+  RG_CHECK(prop.major == 9 && prop.minor == 0, std::string("librg_b200 is built for sm_90a only; device is sm_") +
                                  std::to_string(prop.major) + std::to_string(prop.minor));
 }
 
@@ -246,7 +246,7 @@ void ensure_W(::rg_ctx* h) {
 }
 
 // profiling aid: RG_DBG_SKIP=<names> drops kernel groups from the pipeline (results are garbage) so the marginal
-// cost of each group under multi-lane overlap can be measured (profiles/ablation_r1.txt)
+// cost of each group under multi-lane overlap can be measured
 static bool dbg_skip(const char* name) {
   static const char* e = getenv("RG_DBG_SKIP");
   return e && strstr(e, name) != nullptr;
@@ -311,7 +311,7 @@ static void enqueue_solve_f64(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cu
   }
 }
 
-// Mixed path: K symmetric FP64 fold systems -> tcgen05 factorisation / inverse -> FP64 refinement.  Solutions in L.mx_x.
+// Mixed path: K symmetric FP64 fold systems -> tensor-core factorisation / inverse -> FP64 refinement.  Solutions in L.mx_x.
 static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, int n, cudaStream_t s) {
   const int C = h->C, P = h->P, K = h->K, R = h->R;
   const int Pp = mx_pp(P);
@@ -372,17 +372,17 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
   pa.gp = L.gp.p; pa.tile_fold = h->tile_fold.p; pa.gam = L.gam.p; pa.gmu = L.gmu.p;
   pa.cvec = L.cvec.p; pa.xy = h->xy.p; pa.mask = h->mask.p; pa.W = L.wraw_tab.p; pa.part = L.part.p;
   int nparts = d.ntiles_s;
-  // RG_B200_PREDICT = i8 (default: kind::i8, 5 radix-254 limbs) | f8 (kind::f8f6f4, 9 radix-30 limbs) | f64 (CUDA cores)
+  // RG_B200_PREDICT = i8 (default: s8 wgmma, 5 radix-254 limbs) | f64 (CUDA cores; also blocks beyond the INT8 bound)
   static const std::string predict_kind = [] { const char* e = getenv("RG_B200_PREDICT"); return std::string(e ? e : "i8"); }();
-  RG_CHECK(predict_kind == "i8" || predict_kind == "f8" || predict_kind == "f64", "RG_B200_PREDICT must be i8, f8 or f64");
+  RG_CHECK(predict_kind == "i8" || predict_kind == "f64", "RG_B200_PREDICT must be i8 or f64");
   const bool use_i8 = predict_kind == "i8" && 2 * d.rows_p <= 4096;
-  if (predict_kind == "f64") {
+  if (!use_i8) {
     launch_l0_predict(pa, d.ntiles_s, s);
   } else {
     // exact tensor-core path: digit rows of gamma against the genotype operand planes
-    const int ngroups = (int)ceil_div(d.Q, use_i8 ? kLimbQI8 : kLimbQ);
-    const int drows_per_group = use_i8 ? 256 : 512;
-    const size_t need = use_i8 ? predict_i8_dig_bytes(K, ngroups, h->rows_p_max) : predict_tc_dig_bytes(K, ngroups, h->rows_p_max);
+    const int ngroups = (int)ceil_div(d.Q, kLimbQI8);
+    const int drows_per_group = 256;
+    const size_t need = predict_i8_dig_bytes(K, ngroups, h->rows_p_max);
     if (L.dig.n < need) {
       L.dig.alloc(need);
       RG_CUDA(cudaMemsetAsync(L.dig.p, 0, need, s));
@@ -394,20 +394,14 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
       make_byte_tensor_map(&tm, L.dig.p, 2 * d.rows_p, (int64_t)K * ngroups * drows_per_group);
       L.dmaps[d.rows_p] = tm;
     }
-    if (use_i8) launch_l0_gamma_limbs_i8(L.gam.p, L.gmu.p, d.Qp, d.Q, d.bs, d.rows_p, K, L.dscale.p, L.dig.p, ngroups, s);
-    else launch_l0_gamma_limbs(L.gam.p, L.gmu.p, d.Qp, d.Q, d.bs, d.rows_p, K, L.dscale.p, L.dig.p, ngroups, s);
+    launch_l0_gamma_limbs_i8(L.gam.p, L.gmu.p, d.Qp, d.Q, d.bs, d.rows_p, K, L.dscale.p, L.dig.p, ngroups, s);
     PredictTcArgs ta;
     ta.rows_p = d.rows_p; ta.C = C; ta.P = P; ta.Q = d.Q; ta.Qp = d.Qp; ta.cpp = h->cpp; ta.col0 = 0; ta.ngroups = ngroups;
     ta.npad = Npad; ta.tile_fold = h->tile_fold.p; ta.scale = L.dscale.p; ta.cvec = L.cvec.p;
     ta.xy = h->xy.p; ta.mask = h->mask.p; ta.W = L.wraw_tab.p; ta.part = L.part.p;
-    ta.dbg = nullptr;
     static const int pred_pf = [] { const char* e = getenv("RG_B200_PREDICT_L2PF"); return e ? std::max(0, std::min(8, atoi(e))) : 0; }();
-    ta.l2_prefetch = pred_pf;       // measured: no gain (profiles/ab_r2m_solver_variants.txt)
-    if (!use_i8 && getenv("RG_DBG_CLK")) { h->dbg_clk.alloc((size_t)d.ntiles_s * ngroups * 4); ta.dbg = h->dbg_clk.p; }
-    if (!dbg_skip("predict")) {
-      if (use_i8) launch_l0_predict_i8(L.tmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
-      else launch_l0_predict_tcgen05(L.tmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
-    }
+    ta.l2_prefetch = pred_pf;       // measured: no gain
+    if (!dbg_skip("predict")) launch_l0_predict_i8(L.tmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
     nparts = launch_l0_colsum(L.wraw_tab.p, Npad, 0, P, d.Q, d.Qp, L.part.p, s);
     h->launches += 2;
   }
@@ -595,8 +589,8 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
       h->tile_counts[rows_p] = (int)tiles.size();
       h->tile_lists[rows_p] = std::move(buf);
     }
-    ScopedTimer t(h, "gram_tcgen05", s);
-    if (!dbg_skip("gram")) launch_gram_tcgen05(L.tmaps[rows_p], L.tmaps[rows_p], h->tile_lists[rows_p]->p, h->tile_counts[rows_p], h->fold_k.p, K,
+    ScopedTimer t(h, "gram_wgmma", s);
+    if (!dbg_skip("gram")) launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], h->tile_lists[rows_p]->p, h->tile_counts[rows_p], h->fold_k.p, K,
                         L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, kZScaleGram, s);
     h->launches += 1;
   }
@@ -616,7 +610,7 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     }
     L.tstat.alloc((size_t)K * 2 * h->rows_p_max * h->stat_drows);
     const int64_t tfs = (int64_t)2 * rows_p * h->stat_drows;
-    if (!dbg_skip("stats")) launch_gram_tcgen05(L.tmaps[rows_p], h->tmD, h->stat_tile_lists[rows_p]->p, h->stat_tile_counts[rows_p], h->fold_k.p,
+    if (!dbg_skip("stats")) launch_gram_wgmma(L.tmaps[rows_p], h->tmD, h->stat_tile_lists[rows_p]->p, h->stat_tile_counts[rows_p], h->fold_k.p,
                         K, L.tstat.p, h->stat_drows, tfs, kZScaleStat, s, stat_bn);
     launch_l0_stats_finish(L.tstat.p, h->stat_drows, tfs, L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, rows_p,
                            h->cpp, C + P, K, h->xy_scale.p, L.cnt_fold.p, L.sum_fold.p, s);
@@ -767,7 +761,7 @@ using namespace rg;
 extern "C" {
 
 const char* rg_last_error(void) { return rg::g_last_error.c_str(); }
-const char* rg_version(void) { return "regenie_b200 0.1 (sm_100a)"; }
+const char* rg_version(void) { return "regenie_b200 0.1 (sm_90a)"; }
 
 int rg_device_count(void) {
   int n = 0;
@@ -804,9 +798,8 @@ int rg_step1_create(const rg_step1_config* cfg, const double* X, const double* Y
   {
     // The CUDA driver multiplexes streams onto CUDA_DEVICE_MAX_CONNECTIONS hardware queues (default 8, read when the context
     // is created); streams that share a queue serialise behind each other, which is why more than 8 lanes do not pay at the
-    // default.  With 32 queues 12 lanes do (profiles/ab_r2u_connections_lanes.txt: 8 queues / 8 lanes 1.305 M SNPs/s, 32 / 12
-    // 1.343 M, flat beyond; from host rows 1.22 -> 1.31 M) - but a context with 32 queues takes 1.2 s to create instead of
-    // 0.2 s (RG_B200_PHASES of rgb200), so the library leaves the choice to the process: a long job exports
+    // default.  With 32 queues 12 lanes do - but a context with 32 queues takes about a second longer
+    // to create (RG_B200_PHASES of rgb200), so the library leaves the choice to the process: a long job exports
     // CUDA_DEVICE_MAX_CONNECTIONS=32 before its first CUDA call (bench.py does), a short one does not.
     int nl = 8;
     if (const char* q = getenv("CUDA_DEVICE_MAX_CONNECTIONS")) if (atoi(q) >= 16) nl = 12;

@@ -102,7 +102,7 @@ static void s2_build_digits(rg_ctx* h, const double* Fdev, int dp, int D) {
   RG_CUDA(cudaMemcpyAsync(h->s2_fold_k.p, fk.data(), fk.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
 }
 
-// 2-bit rows in h->gp -> S1 / S2 / Sm digit sums in h->s2_T (three e4m3 planes x digit rows, FP8 Gram kernel)
+// 2-bit rows in h->gp -> S1 / S2 / Sm digit sums in h->s2_T (three int8 planes x digit rows, INT8 Gram kernel)
 static void s2_tensor_sums(rg_ctx* h, int rows_p, cudaStream_t s) {
   const int drows = h->s2_drows;
   const int64_t Npad = h->Npad;
@@ -125,7 +125,7 @@ static void s2_tensor_sums(rg_ctx* h, int rows_p, cudaStream_t s) {
     h->s2_ntiles[key] = (int)tiles.size();
     h->s2_tile_lists[key] = std::move(buf);
   }
-  launch_gram_tcgen05(h->s2_tmZ[rows_p], h->s2_tmD, h->s2_tile_lists[key]->p, h->s2_ntiles[key], h->s2_fold_k.p,
+  launch_gram_wgmma(h->s2_tmZ[rows_p], h->s2_tmD, h->s2_tile_lists[key]->p, h->s2_ntiles[key], h->s2_fold_k.p,
                       h->s2_nchunk, h->s2_T.p, drows, (int64_t)3 * rows_p * drows, 1.f, s);
 }
 

@@ -177,9 +177,9 @@ __global__ void s2_finalize_kernel(S2FinalizeArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The same sums on the tensor cores, exactly: three e4m3 planes of a variant row (g0, g0^2, missing) against the
+// The same sums on the tensor cores, exactly: three int8 planes of a variant row (g0, g0^2, missing) against the
 // radix-30 digit rows of the feature matrix F (built once per chromosome by l0_xy_digits_kernel), as column tiles of
-// the FP8 Gram kernel.  Products are integers <= 60, sample chunks are kept below 2^18 so every TMEM sum is an exact
+// the INT8 Gram kernel.  Products are integers <= 60, sample chunks are kept below 2^18 so every sum is an exact
 // integer < 2^24; the chunk sums are added and reassembled in FP64 here.  Counts (N, A1FREQ numerators) come from the
 // 0/1 columns of F, whose digits are exact, so they stay bit-exact.
 __global__ void bed_expand3_fp8_kernel(const uint32_t* __restrict__ gp, int64_t words_per_row, int rows_p,
@@ -188,9 +188,9 @@ __global__ void bed_expand3_fp8_kernel(const uint32_t* __restrict__ gp, int64_t 
   const int row = blockIdx.y;
   if (w >= words_per_row) return;
   const uint32_t word = __ldg(gp + (int64_t)row * words_per_row + w);
-  const uint32_t kLutG = 0x00403800u;   // code 0 -> 0, 1 -> 1.0, 2 -> 2.0, 3 (missing) -> 0
-  const uint32_t kLutQ = 0x00483800u;   // g^2: 0, 1.0, 4.0 (0x48), 0
-  const uint32_t kLutM = 0x38000000u;   // missing -> 1.0
+  const uint32_t kLutG = 0x00020100u;   // code 0 -> 0, 1 -> 1, 2 -> 2, 3 (missing) -> 0
+  const uint32_t kLutQ = 0x00040100u;   // g^2: 0, 1, 4, 0
+  const uint32_t kLutM = 0x01000000u;   // missing -> 1
   uint4 g, q, m;
   uint32_t* gv = reinterpret_cast<uint32_t*>(&g);
   uint32_t* qv = reinterpret_cast<uint32_t*>(&q);

@@ -1,9 +1,9 @@
-// Batched "NT" GEMM tiles  D = A B^T  in 3xTF32 on the 5th-generation tensor cores (tcgen05 + TMEM + TMA):
+// Batched "NT" GEMM tiles  D = A B^T  in 3xTF32 on the Hopper tensor cores (wgmma + TMA + mbarrier):
 // the arithmetic engine of the mixed-precision ridge solver (chol_mixed.cu).
 //
 // Every FP32 operand lives in global memory as two planes, hi = rn_tf32(x) and lo = x - hi (exact in FP32, itself
 // truncated to TF32 by the tensor core), so that
-//     a b  ~  a_hi b_hi + a_hi b_lo + a_lo b_hi          (relative error ~2^-21, FP32 accumulation in TMEM)
+//     a b  ~  a_hi b_hi + a_hi b_lo + a_lo b_hi          (relative error ~2^-21, FP32 accumulation)
 // which is what an FP32 factorisation needs; the FP64 iterative refinement on top (chol_mixed.cu) removes the rest.
 //
 // Operand buffers are [batch][2 planes][n rows][n cols] FP32, row-major: a tile of A is 128 rows of one matrix, a
@@ -12,119 +12,35 @@
 // solve against a stored inverse  P_ik M_k^T, and of the triangular-inverse products.
 //
 // One CTA per (tile, matrix of the batch):
-//   warp 0     : TMA producer - 3-D boxes {32 floats, 128 rows, 2 planes} with 128B swizzle, 3-stage mbarrier ring
-//   warp 1     : TMEM allocator + single-thread tcgen05.mma issuer (kind::tf32, M128 N128 K8, 12 MMAs per stage)
-//   warps 2..5 : epilogue: tcgen05.ld -> registers -> optional  C_in - acc  in FP64 -> hi/lo planes (and / or the
-//                transposed tile, and / or a plain FP32 plane) with 128-bit or lane-coalesced stores
+//   warps 0..3 : one consumer warpgroup: two wgmma m64n128k8 accumulators (tile rows 0-63, 64-127, 12 MMAs each per
+//                stage), then the epilogue: accumulators -> shared memory -> optional  C_in - acc  in FP64 -> hi/lo
+//                planes (and / or the transposed tile, and / or a plain FP32 plane), one thread per tile row
+//   warp 4     : TMA producer - 3-D boxes {32 floats, 128 rows, 2 planes} with 128B swizzle, mbarrier ring
 #include <stdlib.h>
 
 #include "kernels.cuh"
+#include "wgmma_sm90.cuh"
 
 namespace rg {
 
 namespace {
 
+using namespace sm90;
+
 constexpr int TG_M = 128, TG_N = 128;
 constexpr int TG_KC = 32;                          // floats per K chunk = one 128-byte swizzle atom
-// TG_STAGES is a template parameter: 1 (default) = one 64 KiB stage per CTA, THREE CTAs per SM: the tiles of this
-                                                   // solver are short (K <= 1024) and the launches small, so latency is hidden
-                                                   // across co-resident CTAs instead of a deep per-CTA ring (profiles/ncu_r2c_*)
+// TG_STAGES is a template parameter: 1 (default) = one 64 KiB stage per CTA and several co-resident CTAs per SM: the
+// tiles of this solver are short (K <= 1024) and the launches small, so latency is hidden across CTAs
 constexpr int TG_PLANE_BYTES = TG_M * 128;         // 16 KiB
 constexpr int TG_OP_BYTES = 2 * TG_PLANE_BYTES;    // hi + lo
-constexpr int TG_STAGE_BYTES = 2 * TG_OP_BYTES;    // A + B = 64 KiB
-constexpr int TG_TMEM_COLS = 128;
-constexpr int TG_THREADS = 192;
-constexpr uint32_t TG_SPIN_LIMIT = 1u << 28;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done = 0, spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    if (done) break;
-    if (++spins > TG_SPIN_LIMIT) __trap();
-  }
-}
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// L2 prefetch of a box (no shared memory, no barrier): the operands of this solver stream from DRAM (8 lanes x 0.5 GB of
-// factor planes do not stay in the 126 MB L2) and a CTA has ONE 64 KiB stage, so the TMA load of chunk k+1 cannot start
-// before the MMAs of chunk k retire - but its bytes can already be on their way into L2.
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap* tm, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];" ::"l"(tm), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// K-major, 128B-swizzled shared-memory matrix descriptor (8-row groups 1024 B apart): same bytes as the e4m3 Gram
-// kernel's - a row is one 128-byte atom = 32 TF32 values.
-__device__ __forceinline__ uint64_t make_desc(uint32_t addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// kind::tf32: D = F32 (bits 4-5 = 1), A = B = TF32 (format 2 at bits 7-9 / 10-12), both K-major, N = 128, M = 128
-constexpr uint32_t kTf32Idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TG_N >> 3) << 17) | ((uint32_t)(TG_M >> 4) << 24);
-
-constexpr uint32_t kTf32IdescNegA = kTf32Idesc | (1u << 13);      // D (+)= (-A) B^T
-
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate, uint32_t idesc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+constexpr int TG_STAGE_BYTES = 2 * TG_OP_BYTES;    // A + B = 64 KiB (also holds the 128 x 128 FP32 result tile)
+constexpr int TG_THREADS = 160;
 
 }  // namespace
 
 // grid: (ntiles, batch); tile entry = (A row tile, B row tile, first K chunk, number of K chunks)
 template <int TG_STAGES>
-__global__ void __launch_bounds__(TG_THREADS, TG_STAGES == 1 ? 3 : 1)
+__global__ void __launch_bounds__(TG_THREADS, TG_STAGES == 1 ? 2 : 1)
 tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmI,
                       const int4* __restrict__ tiles, Tf32GemmEpilogue ep) {
@@ -135,10 +51,8 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(gen_base + TG_STAGES * TG_STAGE_BYTES);
   const uint32_t full_bar = smem_u32(bars);
   const uint32_t empty_bar = smem_u32(bars + TG_STAGES);
-  const uint32_t tmem_full_bar = smem_u32(bars + 2 * TG_STAGES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * TG_STAGES + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role
   const int4 tile = tiles[blockIdx.x];
   const int mat = blockIdx.y;
   // optional leading chunks:  acc = C_tile * I  (C = FP32 hi/lo planes of the matrix the product is subtracted from,
@@ -146,32 +60,22 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   const int ncc = ep.c_chunks;
   const int nkc = tile.w + ncc;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     for (int s = 0; s < TG_STAGES; ++s) {
       mbar_init(full_bar + 8 * s, 1);
       mbar_init(empty_bar + 8 * s, 1);
     }
-    mbar_init(tmem_full_bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    fence_barrier_init();
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
     if (ncc > 0) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmI) : "memory");
+      prefetch_tmap(&tmC);
+      prefetch_tmap(&tmI);
     }
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)TG_TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_before();
   __syncthreads();
-  fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
       const int cmat = 2 * (ep.c_mat_div > 0 ? mat / ep.c_mat_div : mat);
       // chunk kc: (kc < ncc) C tile x identity, else A / B row tiles at column (tile.z + kc - ncc) * TG_KC
@@ -202,44 +106,86 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      for (int kc = 0; kc < nkc; ++kc) {
-        const int s = kc % TG_STAGES;
-        const uint32_t ph = (kc / TG_STAGES) & 1;
-        mbar_wait(full_bar + 8 * s, ph);
-        fence_after();
-        const uint64_t a_hi = make_desc(base + s * TG_STAGE_BYTES);
-        const uint64_t a_lo = make_desc(base + s * TG_STAGE_BYTES + TG_PLANE_BYTES);
-        const uint64_t b_hi = make_desc(base + s * TG_STAGE_BYTES + TG_OP_BYTES);
-        const uint64_t b_lo = make_desc(base + s * TG_STAGE_BYTES + TG_OP_BYTES + TG_PLANE_BYTES);
-        if (kc < ncc) {
+    return;
+  }
+
+  // ===== consumer warpgroup: acc0 = tile rows 0..63, acc1 = rows 64..127 =====
+  float acc0[64], acc1[64];
 #pragma unroll
-          for (int k = 0; k < TG_KC / 8; ++k) {           // (C_lo + C_hi) * 1: the lo plane of the identity is zero
-            mma_tf32(tmem_base, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), (kc | k) ? 1u : 0u, kTf32Idesc);
-            mma_tf32(tmem_base, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u, kTf32Idesc);
-          }
-        } else {
-          const uint32_t idesc = ncc > 0 ? kTf32IdescNegA : kTf32Idesc;
+  for (int i = 0; i < 64; ++i) acc0[i] = acc1[i] = 0.f;
+  fence_regs(acc0);
+  fence_regs(acc1);
+  constexpr uint64_t kHalf = (64 * 128) >> 4;              // 64 rows further down the tile, in 16-byte units
+  for (int kc = 0; kc < nkc; ++kc) {
+    const int s = kc % TG_STAGES;
+    const uint32_t ph = (kc / TG_STAGES) & 1;
+    mbar_wait(full_bar + 8 * s, ph);
+    const uint64_t a_hi = desc_k128(base + s * TG_STAGE_BYTES);
+    const uint64_t a_lo = desc_k128(base + s * TG_STAGE_BYTES + TG_PLANE_BYTES);
+    const uint64_t b_hi = desc_k128(base + s * TG_STAGE_BYTES + TG_OP_BYTES);
+    const uint64_t b_lo = desc_k128(base + s * TG_STAGE_BYTES + TG_OP_BYTES + TG_PLANE_BYTES);
+    wgmma_fence();
+    if (kc < ncc) {
 #pragma unroll
-          for (int k = 0; k < TG_KC / 8; ++k) {
-            // +32 bytes per K = 8 step inside the swizzle atom: +2 in 16-byte descriptor units; small terms first
-            mma_tf32(tmem_base, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), (kc | k) ? 1u : 0u, idesc);
-            mma_tf32(tmem_base, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), 1u, idesc);
-            mma_tf32(tmem_base, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u, idesc);
-          }
-        }
-        tcgen05_commit(empty_bar + 8 * s);
+      for (int k = 0; k < TG_KC / 8; ++k) {             // (C_lo + C_hi) * 1: the lo plane of the identity is zero
+        const uint64_t dk = (uint64_t)(2 * k);          // +32 bytes per K = 8 step inside the swizzle atom
+        wgmma_tf32_n128(acc0, a_lo + dk, b_hi + dk);
+        wgmma_tf32_n128(acc1, a_lo + kHalf + dk, b_hi + dk);
+        wgmma_tf32_n128(acc0, a_hi + dk, b_hi + dk);
+        wgmma_tf32_n128(acc1, a_hi + kHalf + dk, b_hi + dk);
       }
-      tcgen05_commit(tmem_full_bar);
+    } else if (ncc > 0) {                               // acc = C - A B^T: A negated; small terms first
+#pragma unroll
+      for (int k = 0; k < TG_KC / 8; ++k) {
+        const uint64_t dk = (uint64_t)(2 * k);
+        wgmma_tf32_n128_nega(acc0, a_lo + dk, b_hi + dk);
+        wgmma_tf32_n128_nega(acc1, a_lo + kHalf + dk, b_hi + dk);
+        wgmma_tf32_n128_nega(acc0, a_hi + dk, b_lo + dk);
+        wgmma_tf32_n128_nega(acc1, a_hi + kHalf + dk, b_lo + dk);
+        wgmma_tf32_n128_nega(acc0, a_hi + dk, b_hi + dk);
+        wgmma_tf32_n128_nega(acc1, a_hi + kHalf + dk, b_hi + dk);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < TG_KC / 8; ++k) {
+        const uint64_t dk = (uint64_t)(2 * k);
+        wgmma_tf32_n128(acc0, a_lo + dk, b_hi + dk);
+        wgmma_tf32_n128(acc1, a_lo + kHalf + dk, b_hi + dk);
+        wgmma_tf32_n128(acc0, a_hi + dk, b_lo + dk);
+        wgmma_tf32_n128(acc1, a_hi + kHalf + dk, b_lo + dk);
+        wgmma_tf32_n128(acc0, a_hi + dk, b_hi + dk);
+        wgmma_tf32_n128(acc1, a_hi + kHalf + dk, b_hi + dk);
+      }
     }
-  } else {
-    // ===== epilogue: one thread per tile row =====
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (warp == 0 && lane == 0) mbar_arrive(empty_bar + 8 * s);
+  }
+  fence_regs(acc0);
+  fence_regs(acc1);
+
+  // ===== epilogue =====
+  // the result tile goes to shared memory (stage 0, free now) as 128 rows of 128 floats, 16-byte chunk c of row r at
+  // chunk c ^ (r % 32); every thread then owns one tile row, as the row-major staging below expects
+  named_sync(1, 128);                                    // all MMAs of the warpgroup have read their operands
+  {
+    float* tilef = reinterpret_cast<float*>(gen_base);
+    const int fr = (warp & 3) * 16 + (lane >> 2);       // fragment row (+8, +64)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 4; ++h) {                      // (acc, +8 rows)
+        const int r = fr + 8 * (h & 1) + 64 * (h >> 1);
+        const float* a = (h >> 1) ? acc1 : acc0;
+        *reinterpret_cast<float2*>(tilef + (size_t)r * TG_N + 4 * ((col >> 2) ^ (r & 31)) + (col & 3)) =
+            make_float2(a[4 * j + 2 * (h & 1)], a[4 * j + 2 * (h & 1) + 1]);
+      }
+    }
+  }
+  named_sync(1, 128);
+  {
     const int q = warp & 3;
-    if (nkc > 0) {
-      mbar_wait(tmem_full_bar, 0);
-      fence_after();
-    }
     const int r_loc = q * 32 + lane;
     const int row = tile.x * TG_M + r_loc;               // output row (A row index)
     const int col0 = tile.y * TG_N;                      // first output column (B row index)
@@ -249,27 +195,27 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                                : nullptr;
     const double diag_add = (ep.diag_add != nullptr && tile.x == tile.y) ? ep.diag_add[ep.diag_mod > 0 ? mat % ep.diag_mod : mat] : 0.0;
     const bool diag_tile = tile.x == tile.y;
-    constexpr int EC = 16;                               // columns per epilogue pass (register budget of 3 CTAs / SM)
+    float* st = reinterpret_cast<float*>(gen_base) + (size_t)q * (32 * TG_N) + (size_t)lane * TG_N;   // this thread's row
+    constexpr int EC = 16;                               // columns per epilogue pass
 #pragma unroll 1
     for (int c = 0; c < TG_N / EC; ++c) {
-      uint32_t v[EC];
-      if (nkc > 0) {
-        tmem_ld_32x16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * EC), v);
-      } else {
+      float v[EC];
 #pragma unroll
-        for (int j = 0; j < EC; ++j) v[j] = 0u;
+      for (int j = 0; j < EC; j += 4) {
+        const float4 t4 = *reinterpret_cast<const float4*>(st + 4 * (((c * EC + j) >> 2) ^ lane));
+        v[j] = t4.x; v[j + 1] = t4.y; v[j + 2] = t4.z; v[j + 3] = t4.w;
       }
       float o[EC];
       if (cin) {
 #pragma unroll
         for (int j = 0; j < EC; j += 2) {
           const double2 cc = *reinterpret_cast<const double2*>(cin + c * EC + j);
-          o[j] = (float)(cc.x - (double)__uint_as_float(v[j]));
-          o[j + 1] = (float)(cc.y - (double)__uint_as_float(v[j + 1]));
+          o[j] = (float)(cc.x - (double)v[j]);
+          o[j + 1] = (float)(cc.y - (double)v[j + 1]);
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < EC; ++j) o[j] = ep.negate ? -__uint_as_float(v[j]) : __uint_as_float(v[j]);
+        for (int j = 0; j < EC; ++j) o[j] = ep.negate ? -v[j] : v[j];
       }
       if (diag_tile && diag_add != 0.0) {
 #pragma unroll
@@ -279,15 +225,12 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 #pragma unroll
         for (int j = 0; j < EC; ++j) if (c * EC + j > r_loc) o[j] = 0.f;
       }
-      // row-major outputs go through shared memory (below) so that a warp stores whole 512-byte rows; the transposed
-      // copies are already lane-coalesced (lanes hold consecutive rows) and leave from registers
-      {
-        float* st = reinterpret_cast<float*>(gen_base) + (size_t)q * (32 * TG_N) + (size_t)lane * TG_N;
+      // row-major outputs go back to the thread's own row of the staging tile (below, a warp stores whole 512-byte
+      // rows); the transposed copies are already lane-coalesced (lanes hold consecutive rows) and leave from registers
 #pragma unroll
-        for (int j = 0; j < EC; j += 4) {
-          const int chunk = (c * EC + j) >> 2;                              // 16-byte chunk of the row, XOR-swizzled by the row
-          *reinterpret_cast<float4*>(st + 4 * (chunk ^ lane)) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
-        }
+      for (int j = 0; j < EC; j += 4) {
+        const int chunk = (c * EC + j) >> 2;                                // 16-byte chunk of the row, XOR-swizzled by the row
+        *reinterpret_cast<float4*>(st + 4 * (chunk ^ lane)) = make_float4(o[j], o[j + 1], o[j + 2], o[j + 3]);
       }
       if (ep.out_t) {                                     // D^T as hi / lo planes: lanes of a warp hold consecutive rows
         float* th = ep.out_t + 2 * mat_off + (int64_t)(col0 + c * EC) * n + row;
@@ -330,13 +273,6 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         if (po) *reinterpret_cast<float4*>(po + (int64_t)rr * n) = v;
       }
     }
-  }
-  fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TG_TMEM_COLS)
-                 : "memory");
   }
 }
 
@@ -394,7 +330,7 @@ void launch_tf32x3_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const in
                         const Tf32GemmEpilogue& ep, cudaStream_t s, const CUtensorMap* tmC, const CUtensorMap* tmI) {
   RG_CHECK(ep.c_chunks == 0 || (tmC && tmI), "tf32 gemm: the C phase needs its tensor maps");
   if (ntiles <= 0 || batch <= 0) return;
-  // RG_B200_MX_STAGES = 1 (default: three co-resident CTAs hide the TMA latency) | 2 | 3 (one CTA per SM with a deeper ring)
+  // RG_B200_MX_STAGES = 1 (default: co-resident CTAs hide the TMA latency) | 2 | 3 (one CTA per SM with a deeper ring)
   static const int nst = [] { const char* e = getenv("RG_B200_MX_STAGES"); const int v = e ? atoi(e) : 1; return (v == 2 || v == 3) ? v : 1; }();
   const size_t smem = (size_t)nst * TG_STAGE_BYTES + 1024 + 128;
   dim3 grid(ntiles, batch);

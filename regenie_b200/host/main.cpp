@@ -1,5 +1,5 @@
 // rgb200 -- host driver keeping regenie's CLI surface for the Step-1 / Step-2 hot path and calling
-// the sm_100a kernels through the C ABI (include/rg_b200.h).
+// the sm_90a kernels through the C ABI (include/rg_b200.h).
 // Mirrors the control flow of the reference driver (restated, not copied):
 //   main / read_params_and_check   src/Regenie.cpp:60-142
 //   Data::run_step1                src/Data.cpp:95-133   (level_0_calculations :594, output :956,
@@ -251,7 +251,7 @@ Params parse_cli(int argc, char** argv) {
     else if (a == "--force-step1") p.force_step1 = true;
     else if (a == "--use-relative-path") p.rel_path = true;
     else if (a == "--help" || a == "-h") {
-      std::cout << "rgb200: B200-native regenie Step 1 / Step 2 hot path\n"
+      std::cout << "rgb200: H100-native regenie Step 1 / Step 2 hot path\n"
                    "  --step 1|2 --bed PREFIX | --pgen PREFIX | --bgen FILE --phenoFile F [--covarFile F] --bsize N --out PREFIX\n"
                    "  [--pred LIST] [--loocv] [--lowmem] [--cv K] [--l0 R] [--l1 R] [--remove F] [--keep F]\n"
                    "  [--exclude F] [--extract F] [--ref-first] [--minMAC x] [--strict] [--gpu ordinal]\n"

@@ -41,7 +41,7 @@ def test_l0_kfold_matches_oracle(tmp_path, N, M, bs, miss, P, K):
 
 
 def test_integer_gram_is_exact(tmp_path):
-    """tcgen05 e4m3 Gram == CUDA-core integer Gram == numpy integer Gram, bit for bit."""
+    """wgmma int8 Gram == CUDA-core integer Gram == numpy integer Gram, bit for bit."""
     pb = helpers.synthetic_problem(tmp_path, N=1500, M=256, bsize=256, miss=0.03)
     st = pb.gpu_step1()
     pb.gpu_l0_block(st, 0)

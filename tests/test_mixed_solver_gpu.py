@@ -1,4 +1,4 @@
-"""The mixed-precision ridge solver (csrc/chol_mixed.cu + csrc/tf32_gemm.cu): 3xTF32 tcgen05 factorisation / inverse +
+"""The mixed-precision ridge solver (csrc/chol_mixed.cu + csrc/tf32_gemm.cu): 3xTF32 wgmma factorisation / inverse +
 FP64 iterative refinement, against numpy's FP64 solve; its convergence flag; and the FP64 fallback of the level-0 path.
 
 What the reference computes here: beta = V (D + lambda I)^-1 V^T (GtY - GtY_f), src/Step1_Models.cpp:484-494."""

@@ -2,6 +2,8 @@
 exactly the genotypes of example/example.bed (both ship with the reference and hold the same 1000 x 500 calls), and a
 synthetic file written record type by record type (tests/helpers.write_pgen) must round-trip."""
 import collections
+import hashlib
+import os
 
 import numpy as np
 
@@ -65,45 +67,46 @@ def test_pgen_round_trip_all_record_types(tmp_path):
 
 
 # ------------------------------------------------------------------------------------ pinned on the reference's own pgenlib
-def _pgenlib():
-    import pytest
-    from oracle import pgenlib_ref
-    if not pgenlib_ref.available():
-        pytest.skip("oracle/_ref/libpgenlib_ref.so not built (needs /root/reference/external_libs/pgenlib)")
-    return pgenlib_ref
+# The reference's vendored pgenlib was run on these inputs when the digests under tests/golden/pgenlib/ were stored:
+# PgrValidate accepted every file, and ReadHardcalls (allele 1, missing = -3) returned int8 calls.  Stored: the SHA-256
+# of those calls and, for the synthetic files, of the .pgen bytes pgenlib validated and decoded.
+def _digest(a):
+    return hashlib.sha256(np.ascontiguousarray(np.asarray(a, dtype=np.int8)).tobytes()).hexdigest()
+
+
+def _pgenlib_digests(golden_dir, name):
+    path = os.path.join(os.path.dirname(golden_dir), "pgenlib", name)
+    return [line.split() for line in open(path).read().splitlines() if line.strip()]
 
 
 def test_oracle_equals_pgenlib_on_the_reference_fixture(golden_dir):
     """oracle/pgen.py vs the reference's vendored pgenlib, called as the reference calls it (ReadHardcalls, allele 1)."""
-    ref = _pgenlib()
-    path = golden_dir + "/example.pgen"
-    ref.validate(path)
-    want = ref.read_hardcalls(path, 500, 0, 1000)
-    pg = pgen.Pgen(path)
-    for v in range(1000):
-        g = pg.read(v).astype(float)
-        g[g == 3] = -3.0
-        assert np.array_equal(g, want[v]), v
+    [[want]] = _pgenlib_digests(golden_dir, "example_hardcalls.sha256")
+    pg = pgen.Pgen(golden_dir + "/example.pgen")
+    got = np.stack([pg.read(v) for v in range(1000)]).astype(np.int8)
+    got[got == 3] = -3
+    assert _digest(got) == want
 
 
-def test_synthetic_files_pass_pgenlib_validation_and_read_back(tmp_path):
+def test_synthetic_files_pass_pgenlib_validation_and_read_back(tmp_path, golden_dir):
     """The test writer (helpers.write_pgen) is itself checked by the reference library: PgrValidate accepts the files
     (record types, difflist group byte counts, trailing bits) and ReadHardcalls returns the calls that were written - with
     all samples and with a sample subset (pgenlib's proper-subset readers skip difflist groups by their byte counts) - and
     oracle/pgen.py agrees.  Covers difflists of > 32 groups and 1 / 2 / 3-byte sample ids, which the fixture does not."""
-    ref = _pgenlib()
     from test_host_cpu import big_pgen_calls
+    digests = {int(n): (full, part, file) for n, full, part, file in _pgenlib_digests(golden_dir, "synthetic_hardcalls.sha256")}
     for N, M, storage in ((700, 160, 5), (33333, 40, 6), (70001, 20, 2)):
         g = synthetic_calls() if N == 700 else big_pgen_calls(N, M)
         pfx = str(tmp_path / ("s%d" % N))
         types = helpers.write_pgen(pfx, g, storage=storage)
         assert set(types) >= set(range(8))
-        ref.validate(pfx + ".pgen")
-        want = g.astype(float)
-        want[want == 3] = -3.0
-        assert np.array_equal(ref.read_hardcalls(pfx + ".pgen", g.shape[1], 0, g.shape[0]), want)
+        # the writer reproduces, byte for byte, the files pgenlib validated and read back
+        assert hashlib.sha256(open(pfx + ".pgen", "rb").read()).hexdigest() == digests[N][2], N
+        want = g.astype(np.int8)
+        want[want == 3] = -3
         sub = np.sort(np.random.default_rng(N).choice(g.shape[1], g.shape[1] // 3, replace=False))
-        assert np.array_equal(ref.read_hardcalls(pfx + ".pgen", g.shape[1], 0, g.shape[0], subset=sub), want[:, sub])
+        assert _digest(want) == digests[N][0]
+        assert _digest(want[:, sub]) == digests[N][1]
         pg = pgen.Pgen(pfx + ".pgen")
         for v in (list(range(g.shape[0])) + [g.shape[0] - 1, 3, 1]):
             assert np.array_equal(pg.read(v), g[v]), (N, v)

@@ -8,7 +8,7 @@ import json,sys
 t=sys.stdin.read().strip().splitlines()
 if t:
     j=json.loads(t[-1]); k=j.get('kernels',{})
-    print('%-28s ms/step %6.2f  (%.0f SNPs/s, e2e %.0f)  single-lane ms/50 blocks: predict %.1f mx %.1f gram %.1f stats %.1f' % ('$label', j['ms_per_step'], j['value'], j.get('e2e',{}).get('value',0), k.get('l0_predict',{}).get('ms_total',0), k.get('mx_solve',{}).get('ms_total',0), k.get('gram_tcgen05',{}).get('ms_total',0), k.get('l0_stats',{}).get('ms_total',0)))
+    print('%-28s ms/step %6.2f  (%.0f SNPs/s, e2e %.0f)  single-lane ms/50 blocks: predict %.1f mx %.1f gram %.1f stats %.1f' % ('$label', j['ms_per_step'], j['value'], j.get('e2e',{}).get('value',0), k.get('l0_predict',{}).get('ms_total',0), k.get('mx_solve',{}).get('ms_total',0), k.get('gram_wgmma',{}).get('ms_total',0), k.get('l0_stats',{}).get('ms_total',0)))
 else:
     print('%-28s failed: ' % '$label', open('gpurun_out/ab_err.txt').read()[-300:])"
 done

@@ -30,7 +30,7 @@ def main():
         zr = st.debug("zz_ref", np.float32, K * 4 * rp * rp).reshape(K, 2 * rp, 2 * rp)
         tri = np.tril(np.ones((2 * rp, 2 * rp), dtype=bool))
         d = np.abs(zz - zr)[:, tri]
-        print("  gram tcgen05 vs cuda-core ref: max abs diff", d.max(), " ref max", zr.max(), " nonzero frac", (zz[:, tri] != 0).mean())
+        print("  gram wgmma vs cuda-core ref: max abs diff", d.max(), " ref max", zr.max(), " nonzero frac", (zz[:, tri] != 0).mean())
         if d.max() != 0:
             bad = np.argwhere(np.abs(zz - zr) * tri[None] > 0)
             print("  first bad entries", bad[:10], "count", len(bad))
@@ -62,7 +62,7 @@ def main():
         for ph in range(pr.Y.shape[1]):
             W = st.fetch_W(b, ph)
             print("  W ph", ph, "rel", rel(W, W_o[ph]))
-    for k in ["h2d", "bed_relayout", "bed_expand", "l0_stats", "gram_tcgen05", "l0_assemble", "chol_factor",
+    for k in ["h2d", "bed_relayout", "bed_expand", "l0_stats", "gram_wgmma", "l0_assemble", "chol_factor",
               "chol_backsolve", "l0_predict"]:
         ms, n = st.timing(k)
         print("  time %-16s %8.3f ms over %d" % (k, ms, n))

@@ -1,6 +1,6 @@
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list: per-kernel time of the LAST level-0 block
 (single lane), plus the launch sequence of the solver kernels.  ncu serialises launches and runs them cold-cache, so the
-SHARES are meaningful, not the absolutes (B200_PROFILING.md)."""
+SHARES are meaningful, not the absolutes."""
 import collections
 import csv
 import sys

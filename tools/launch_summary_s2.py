@@ -1,6 +1,6 @@
 """Summarise the `ncu --metrics gpu__time_duration.sum --csv` launch list of tools/step2_probe.py: the kernels of the last
 quantitative-trait block on .bed rows and of the last binary-trait block on 8-bit dosages (us, launches, share).  ncu
-serialises launches and runs them cold-cache: the SHARES are meaningful, not the absolutes (B200_PROFILING.md)."""
+serialises launches and runs them cold-cache: the SHARES are meaningful, not the absolutes."""
 import collections
 import csv
 import sys

@@ -1,5 +1,5 @@
 """Numerical study for DESIGN.md section 8 (1): can the level-0 ridge systems (A_-f + lambda_j I) beta = b be factorised in
-reduced precision on the tcgen05 pipe and polished by FP64 iterative refinement?
+reduced precision on the tensor cores and polished by FP64 iterative refinement?
 
 Synthetic block as bench.py builds it (MAF ~ U(0.01, 0.5), 1 % missing, mean-imputed, residualised on C = 3 covariates,
 unit variance), N samples, bs SNPs, K = 5 folds, the reference's lambda grid M (1 - h) / h, h in {0.01, .25, .5, .75, .99}.
