@@ -688,11 +688,13 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
   ensure_dyn_smem(reinterpret_cast<const void*>(mx_residual_kernel<12>), 98304);
   ensure_dyn_smem(reinterpret_cast<const void*>(mx_residual_kernel<10>), 98304);
   static const bool res_fused = [] { const char* e = getenv("RG_B200_MX_RES"); return !(e && strcmp(e, "plain") == 0); }();
-  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<12, 8>), 220 * 1024);
-  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<10, 8>), 220 * 1024);
-  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<12, 16>), 220 * 1024);
-  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<10, 16>), 220 * 1024);
   RG_CHECK(n <= 2048, "mixed solver: n <= 2048");
+  // substitution sweeps: the stage ring, the solution vector of all n rows and the slice partial sums.  At n = 2048 with
+  // 16 consumer warps that is 222 KiB, close to the 227 KiB a block may opt into, so the limit is set from the same formula
+  static const int tri_warps = [] { const char* e = getenv("RG_B200_MX_TRI_WARPS"); return (e && atoi(e) == 8) ? 8 : 16; }();
+  const size_t sm_t = (size_t)TS_STAGES * TS_STAGE_BYTES + ((size_t)n + (1 + tri_warps / 4) * PT) * TS_VP * sizeof(float) + 2 * TS_STAGES * 8 + 256;
+  ensure_dyn_smem(reinterpret_cast<const void*>(tri_warps == 8 ? mx_trisolve_kernel<12, 8> : mx_trisolve_kernel<12, 16>), sm_t);
+  ensure_dyn_smem(reinterpret_cast<const void*>(tri_warps == 8 ? mx_trisolve_kernel<10, 8> : mx_trisolve_kernel<10, 16>), sm_t);
   // profiling aid (results are garbage): RG_DBG_SKIP=mxgemm|mxpotrf|mxtri|mxres drops one kernel family of the solver so
   // its marginal cost under multi-lane overlap can be read off
   static const char* skip_env = getenv("RG_DBG_SKIP");
@@ -730,8 +732,6 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
     for (int p0 = 0; p0 < P; p0 += pc) {
       const int np = std::min(pc, P - p0);
       const size_t sm_r = (size_t)np * n * sizeof(double);
-      static const int tri_warps = [] { const char* e = getenv("RG_B200_MX_TRI_WARPS"); return (e && atoi(e) == 8) ? 8 : 16; }();
-      const size_t sm_t = (size_t)TS_STAGES * TS_STAGE_BYTES + ((size_t)n + (1 + tri_warps / 4) * PT) * TS_VP * sizeof(float) + 2 * TS_STAGES * 8 + 256;
       const int64_t o = (int64_t)p0 * n;
       // right-hand-side count is a template parameter (register blocking): 10 is the benchmark's trait count
       auto tri = [&](const double* rv, int64_t rs, int rdiv, int step) {

@@ -91,6 +91,9 @@ struct rg_ctx {
     cudaEvent_t mx_ev = nullptr;
     bool mx_pending = false;                      // a block went through the mixed path and its flag has not been read yet
     int mx_bs = 0, mx_block_id = 0;               // the block to re-solve in FP64 if the flag is set
+    // kernels that produced this lane's last block (rg_debug_fetch "paths"): INT8 (1) or FP64 (0) prediction; the
+    // mixed solver's dimension, or 0 when the FP64 Cholesky solved it
+    int last_pred_i8 = 0, last_mx_n = 0;
   };
   std::vector<std::unique_ptr<Lane>> lanes;
   int next_lane = 0, last_lane = 0;

@@ -6,7 +6,8 @@
 // (bed_expand_fp8_kernel).  The real-valued coefficients are split into FIVE balanced radix-254 digits
 //   gamma[i,q] = (s_q / 127) * sum_l d_l[i,q] 254^-l,   d_l in {-127..127}  (int8),
 // so the s8 x s8 -> s32 MMAs accumulate exact integer sums (|sum| <= K2 * 16 * 127 < 2^24 for K2 <= 4096) and the FP64
-// epilogue reassembles the prediction to 254^-5 / 2 = 4.7e-13 s_q per coefficient, far inside the 1e-5 parity budget.
+// epilogue reassembles the prediction to s_q 254^-5 = 9.4e-13 s_q per coefficient (the last limb is rounded to within 1/2,
+// and one unit of it is worth (s_q / 127) 254^-4), far inside the 1e-5 parity budget.
 //
 // Orientation: samples are the MMA M dimension, the 5 x 50 digit rows are N (256, zero padded), the SNP/plane index
 // is K.  The digit rows are K-major in shared memory (wgmma B operand).  The genotype tile arrives samples-contiguous

@@ -130,18 +130,35 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
       maskp[(size_t)p * h->Npad + t] = mask[(size_t)p * N + s] ? 1 : 0;
     }
   }
-  // per-fold X_f^T X_f and X_f^T Y_f (Appendix B item 6 of SURVEY.md)
+  // per-fold X_f^T X_f and X_f^T Y_f (Appendix B item 6 of SURVEY.md), summed with Neumaier compensation: the level-0
+  // Gram subtracts B (X_f^T X_f) B^T from G_f G_f^T, and for a variant whose mean is large against its spread (the
+  // counted allele nearly fixed) the two agree to 1 part in 10^3 or more, so the ~n u error of a plain running sum over
+  // a fold of 10^5 .. 10^6 samples would show in the predictors
   std::vector<double> XtX((size_t)K * C * C, 0.0), XtY((size_t)K * C * P, 0.0);
   {
+    std::vector<double> cXtX(XtX.size(), 0.0), cXtY(XtY.size(), 0.0);
+    auto add = [](double& sum, double& comp, double v) {
+      const double t = sum + v;
+      comp += (std::fabs(sum) >= std::fabs(v)) ? (sum - t) + v : (v - t) + sum;
+      sum = t;
+    };
     int64_t s = 0;
     for (int f = 0; f < K; ++f)
       for (int64_t o = 0; o < h->fold_sizes[f]; ++o, ++s)
         for (int c = 0; c < C; ++c) {
           const double xc = X[(size_t)c * N + s];
           if (xc == 0.0) continue;
-          for (int c2 = 0; c2 < C; ++c2) XtX[((size_t)f * C + c) * C + c2] += xc * X[(size_t)c2 * N + s];
-          for (int p = 0; p < P; ++p) XtY[((size_t)f * C + c) * P + p] += xc * Y[(size_t)p * N + s];
+          for (int c2 = 0; c2 < C; ++c2) {
+            const size_t e = ((size_t)f * C + c) * C + c2;
+            add(XtX[e], cXtX[e], xc * X[(size_t)c2 * N + s]);
+          }
+          for (int p = 0; p < P; ++p) {
+            const size_t e = ((size_t)f * C + c) * P + p;
+            add(XtY[e], cXtY[e], xc * Y[(size_t)p * N + s]);
+          }
         }
+    for (size_t e = 0; e < XtX.size(); ++e) XtX[e] += cXtX[e];
+    for (size_t e = 0; e < XtY.size(); ++e) XtY[e] += cXtY[e];
   }
   // chunk table for the f64 reductions
   std::vector<int4> chunks;
@@ -315,17 +332,21 @@ static void enqueue_solve_f64(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cu
 static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, int n, cudaStream_t s) {
   const int C = h->C, P = h->P, K = h->K, R = h->R;
   const int Pp = mx_pp(P);
-  const int n_max = MixedSolver::dim_for(h->bs_max);
   if (!L.mx) {
     L.mx = std::make_unique<MixedSolver>();
     L.mx_fail.alloc(1);
     RG_CUDA(cudaMallocHost(&L.mx_fail_host, sizeof(unsigned int)));
     RG_CUDA(cudaEventCreateWithFlags(&L.mx_ev, cudaEventDisableTiming));
-    L.mx_Af.alloc((size_t)K * n_max * n_max);
-    L.mx_b.alloc((size_t)K * Pp * n_max);
-    L.mx_x.alloc((size_t)K * R * Pp * n_max);
-    L.mx_r.alloc((size_t)K * R * Pp * n_max);
   }
+  // sized from the block being solved: with bsize > 2048 the largest blocks take the FP64 path, but a chromosome's short
+  // last block still comes here (alloc is a no-op once the buffers are large enough)
+  const size_t need_A = (size_t)K * n * n, need_b = (size_t)K * Pp * n, need_x = (size_t)K * R * Pp * n;
+  L.mx_Af.alloc(need_A);
+  L.mx_b.alloc(need_b);
+  L.mx_x.alloc(need_x);
+  L.mx_r.alloc(need_x);
+  RG_CHECK(L.mx_Af.n >= need_A && L.mx_b.n >= need_b && L.mx_x.n >= need_x && L.mx_r.n >= need_x,
+           "mixed solver: scratch smaller than the block's systems");
   L.mx->prepare(n, K, R, Pp);
   RG_CUDA(cudaMemsetAsync(L.mx_fail.p, 0, sizeof(unsigned int), s));
   AssembleArgs aa;
@@ -376,6 +397,7 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
   static const std::string predict_kind = [] { const char* e = getenv("RG_B200_PREDICT"); return std::string(e ? e : "i8"); }();
   RG_CHECK(predict_kind == "i8" || predict_kind == "f64", "RG_B200_PREDICT must be i8 or f64");
   const bool use_i8 = predict_kind == "i8" && 2 * d.rows_p <= 4096;
+  L.last_pred_i8 = use_i8 ? 1 : 0;
   if (!use_i8) {
     launch_l0_predict(pa, d.ntiles_s, s);
   } else {
@@ -429,6 +451,7 @@ void resolve_lane(rg_ctx* h, rg_ctx::Lane& L) {
   L.mx_pending = false;
   if (*L.mx_fail_host == 0) return;
   h->mx_fallbacks += 1;
+  L.last_mx_n = 0;
   const BlockDims d = block_dims(h, L.mx_bs, L.mx_block_id);
   enqueue_solve_f64(h, L, d, L.stream);
   enqueue_predict(h, L, d, L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.nC, L.stream);
@@ -631,6 +654,7 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
 
   // --- 4./5. ridge systems -> coefficients -> out-of-fold predictions, standardised into W
   const int mx_n = (!h->loocv && h->solver_mixed) ? MixedSolver::dim_for(bs) : 0;
+  L.last_mx_n = mx_n;
   if (mx_n > 0) {
     enqueue_solve_mixed(h, L, d, mx_n, s);
     enqueue_predict(h, L, d, L.mx_x.p, (int64_t)mx_pp(P) * mx_n, mx_n, 0, s);
@@ -669,6 +693,7 @@ static void l0_block_dense(rg_ctx* h, const uint8_t* probs, const uint8_t* miss,
   cudaStream_t s = L.stream;
   const BlockDims d = block_dims(h, bs, block_id);
   h->last_bs = bs; h->last_rows_p = d.rows_p; h->last_nC = d.nC; h->last_n_aug = d.n_aug; h->last_nmat = d.nmat;
+  L.last_pred_i8 = 0; L.last_mx_n = 0;     // dense FP64 prediction and Cholesky
 
   L.gd.alloc((size_t)h->bs_max * Npad);
   L.mu.alloc(h->rows_p_max);
@@ -1102,6 +1127,21 @@ int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_byt
   else if (n == "rhs") { p = L.rhs.p; bytes = (size_t)h->K * rp * h->P * 8; }
   else if (n == "cm") { p = L.cm.p; bytes = (size_t)h->last_nmat * h->last_n_aug * h->last_nC * 8; }
   else if (n == "mean_invsd") { p = L.mean_invsd.p; bytes = (size_t)2 * h->R * h->P * 8; }
+  else if (n == "wraw") { p = L.wraw.p; bytes = (size_t)h->P * h->R * h->Npad * 8; }
+  else if (n == "gam" || n == "gmu" || n == "cvec") {
+    const size_t Kg = h->loocv ? 1 : h->K, Qp = (size_t)round_up(h->R * h->P, predict_qt());
+    p = (n == "gam" ? L.gam : n == "gmu" ? L.gmu : L.cvec).p;
+    bytes = (n == "cvec" ? Kg * Qp * h->C : Kg * rp * Qp) * 8;
+  }
+  else if (n == "cnt_fold") { p = L.cnt_fold.p; bytes = (size_t)h->K * rp * 4 * 4; }
+  else if (n == "sum_fold") { p = L.sum_fold.p; bytes = (size_t)h->K * rp * 2 * h->cpp * 8; }
+  else if (n == "paths") {
+    // which kernels produced the last block: statistics on the tensor cores, INT8 prediction, mixed-solver dimension
+    const int64_t v[3] = {h->stats_tc ? 1 : 0, L.last_pred_i8, L.last_mx_n};
+    if (max_bytes < (int64_t)sizeof(v)) return -1;
+    memcpy(out, v, sizeof(v));
+    return sizeof(v);
+  }
   else if (n == "dbg_clk") {
     if (!h->dbg_clk.p) return -1;
     bytes = std::min<size_t>(h->dbg_clk.n * 8, (size_t)max_bytes);
@@ -1139,6 +1179,7 @@ int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_byt
     rg::set_last_error("unknown debug buffer: " + n);
     return -1;
   }
+  if (!p) { rg::set_last_error("debug buffer not allocated: " + n); return -1; }
   if ((int64_t)bytes > max_bytes) return -1;
   if (cudaMemcpy(out, p, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
   return (int64_t)bytes;
@@ -1193,7 +1234,8 @@ int rg_dbg_mixed_solve(int32_t device, int32_t n, int32_t K, int32_t R, int32_t 
   cudaStream_t st;
   RG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   mx.solve(dA.p, dl.p, db.p, dx.p, dr.p, P, steps, (float)tol, dfail.p, st);
-  cudaError_t e = cudaStreamSynchronize(st);
+  cudaError_t e = cudaGetLastError();                        // a launch the device refused (shared memory, grid)
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   cudaStreamDestroy(st);
   RG_CHECK(e == cudaSuccess, std::string("mixed solver kernels failed: ") + cudaGetErrorString(e));
   for (int m = 0; m < nmat; ++m)

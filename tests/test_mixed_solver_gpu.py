@@ -28,7 +28,8 @@ def _systems(n, K, P, seed, cond=50.0, n_real=None):
     return Af, b
 
 
-@pytest.mark.parametrize("n,K,R,P,n_real", [(128, 2, 2, 3, 100), (256, 2, 3, 2, 256), (512, 1, 2, 10, 450), (1024, 2, 2, 10, 1000)])
+@pytest.mark.parametrize("n,K,R,P,n_real", [(128, 2, 2, 3, 100), (256, 2, 3, 2, 256), (512, 1, 2, 10, 450), (1024, 2, 2, 10, 1000),
+                                             (2048, 1, 2, 3, 1900)])   # the largest dimension (bsize 1025 .. 2048)
 def test_mixed_solve_matches_numpy(n, K, R, P, n_real):
     from regenie_b200 import capi
     Af, b = _systems(n, K, P, seed=n + K, n_real=n_real)
