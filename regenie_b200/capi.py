@@ -473,6 +473,10 @@ class Step2:
         check(L.rg_s2_spa(self.h, len(vi), _ptr(vi), _ptr(ti), _ptr(pv), _ptr(status)))
         return pv, status
 
+    def debug(self, name, dtype, count):
+        """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block."""
+        return debug_fetch(self, name, dtype, count)
+
     def firth(self, variant_idx, trait_idx):
         L = lib()
         L.rg_s2_firth.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 6

@@ -148,6 +148,7 @@ struct rg_ctx {
   // quantitative-trait statistics on the tensor cores (bed / pgen input)
   bool s2_tc = false;
   int s2_drows = 0, s2_nchunk = 0, s2_ncol = 0;
+  int64_t s2_chunk_len = 0;                   // samples per tensor-core chunk (the last one may be shorter)
   rg::DevBuf<uint8_t> s2_z3, s2_FD;           // [3 rows_p][Npad] planes; digit rows of F
   rg::DevBuf<double> s2_Fscale;
   rg::DevBuf<float> s2_T;                     // [chunk][3 rows_p][drows]
@@ -168,6 +169,8 @@ struct rg_ctx {
   int s2_fcols = 0;                           // the same for the quantitative-trait feature rows (dp)
   bool bt_chr_set = false;
   int s2_last_bs = 0;                // variants resident in dz (for rg_s2_firth)
+  // shape of the sums the last block left (rg_debug_fetch "s2_sums" / "bt_sums"): padded rows, and the row width of bt_sums
+  int s2_sums_rows = 0, bt_sums_rows = 0, bt_sums_dp = 0;
   // rg_s2_stage: input bytes of the NEXT block travel on a copy stream while the current block computes
   static constexpr int kStageSlots = 4;
   rg::DevBuf<uint8_t> s2_stage[kStageSlots];

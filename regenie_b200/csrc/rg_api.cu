@@ -1112,6 +1112,25 @@ int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_byt
     if (cudaMemcpy(out, r.p, nb, cudaMemcpyDeviceToHost) != cudaSuccess) { rg::set_last_error("copy failed"); return -1; }
     return (int64_t)nb;
   }
+  if (h->kind == 2) {                  // test-only: how Step 2 computed its last block, and the sums it came from
+    const void* p = nullptr;
+    size_t bytes = 0;
+    if (n == "s2_paths") {
+      const int64_t v[8] = {h->s2_tc ? 1 : 0, h->s2_nchunk, h->s2_chunk_len, h->s2_drows, h->nchunks, h->Npad, h->dp, h->bt_dp};
+      if (max_bytes < (int64_t)sizeof(v)) { rg::set_last_error("buffer too small: " + n); return -1; }
+      memcpy(out, v, sizeof(v));
+      return sizeof(v);
+    }
+    if (n == "s2_sums") { p = h->s2_sums.p; bytes = (size_t)h->s2_sums_rows * 3 * h->dp * 8; }              // [rows_p][3][dp]
+    else if (n == "bt_sums") { p = h->bt_sums.p; bytes = (size_t)h->bt_sums_rows * 4 * h->bt_sums_dp * 8; }  // [rows_p][4][dp]
+    else if (n == "bt_nnz") { p = h->bt_nnz.p; bytes = (size_t)h->bt_sums_rows * 8; }
+    else if (n == "bt_n510") { p = h->bt_n510.p; bytes = (size_t)h->bt_sums_rows * 8; }
+    else { rg::set_last_error("unknown Step-2 debug buffer: " + n); return -1; }
+    if (!p || bytes == 0) { rg::set_last_error("no Step-2 block has filled " + n); return -1; }
+    if ((int64_t)bytes > max_bytes) { rg::set_last_error("buffer too small: " + n); return -1; }
+    if (cudaMemcpy(out, p, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) { rg::set_last_error("copy failed"); return -1; }
+    return (int64_t)bytes;
+  }
   if (h->lanes.empty()) { rg::set_last_error("no level-0 lane"); return -1; }
   rg_ctx::Lane& L = *h->lanes[h->last_lane];
   const void* p = nullptr;

@@ -74,9 +74,13 @@ static void s2_create(rg_ctx* h, const rg_step2_config* cfg, const double* X, co
 
 // tensor-core statistics for 2-bit input: digit rows of the chromosome's feature matrix (exact, see s2_kernels.cu)
 static void s2_build_digits(rg_ctx* h, const double* Fdev, int dp, int D) {
-  static const bool f64_only = [] { const char* e = getenv("RG_B200_S2_STATS"); return e && std::string(e) == "f64"; }();
-  h->s2_tc = !f64_only;
-  if (!h->s2_tc) return;
+  // read on every call (once per chromosome), like RG_B200_STATS at level 0, so each handle follows the current setting
+  const char* e = getenv("RG_B200_S2_STATS");
+  h->s2_tc = !(e && std::string(e) == "f64");
+  if (!h->s2_tc) {
+    h->s2_nchunk = 0; h->s2_chunk_len = 0; h->s2_drows = 0;
+    return;
+  }
   cudaStream_t s = h->stream;
   h->s2_ncol = D;
   h->s2_drows = (int)round_up((int64_t)ceil_div(D, kStatQ) * 128, 256);
@@ -98,6 +102,7 @@ static void s2_build_digits(rg_ctx* h, const double* Fdev, int dp, int D) {
   for (int64_t o = 0; o < h->Npad; o += len)
     fk.push_back(make_int2((int)(o / 128), (int)(std::min<int64_t>(len, h->Npad - o) / 128)));
   h->s2_nchunk = (int)fk.size();
+  h->s2_chunk_len = len;
   h->s2_fold_k.alloc(fk.size());
   RG_CUDA(cudaMemcpyAsync(h->s2_fold_k.p, fk.data(), fk.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
 }
@@ -284,6 +289,7 @@ static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
   launch_s2_finalize(a, s);
   h->launches += 4;
+  h->s2_sums_rows = rows_p;
   s2_copy_out(h, bs, out, nullptr, nullptr, s);
 }
 
@@ -408,6 +414,7 @@ static void s2_block_bgen8_bt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
   launch_s2_bt_finalize(a, s);
   h->launches += 5;
   h->s2_last_bs = bs;
+  h->bt_sums_rows = rows_p; h->bt_sums_dp = dp;
   s2_copy_out(h, bs, out, info_out, a.info, s);
 }
 
@@ -477,6 +484,8 @@ static void s2_block_bgen8_qt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
   a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
   launch_s2_finalize(a, s);
   h->launches += 6;
+  h->s2_sums_rows = rows_p;
+  h->bt_sums_rows = rows_p; h->bt_sums_dp = dp;
   s2_copy_out(h, bs, out, info_out, a.info, s);
 }
 
@@ -541,6 +550,7 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   launch_s2_bt_finalize(a, s);
   h->launches += 7;
   h->s2_last_bs = bs;
+  h->bt_sums_rows = rows_p; h->bt_sums_dp = dp;
   s2_copy_out(h, bs, out, nullptr, nullptr, s);
 }
 
