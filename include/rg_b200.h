@@ -407,8 +407,8 @@ int rg_W_info(rg_handle h, int32_t ph, void** dev_ptr, int64_t* ld, int64_t* nco
 int rg_W_attach_local(rg_handle h, rg_handle peer, const uint8_t* owned_by_peer);
 
 /* ------------------------------------------------------------------ test / profiling hooks */
-/* Copy a named intermediate of the last level-0 block, or of the last Step-2 block on a Step-2 handle, to the host
- * (tests only).  Returns the number of bytes written, or <0 on error.  See DESIGN.md for names. */
+/* Copy a named intermediate of the last level-0 block or level-1 fit ("l1_*"), or of the last Step-2 block on a Step-2
+ * handle, to the host (tests only).  Returns the number of bytes written, or <0 on error.  See DESIGN.md for names. */
 int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_bytes);
 /* Level-0 ridge solver bookkeeping: blocks whose K*R systems were solved by the tensor-core factorisation + FP64
  * iterative refinement (csrc/chol_mixed.cu), and how many of those raised the convergence flag and were re-solved

@@ -252,11 +252,10 @@ class Step1:
         return out
 
     def debug(self, name, dtype, count):
-        out = np.empty(count, dtype=dtype)
-        n = lib().rg_debug_fetch(self.h, name.encode(), _ptr(out), out.nbytes)
-        if n < 0:
-            raise RgError("debug fetch failed for %s: %s" % (name, lib().rg_last_error().decode()))
-        return out[: n // out.itemsize]
+        """rg_debug_fetch: level-0 intermediates of the last block, or of the last level-1 fit: "l1_dims" (int64 x 8:
+        B, nC, R1, K, systems, rows per system, chunks, chunk length), "l1_chunks" (int32 x 4 per chunk), "l1_beta"
+        ([P][K R1][nC], k-fold), "l1_sums" ([P][3 kMaxRidge + 2]), "l1_bvec" ([P][nC]) and "l1_hvec" ([P][Npad]) (LOOCV)."""
+        return debug_fetch(self, name, dtype, count)
 
     def launch_count(self):
         return lib().rg_launch_count(self.h)

@@ -124,6 +124,8 @@ struct rg_ctx {
   std::vector<int32_t> best_idx;
   std::vector<double> prs_host;                      // [P][N] whole-genome predictions kept by rg_loco for rg_prs
   int l1_nC = 0;
+  int l1_nmat = 0, l1_n_aug = 0;                     // systems and rows per system of the last fit (rg_debug_fetch "l1_dims")
+  int64_t l1_chunk_len = 0;                          // sample chunk length of the last fit's chunk table
   bool l1_done = false;
   rg::DevBuf<double*> W_tab;                         // [P] where each phenotype's W lives (local or peer HBM)
   std::vector<double*> W_host_tab;

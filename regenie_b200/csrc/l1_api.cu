@@ -28,11 +28,13 @@ static void l1_setup_chunks(rg_ctx* h, int nC, int ldp) {
   cudaStream_t s = h->stream;
   const int K = h->K;
   const int64_t Npad = h->Npad;
-  // chunk table for the sample-axis reductions: bounded partial storage (<= ~1 GiB)
+  // chunk table for the sample-axis reductions: bounded partial storage (<= ~1 GiB).  A fold of n samples takes
+  // ceil(n / len) chunks <= n / len + 1, so the K folds take at most max_chunks chunks of nC x ldp partials.
   {
     const int64_t per = (int64_t)nC * ldp * 8;
     const int64_t max_chunks = std::max<int64_t>(K, (1ll << 30) / per);
     int64_t len = round_up(std::max<int64_t>(kStatChunk, ceil_div(Npad, max_chunks - K + 1)), 128);
+    h->l1_chunk_len = len;
     std::vector<int4> chunks;
     std::vector<int2> fold_chunks(K);
     for (int f = 0; f < K; ++f) {
@@ -53,6 +55,7 @@ static void l1_setup_chunks(rg_ctx* h, int nC, int ldp) {
 
 static void l1_fit(rg_ctx* h, const double* tau_host, double* cumsum, int32_t* best_idx) {
   RG_CHECK(h->kind == 1, "handle is not a Step-1 handle");
+  h->l1_done = false;                                     // until this fit completes, rg_loco and the hooks refuse
   RG_CHECK(h->R1 >= 1 && h->R1 <= kMaxRidge, "n_ridge_l1 out of range");
   RG_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
@@ -65,6 +68,9 @@ static void l1_fit(rg_ctx* h, const double* tau_host, double* cumsum, int32_t* b
   const int ldp = nC;
   const int64_t Npad = h->Npad;
   h->l1_nC = nC;
+  h->l1_nmat = nmat;
+  h->l1_n_aug = n_aug;
+  h->l1_bt = false;                                       // rg_loco takes the QT route after this fit
   l1_setup_chunks(h, nC, ldp);
   const int nch = h->l1_nchunks;
   const int64_t part_stride = (int64_t)nC * ldp;
@@ -356,6 +362,7 @@ static void l1_fit_bt_kfold_pheno(rg_ctx* h, LgState& st, int p, const std::vect
 static void l1_fit_bt(rg_ctx* h, const double* y_raw, const double* offset, const double* tau_host, double* cumsum,
                       int32_t* best_idx) {
   RG_CHECK(h->kind == 1, "handle is not a Step-1 handle");
+  h->l1_done = false;                                     // as in l1_fit: a fit that fails leaves no fit behind
   RG_CHECK(h->R1 >= 1 && h->R1 <= kMaxRidge, "n_ridge_l1 out of range");
   RG_CHECK(h->B <= 6000, "logistic level 1 supports up to 6000 level-0 predictors (blocks x ridge values) in this build");
   RG_CUDA(cudaSetDevice(h->device));
@@ -370,6 +377,8 @@ static void l1_fit_bt(rg_ctx* h, const double* y_raw, const double* offset, cons
   const int nch = h->l1_nchunks;
   const int loocv = h->loocv;
   const int64_t cm_stride = (int64_t)(nC + 64 + (loocv ? Npad : 0)) * nC;
+  h->l1_nmat = 1;                                         // one system, refactored at every Newton step
+  h->l1_n_aug = (int)(cm_stride / nC);
   {
     const int2 all = make_int2(0, nch);
     h->lg_all_chunks.alloc(1);

@@ -11,13 +11,14 @@
 namespace rg {
 
 // rows nrow0 + t of every system r:  g~_t = (g_imp(:, t) - Bv x_t) * inv_sd   (level 0)
-// grid: (ceil(nC/128), Npad), block 128: thread = SNP i.
+// grid: (Npad, ceil(nC/128)), block 128: thread = SNP i.  The sample axis is grid.x (limit 2^31 - 1): on grid.y it
+// would cap LOOCV at 65 535 padded samples.
 __global__ void l0_loocv_fill_kernel(const uint32_t* __restrict__ gp, int64_t words_per_row, int bs, int nC,
                                      const double* __restrict__ mu, const double* __restrict__ inv_sd,
                                      const double* __restrict__ Bv, int C, const double* __restrict__ xy, int cpp,
                                      double* __restrict__ cm, int64_t cm_stride, int nrow0, int R) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int t = blockIdx.y;
+  const int i = blockIdx.y * blockDim.x + threadIdx.x;
+  const int t = blockIdx.x;
   if (i >= nC) return;
   double v = 0.0;
   if (i < bs) {
@@ -107,11 +108,11 @@ __global__ void l0_loocv_std_apply_kernel(double* const* __restrict__ W, int64_t
 
 // ---------------------------------------------------------------------------------------- level 1
 // sample rows of the R1 systems:  row (nrow0 + t) = W[t, 0:B]   (tile transpose, coalesced both ways)
-// grid: (ceil(nC/32), Npad/32), block (32, 8)
+// grid: (Npad/32, ceil(nC/32)), block (32, 8); the sample axis is grid.x, like l0_loocv_fill_kernel
 __global__ void l1_loocv_fill_kernel(const double* __restrict__ W, int64_t ldw, int B, int nC,
                                      double* __restrict__ cm, int64_t cm_stride, int nrow0, int R1) {
   __shared__ double tile[32][33];
-  const int c0 = blockIdx.x * 32, t0 = blockIdx.y * 32;
+  const int c0 = blockIdx.y * 32, t0 = blockIdx.x * 32;
   for (int j = threadIdx.y; j < 32; j += 8) {
     const int c = c0 + j;
     tile[j][threadIdx.x] = (c < B) ? W[(int64_t)c * ldw + t0 + threadIdx.x] : 0.0;
@@ -222,7 +223,7 @@ rows_sqnorm_kernel(const double* __restrict__ rows, int nC, int B, double* __res
 void launch_l0_loocv_fill(const uint32_t* gp, int64_t npad, int bs, int nC, const double* mu, const double* inv_sd,
                           const double* Bv, int C, const double* xy, int cpp, double* cm, int64_t cm_stride,
                           int nrow0, int R, cudaStream_t s) {
-  dim3 grid((unsigned)ceil_div(nC, 128), (unsigned)npad);
+  dim3 grid((unsigned)npad, (unsigned)ceil_div(nC, 128));
   l0_loocv_fill_kernel<<<grid, 128, 0, s>>>(gp, npad / 16, bs, nC, mu, inv_sd, Bv, C, xy, cpp, cm, cm_stride, nrow0, R);
 }
 
@@ -244,7 +245,7 @@ void launch_l0_loocv_std_apply(double* const* W, int64_t npad, int col0, int P, 
 
 void launch_l1_loocv_fill(const double* W, int64_t ldw, int B, int nC, double* cm, int64_t cm_stride, int nrow0,
                           int R1, int64_t npad, cudaStream_t s) {
-  dim3 grid((unsigned)ceil_div(nC, 32), (unsigned)(npad / 32));
+  dim3 grid((unsigned)(npad / 32), (unsigned)ceil_div(nC, 32));
   l1_loocv_fill_kernel<<<grid, dim3(32, 8), 0, s>>>(W, ldw, B, nC, cm, cm_stride, nrow0, R1);
 }
 

@@ -1131,6 +1131,28 @@ int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_byt
     if (cudaMemcpy(out, p, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) { rg::set_last_error("copy failed"); return -1; }
     return (int64_t)bytes;
   }
+  if (n.compare(0, 3, "l1_") == 0) {   // test-only: shape and state of the last level-1 fit
+    if (!h->l1_done) { rg::set_last_error("no level-1 fit on this handle"); return -1; }
+    const int64_t nC = h->l1_nC, P = h->P;
+    const void* p = nullptr;
+    size_t bytes = 0;
+    if (n == "l1_dims") {
+      const int64_t v[8] = {h->B, nC, h->R1, h->K, h->l1_nmat, h->l1_n_aug, h->l1_nchunks, h->l1_chunk_len};
+      if (max_bytes < (int64_t)sizeof(v)) { rg::set_last_error("buffer too small: " + n); return -1; }
+      memcpy(out, v, sizeof(v));
+      return sizeof(v);
+    }
+    if (n == "l1_chunks") { p = h->l1_chunks.p; bytes = (size_t)h->l1_nchunks * sizeof(int4); }   // (t0, len, fold, 0)
+    else if (n == "l1_beta" && !h->loocv) { p = h->l1_beta.p; bytes = (size_t)P * h->K * h->R1 * nC * 8; }   // [P][K R1][nC]
+    else if (n == "l1_sums" && !h->l1_bt) { p = h->l1_sums.p; bytes = (size_t)P * (kMaxRidge * 3 + 2) * 8; }
+    else if (n == "l1_bvec" && h->loocv) { p = h->l1_bvec.p; bytes = (size_t)P * nC * 8; }
+    else if (n == "l1_hvec" && h->loocv) { p = h->l1_hvec.p; bytes = (size_t)P * h->Npad * 8; }
+    else { rg::set_last_error("no level-1 debug buffer " + n + " for this fit"); return -1; }
+    if (!p) { rg::set_last_error("debug buffer not allocated: " + n); return -1; }
+    if ((int64_t)bytes > max_bytes) { rg::set_last_error("buffer too small: " + n); return -1; }
+    if (cudaMemcpy(out, p, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) { rg::set_last_error("copy failed"); return -1; }
+    return (int64_t)bytes;
+  }
   if (h->lanes.empty()) { rg::set_last_error("no level-0 lane"); return -1; }
   rg_ctx::Lane& L = *h->lanes[h->last_lane];
   const void* p = nullptr;
