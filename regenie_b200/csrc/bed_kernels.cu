@@ -91,11 +91,6 @@ __global__ void bed_expand_fp8_kernel(const uint32_t* __restrict__ gp, int64_t w
   *reinterpret_cast<uint4*>(z + (int64_t)(rows_p + row) * npad + w * 16) = m;
 }
 
-__global__ void debug_sleep_kernel(unsigned ns) {
-  for (unsigned i = 0; i < ns / 1000u; ++i) __nanosleep(1000u);
-}
-void launch_debug_sleep(unsigned ns, cudaStream_t s) { debug_sleep_kernel<<<1, 1, 0, s>>>(ns); }
-
 void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int rows_p,
                          const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep, int ref_first,
                          uint32_t* gp, int64_t npad,

@@ -20,10 +20,6 @@
 // "lanes" run concurrently, so launch-wide lockstep cannot be assumed.
 // The stored inverses M also turn the backward substitution's triangular solves into GEMVs.
 #include "gemm_dmma.cuh"
-#include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
-
 #include "kernels.cuh"
 
 namespace rg {
@@ -241,36 +237,11 @@ void launch_chol_factor(double* cm, int64_t stride, int nC, int n_aug, int batch
   const int64_t inv_stride = (int64_t)(nC / TB) * TB * TB;
   ensure_dyn_smem(reinterpret_cast<const void*>(chol_update_trsm_kernel), kFusedSmem);
   double* inv_t = inv + (int64_t)batch * inv_stride;      // M^T blocks live behind the M blocks (chol_inv_elems)
-  // profiling aid (RG_B200_CHOL_TIMING=1): CUDA-event time of the three kernels of every panel step
-  static const bool timing = getenv("RG_B200_CHOL_TIMING") != nullptr;
-  static const char* skip = getenv("RG_DBG_SKIP");                       // profiling aid, see rg_api.cu
-  const bool skip_diag = skip && strstr(skip, "diag"), skip_fused = skip && strstr(skip, "fused");
-  static double t_acc[3] = {0, 0, 0};
-  static long t_calls = 0;
-  cudaEvent_t ev[4];
-  if (timing) for (auto& e : ev) cudaEventCreate(&e);
-  auto tick = [&](int i) { if (timing) cudaEventRecord(ev[i], s); };
-  auto tock = [&]() {
-    if (!timing) return;
-    cudaEventSynchronize(ev[3]);
-    for (int i = 0; i < 3; ++i) { float ms = 0; cudaEventElapsedTime(&ms, ev[i], ev[i + 1]); t_acc[i] += ms; }
-  };
   for (int kb = 0; kb < nC / TB; ++kb) {
     const int k = kb * TB;
-    tick(0);
-    tick(1);
-    if (!skip_diag) chol_diag_kernel<<<batch, 256, 0, s>>>(cm, stride, nC, k, inv, inv_t, inv_stride, err_slot, err_base);
-    tick(2);
+    chol_diag_kernel<<<batch, 256, 0, s>>>(cm, stride, nC, k, inv, inv_t, inv_stride, err_slot, err_base);
     dim3 g2(ntiles - kb - 1, 1, batch);
-    if (ntiles - kb - 1 > 0 && !skip_fused) chol_update_trsm_kernel<<<g2, 256, kFusedSmem, s>>>(cm, stride, nC, k, kb, inv_t, inv_stride);
-    tick(3);
-    tock();
-  }
-  if (timing) {
-    for (auto& e : ev) cudaEventDestroy(e);
-    if (++t_calls % 50 == 0)
-      fprintf(stderr, "[chol timing] per factorisation (ms): (unused) %.3f diag %.3f update+solve %.3f\n", t_acc[0] / t_calls,
-              t_acc[1] / t_calls, t_acc[2] / t_calls);
+    if (ntiles - kb - 1 > 0) chol_update_trsm_kernel<<<g2, 256, kFusedSmem, s>>>(cm, stride, nC, k, kb, inv_t, inv_stride);
   }
 }
 

@@ -19,9 +19,6 @@
 //   Lplain, Mplain : [nmat][n][n] L as one FP32 plane (off-diagonal tiles), [nmat][n/128][128][128] the M_k
 //   Af             : [K][n][n] FP64 full symmetric fold systems WITHOUT the ridge shift (l0_assemble_sym_kernel)
 //   bvec, xvec, rvec : [.][Pp][n] FP64 right-hand sides (per fold), solutions and residuals (per system)
-#include <stdlib.h>
-#include <string.h>
-
 #include <algorithm>
 
 #include "gemm_dmma.cuh"
@@ -260,7 +257,7 @@ potrf128_kernel(float* __restrict__ Lp, float* __restrict__ Wp, float* __restric
 //   (b) kMxSafety (dx_s / x)^2 <= tol      : predicted error of x_s = rho dx_s with rho <= kMxSafety dx_s/x.  kMxSafety = 64
 //       covers the worst ratio sqrt(n) = 32..45 between the operator norm and its gain on a generic vector; with the
 //       benchmark's dx_1/x = 2.6e-6 the predicted bound is 4e-10 and the measured error of x_1 8e-12.
-// RG_B200_MX_STRICT=1 keeps only (a).
+// A negative tol (rg_dbg_mixed_solve) keeps only (a).
 constexpr float kMxSafety = 64.f;
 __device__ __forceinline__ bool mx_finished(const unsigned int* conv, int nmat, int m, int upto_step, float tol) {
   const bool strict = tol < 0.f;                      // the host passes -tol for the strict rule
@@ -389,8 +386,8 @@ mx_residual_fused_kernel(const double* __restrict__ Af, const double* __restrict
 //
 // The loads do not depend on the arithmetic, only their ORDER does: a producer thread streams every tile the sweep needs,
 // in consumption order, through a 6-stage TMA ring (16 KiB sub-tiles of 32 contraction indices x 128 output rows), and
-// runs as far ahead as the ring allows; eight consumer warps own one output row per lane and half of each sub-tile's
-// contraction range, so a sub-tile costs no shuffles and no bank conflicts (the tile is read [c][r], r contiguous).  L is
+// runs as far ahead as the ring allows; sixteen consumer warps, in 4 row groups x 4 slices, own one output row per lane and
+// a quarter of each sub-tile's contraction range, so a sub-tile costs no shuffles and no bank conflicts (the tile is read [c][r], r contiguous).  L is
 // kept as one FP32 plane with BOTH triangles (lower = L, upper = L^T, written by the TRSM tiles' epilogue) and M_k in both
 // orientations, which makes the two sweeps the same code on different triangles.  FP32 throughout - a correction needs
 // few digits - and the result is added to the FP64 solution.  The first version (plain loads, one CTA per system) was
@@ -400,7 +397,7 @@ constexpr int TS_STAGES = 6;
 constexpr int TS_SUB = 32;                          // contraction indices per sub-tile
 constexpr int TS_STAGE_BYTES = TS_SUB * PT * 4;     // 16 KiB
 constexpr int TS_VP = 12;                           // floats per row of the vector buffers (P <= 12, 16-byte aligned rows)
-// consumer warps (template parameter TS_CW, 8 or 16): 4 row groups x TS_CW / 4 slices of each sub-tile's contraction range
+constexpr int TS_CW = 16;                           // consumer warps: 4 row groups x TS_CW / 4 slices of the contraction range
 
 __device__ __forceinline__ uint32_t ts_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void ts_mbar_wait(uint32_t bar, uint32_t parity) {
@@ -416,7 +413,7 @@ __device__ __forceinline__ void ts_mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-template <int PMAX, int TS_CW>
+template <int PMAX>
 __global__ void __launch_bounds__(32 * (TS_CW + 1))
 mx_trisolve_kernel(const __grid_constant__ CUtensorMap tmL, const __grid_constant__ CUtensorMap tmM,
                    const __grid_constant__ CUtensorMap tmMT, const double* __restrict__ rvec, int64_t r_mat_stride,
@@ -687,25 +684,16 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
   ensure_dyn_smem(reinterpret_cast<const void*>(potrf128_kernel), potrf_smem);
   ensure_dyn_smem(reinterpret_cast<const void*>(mx_residual_kernel<12>), 98304);
   ensure_dyn_smem(reinterpret_cast<const void*>(mx_residual_kernel<10>), 98304);
-  static const bool res_fused = [] { const char* e = getenv("RG_B200_MX_RES"); return !(e && strcmp(e, "plain") == 0); }();
   RG_CHECK(n <= 2048, "mixed solver: n <= 2048");
   // substitution sweeps: the stage ring, the solution vector of all n rows and the slice partial sums.  At n = 2048 with
   // 16 consumer warps that is 222 KiB, close to the 227 KiB a block may opt into, so the limit is set from the same formula
-  static const int tri_warps = [] { const char* e = getenv("RG_B200_MX_TRI_WARPS"); return (e && atoi(e) == 8) ? 8 : 16; }();
-  const size_t sm_t = (size_t)TS_STAGES * TS_STAGE_BYTES + ((size_t)n + (1 + tri_warps / 4) * PT) * TS_VP * sizeof(float) + 2 * TS_STAGES * 8 + 256;
-  ensure_dyn_smem(reinterpret_cast<const void*>(tri_warps == 8 ? mx_trisolve_kernel<12, 8> : mx_trisolve_kernel<12, 16>), sm_t);
-  ensure_dyn_smem(reinterpret_cast<const void*>(tri_warps == 8 ? mx_trisolve_kernel<10, 8> : mx_trisolve_kernel<10, 16>), sm_t);
-  // profiling aid (results are garbage): RG_DBG_SKIP=mxgemm|mxpotrf|mxtri|mxres drops one kernel family of the solver so
-  // its marginal cost under multi-lane overlap can be read off
-  static const char* skip_env = getenv("RG_DBG_SKIP");
-  const bool sk_gemm = skip_env && strstr(skip_env, "mxgemm"), sk_potrf = skip_env && strstr(skip_env, "mxpotrf");
-  const bool sk_tri = skip_env && strstr(skip_env, "mxtri"), sk_res = skip_env && strstr(skip_env, "mxres");
+  const size_t sm_t = (size_t)TS_STAGES * TS_STAGE_BYTES + ((size_t)n + (1 + TS_CW / 4) * PT) * TS_VP * sizeof(float) + 2 * TS_STAGES * 8 + 256;
+  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<12>), sm_t);
+  ensure_dyn_smem(reinterpret_cast<const void*>(mx_trisolve_kernel<10>), sm_t);
   RG_CUDA(cudaMemsetAsync(d.conv.p, 0, d.conv.n * sizeof(unsigned int), s));
   const int4* tl = d.plan.tiles.p;
   Tf32GemmEpilogue e0{};
   e0.n = n; e0.out_mat_stride = (int64_t)n * n;
-  static const int l2pf = [] { const char* e = getenv("RG_B200_MX_L2PF"); return e ? std::max(0, std::min(8, atoi(e))) : 0; }();
-  e0.l2_prefetch = l2pf;       // off by default
   // ---- factorisation: left-looking, 128-wide panels
   for (int k = 0; k < nt; ++k) {
     Tf32GemmEpilogue e = e0;
@@ -715,14 +703,14 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
     e.c_chunks = 4; e.c_mat_div = d.R;
     e.diag_add = lambda; e.diag_mod = d.R;
     // panel step 0 has nothing to subtract: the assembler already wrote block column 0 of every system (first_col_ready)
-    if (!sk_gemm && !(k == 0 && first_col_ready)) launch_tf32x3_gemm(d.tmL, d.tmL, tl + d.plan.upd[k].x, d.plan.upd[k].y, nmat, e, s, &d.tmAp, &d.tmI);
-    if (!sk_potrf) potrf128_kernel<<<nmat, 256, potrf_smem, s>>>(d.Lp.p, d.Wp.p, d.Mplain.p, d.MTplain.p, n, k, fail_flag);
+    if (!(k == 0 && first_col_ready)) launch_tf32x3_gemm(d.tmL, d.tmL, tl + d.plan.upd[k].x, d.plan.upd[k].y, nmat, e, s, &d.tmAp, &d.tmI);
+    potrf128_kernel<<<nmat, 256, potrf_smem, s>>>(d.Lp.p, d.Wp.p, d.Mplain.p, d.MTplain.p, n, k, fail_flag);
     if (d.plan.trsm[k].y > 0) {
       Tf32GemmEpilogue t = e0;
       t.out = d.Lp.p;
       t.out_plain = d.Lplain.p;                      // the same tiles as one FP32 plane, and their transposes in the upper
       t.mirror = 1;                                  // triangle: what the two substitution sweeps stream
-      if (!sk_gemm) launch_tf32x3_gemm(d.tmL, d.tmW, tl + d.plan.trsm[k].x, d.plan.trsm[k].y, nmat, t, s);
+      launch_tf32x3_gemm(d.tmL, d.tmW, tl + d.plan.trsm[k].x, d.plan.trsm[k].y, nmat, t, s);
     }
   }
   // ---- x0 = (L L^T)^-1 b, then  x += (L L^T)^-1 (b - A x)  by block substitution, one CTA per system
@@ -735,17 +723,15 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
       const int64_t o = (int64_t)p0 * n;
       // right-hand-side count is a template parameter (register blocking): 10 is the benchmark's trait count
       auto tri = [&](const double* rv, int64_t rs, int rdiv, int step) {
-        if (sk_tri) return;
-#define RG_TRI(PM, CW) mx_trisolve_kernel<PM, CW><<<nmat, 32 * (CW + 1), sm_t, s>>>(d.tmLpl, d.tmMpl, d.tmMTpl, rv, rs, rdiv, xvec + o, n, np, d.Pp, nmat, step, d.conv.p, tol)
-        if (np <= 10) { if (tri_warps == 8) RG_TRI(10, 8); else RG_TRI(10, 16); }
-        else { if (tri_warps == 8) RG_TRI(12, 8); else RG_TRI(12, 16); }
+#define RG_TRI(PM) mx_trisolve_kernel<PM><<<nmat, 32 * (TS_CW + 1), sm_t, s>>>(d.tmLpl, d.tmMpl, d.tmMTpl, rv, rs, rdiv, xvec + o, n, np, d.Pp, nmat, step, d.conv.p, tol)
+        if (np <= 10) RG_TRI(10);
+        else RG_TRI(12);
 #undef RG_TRI
       };
       if (st == 0) {
         tri(bvec + o, (int64_t)d.Pp * n, d.R, 0);
       } else {
-        if (sk_res) {}
-        else if (res_fused && d.R * np <= RF_NV && n % RF_ROWS == 0)
+        if (d.R * np <= RF_NV && n % RF_ROWS == 0)
           mx_residual_fused_kernel<<<dim3(n / RF_ROWS, d.K), 256, 0, s>>>(Af, lambda, d.R, bvec + o, xvec + o, rvec + o, n, np, d.Pp, nmat, st, d.conv.p, tol);
         else if (np <= 10) mx_residual_kernel<10><<<grid, 256, sm_r, s>>>(Af, lambda, d.R, bvec + o, xvec + o, rvec + o, n, np, d.Pp, nmat, st, d.conv.p, tol);
         else mx_residual_kernel<12><<<grid, 256, sm_r, s>>>(Af, lambda, d.R, bvec + o, xvec + o, rvec + o, n, np, d.Pp, nmat, st, d.conv.p, tol);
@@ -753,22 +739,6 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
       }
     }
   mx_final_check_kernel<<<(nmat + 63) / 64, 64, 0, s>>>(d.conv.p, nmat, steps, tol, fail_flag);
-  static const bool dbg_conv = getenv("RG_DBG_MX_CONV") != nullptr;      // diagnostic: correction sizes per step
-  if (dbg_conv) {
-    std::vector<unsigned int> hc(d.conv.n);
-    RG_CUDA(cudaStreamSynchronize(s));
-    RG_CUDA(cudaMemcpy(hc.data(), d.conv.p, hc.size() * 4, cudaMemcpyDeviceToHost));
-    for (int m = 0; m < nmat; m += std::max(1, nmat / 5)) {
-      fprintf(stderr, "[mx conv] system %d:", m);
-      for (int st = 1; st <= steps; ++st) {
-        float dx, xx;
-        memcpy(&dx, &hc[((size_t)st * nmat + m) * 2], 4);
-        memcpy(&xx, &hc[((size_t)st * nmat + m) * 2 + 1], 4);
-        fprintf(stderr, "  step %d dx/x = %.3g", st, xx > 0 ? dx / xx : 0.0);
-      }
-      fprintf(stderr, "\n");
-    }
-  }
 }
 
 float* MixedSolver::a_planes() { return impl->Ap.p; }

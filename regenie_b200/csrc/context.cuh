@@ -45,8 +45,6 @@ struct rg_ctx {
   rg::DevBuf<unsigned long long> err_slot;
   cudaStream_t poll_stream = nullptr;              // rg_l0_poll_status: the error word is read here, beside the lanes
   unsigned long long* poll_host = nullptr;         // pinned
-  rg::DevBuf<unsigned long long> dbg_counter;
-  rg::DevBuf<long long> dbg_clk;
 
   // ---- per-lane scratch: consecutive blocks go to different lanes (own stream + buffers) so the
   //      latency-bound solver phases of one block overlap the tensor/HBM phases of the next
@@ -65,7 +63,7 @@ struct rg_ctx {
     int packed_flip = 0;
     rg::DevBuf<uint8_t> pgen_in;      // rg_pgen_decode: metadata blob + record bytes of the block this lane runs next
     rg::DevBuf<uint32_t> gp;          // [rows_p][Npad/16]
-    rg::DevBuf<uint8_t> z;            // [2 rows_p][Npad] e4m3
+    rg::DevBuf<uint8_t> z;            // [2 rows_p][Npad] int8
     rg::DevBuf<float> zz;             // [K][2 rows_p][2 rows_p]
     rg::DevBuf<float> tstat;          // [K][2 rows_p][stat_drows] exact digit sums of the statistics tiles
     rg::DevBuf<int32_t> cnt_part, cnt_fold;
@@ -75,7 +73,7 @@ struct rg_ctx {
     rg::DevBuf<double> inv;           // [nmat][nC/64][64x64]  L_kk^-T blocks
     rg::DevBuf<double> gam, gmu, cvec, part, mean_invsd;
     std::map<int, CUtensorMap> tmaps; // keyed by rows_p (z base differs per lane)
-    rg::DevBuf<uint8_t> dig;          // radix-30 digit rows of gamma for the tensor-core prediction
+    rg::DevBuf<uint8_t> dig;          // radix-254 digit rows of gamma for the tensor-core prediction
     rg::DevBuf<double> wraw;          // [P][R][Npad] raw (unstandardised) predictions of the block, local to this GPU
     rg::DevBuf<double*> wraw_tab;     // [P] per-phenotype base pointers into wraw (same addressing as W_tab with col0 = 0)
     rg::DevBuf<double> dscale;        // [K][Qp] column scales
@@ -99,16 +97,18 @@ struct rg_ctx {
   int next_lane = 0, last_lane = 0;
   rg::DevBuf<uint8_t> packed_dev;    // step 2 (single lane)
   rg::DevBuf<uint32_t> gp;           // step 2
-  std::map<int, std::unique_ptr<rg::DevBuf<int2>>> tile_lists;
-  std::map<int, int> tile_counts;
+  // Gram tile lists on the device, keyed by rows_p: the Z Z^T tiles, and the statistics tiles Z [X | Y]-digits
+  struct TileList {
+    rg::DevBuf<int2> buf;
+    int count = 0;
+  };
+  std::map<int, TileList> tile_lists, stat_tile_lists;
   // statistics on the tensor cores: digit rows of (X | Y), built once
   bool stats_tc = false;
   int stat_drows = 0;
   rg::DevBuf<uint8_t> xyD;
   rg::DevBuf<double> xy_scale;
   CUtensorMap tmD;
-  std::map<int, std::unique_ptr<rg::DevBuf<int2>>> stat_tile_lists;
-  std::map<int, int> stat_tile_counts;
 
   // ---- level-0 output
   rg::DevBuf<double> W;             // [P][Npad x B] column-major
@@ -194,7 +194,6 @@ struct rg_ctx {
 
   // ---- level-0 solver selection (RG_B200_SOLVER = mixed | f64) and its counters
   int solver_mixed = 1;
-  int mx_steps = 3;
   float mx_tol = 1e-9f;
   int64_t mx_blocks = 0, mx_fallbacks = 0;
 
@@ -206,6 +205,11 @@ struct rg_ctx {
 };
 
 namespace rg {
+// throws unless `device` is an sm_90 GPU
+void require_gpu(int device);
+// the genotype file's sample index map (file_idx_pad, word_base, word_keep), rebuilt only when sample_idx changes;
+// sample_idx is a host or a device array of n_samples entries, or null for the identity
+void ensure_file_idx(rg_ctx* h, const int32_t* sample_idx);
 void flush_timers(rg_ctx* h);
 // read the mixed-solver flags of every lane (re-solving flagged blocks in FP64) and wait for all level-0 work
 void sync_lanes(rg_ctx* h);

@@ -15,8 +15,6 @@
 //                in registers, int32) and stores them, times out_scale, as FP32 straight from the fragments
 //   warp 8     : TMA producer (cp.async.bulk.tensor 2D, 128B swizzle, 4-stage mbarrier ring)
 // K loop = the fold's samples in 128-byte (= 128-sample) swizzle atoms, 4 MMAs per atom.
-#include <stdlib.h>
-
 #include "kernels.cuh"
 #include "wgmma_sm90.cuh"
 
@@ -175,8 +173,7 @@ void make_gram_tensor_map(CUtensorMap* tm, const uint8_t* z, int64_t npad, int r
 }
 
 size_t gram_smem_bytes(int bn) {
-  static const bool exclusive = getenv("RG_DBG_GRAM_EXCLUSIVE") != nullptr;   // 227 KiB: the H100 opt-in maximum
-  return exclusive ? (size_t)232448 : (size_t)STAGES * (A_BYTES + bn * BK) + 1024 + 128;
+  return (size_t)STAGES * (A_BYTES + bn * BK) + 1024 + 128;
 }
 
 void gram_tile_list(int rows2, std::vector<int2>& tiles) {

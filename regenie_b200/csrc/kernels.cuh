@@ -17,7 +17,6 @@ void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int 
                          const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep, int ref_first,
                          uint32_t* gp, int64_t npad,
                          cudaStream_t s);
-void launch_debug_sleep(unsigned ns, cudaStream_t s);
 void launch_bed_expand_fp8(const uint32_t* gp, int rows_p, uint8_t* z, int64_t npad, cudaStream_t s);
 
 // ---- l0_stats.cu
@@ -51,8 +50,6 @@ struct AssembleArgs {
                              // receive A_f + lambda_r I (panel step 0 of the left-looking factorisation has nothing to subtract)
 };
 
-void launch_dbg_check_diag(const float* zz, int64_t ldz, int64_t fold_stride, const int32_t* cnt_fold, int rows_p,
-                           int bs, int K, unsigned long long* counter, cudaStream_t s);
 void launch_l0_stats(const uint32_t* gp, int64_t npad, const double* xy, int cpp, const int4* chunks,
                      int nchunks, int rows_p, int32_t* cnt_part, double* sum_part, cudaStream_t s);
 void launch_l0_fold_reduce(const int32_t* cnt_part, const double* sum_part, int rows_p, int cpp,
@@ -108,7 +105,6 @@ struct Tf32GemmEpilogue {
   int diag_mod;
   int c_chunks;               // 0, or 4: leading K chunks  acc = C_tile * I  followed by the main chunks with A negated
   int c_mat_div;              // C matrix index = mat / c_mat_div
-  int l2_prefetch;            // K chunks whose operand boxes are prefetched into L2 ahead of the single shared-memory stage
 };
 void make_tf32_planes_tensor_map(CUtensorMap* tm, const float* planes, int n, int batch);
 void make_tf32_identity_planes(DevBuf<float>& buf, CUtensorMap* tm);
@@ -191,7 +187,6 @@ struct PredictTcArgs {
   const uint8_t* mask;
   double* const* W;
   double* part;
-  int l2_prefetch = 0;       // INT8 kernel: k-blocks of the genotype planes prefetched into L2 ahead of the ring
 };
 void make_byte_tensor_map(CUtensorMap* tm, const uint8_t* basep, int64_t inner, int64_t rows);
 int launch_l0_colsum(double* const* W, int64_t npad, int col0, int P, int Q, int Qp, double* part,

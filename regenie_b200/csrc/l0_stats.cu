@@ -377,23 +377,6 @@ __global__ void l0_rhs_rows_kernel(AssembleArgs a, const double* __restrict__ rh
   a.cm[(int64_t)m * a.cm_stride + (int64_t)(a.nC + p) * a.ldc + i] = v;
 }
 
-// debug-only consistency probe: diag of the tensor-core Grams vs the popcount statistics
-__global__ void dbg_check_diag_kernel(const float* zz, int64_t ldz, int64_t fold_stride, const int32_t* cnt_fold,
-                                      int rows_p, int bs, int K, unsigned long long* counter) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= bs) return;
-  for (int f = 0; f < K; ++f) {
-    const int32_t* c4 = cnt_fold + ((int64_t)f * rows_p + i) * 4;
-    const float gg = zz[(int64_t)f * fold_stride + (int64_t)i * ldz + i];
-    const float mm = zz[(int64_t)f * fold_stride + (int64_t)(rows_p + i) * ldz + rows_p + i];
-    if (gg != (float)(c4[0] + 4 * c4[1]) || mm != (float)c4[2]) atomicAdd(counter, 1ull);
-  }
-}
-void launch_dbg_check_diag(const float* zz, int64_t ldz, int64_t fold_stride, const int32_t* cnt_fold, int rows_p,
-                           int bs, int K, unsigned long long* counter, cudaStream_t s) {
-  dbg_check_diag_kernel<<<(unsigned)ceil_div(bs, 128), 128, 0, s>>>(zz, ldz, fold_stride, cnt_fold, rows_p, bs, K, counter);
-}
-
 void launch_l0_stats(const uint32_t* gp, int64_t npad, const double* xy, int cpp, const int4* chunks,
                      int nchunks, int rows_p, int32_t* cnt_part, double* sum_part, cudaStream_t s) {
   dim3 grid(rows_p / 128, nchunks, cpp / kStatCols);

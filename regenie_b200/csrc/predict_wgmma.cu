@@ -126,13 +126,9 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
     if (lane == 0) {
       // ===== TMA producer: A = 128 plane rows x 128 samples; B = 256 digit rows x 128 k bytes =====
       const int drow0 = (f * a.ngroups + g) * PI_BN;
-      // the genotype planes stream from DRAM: their boxes may be prefetched into L2 `pf` k-blocks ahead of the ring
-      const int pf = a.l2_prefetch;
-      for (int kb = PI_STAGES; kb < PI_STAGES + pf && kb < nkb; ++kb) tma_prefetch_2d(&tmZ, tile * PT_BM, kb * PT_BK);
       for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb % PI_STAGES;
         const uint32_t ph = (kb / PI_STAGES) & 1;
-        if (pf > 0 && kb + PI_STAGES + pf < nkb) tma_prefetch_2d(&tmZ, tile * PT_BM, (kb + PI_STAGES + pf) * PT_BK);
         mbar_wait(empty_bar + 8 * s, ph ^ 1);
         mbar_expect_tx(full_bar + 8 * s, PI_STAGE_BYTES);
         tma_load_2d(sA + s * PI_A_BYTES, &tmZ, full_bar + 8 * s, tile * PT_BM, kb * PT_BK);

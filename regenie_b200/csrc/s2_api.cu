@@ -21,10 +21,6 @@ using namespace rg;
   }                                        \
   return 0;
 
-namespace rg {
-void require_gpu_public(int device);
-}
-
 static void s2_create(rg_ctx* h, const rg_step2_config* cfg, const double* X, const uint8_t* mask,
                       const uint8_t* in_analysis) {
   h->kind = 2;
@@ -185,8 +181,6 @@ static const uint8_t* take_non_par(rg_ctx* h, int bs) {
 }
 
 namespace rg {
-void build_file_idx_public(rg_ctx* h, const int32_t* sample_idx_host);
-
 // A block whose input pointer lies in a staging buffer (rg_s2_stage) waits for that slot's copy, and only for it: the
 // copy of the block AFTER it may already be in flight on the copy stream.
 static void s2_wait_stage(rg_ctx* h, const void* in, cudaStream_t s) {
@@ -241,20 +235,7 @@ static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   const int P = h->P, C = h->C;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  {
-    std::vector<int32_t> host_idx;
-    if (sample_idx) {
-      host_idx.resize(h->N);
-      RG_CUDA(cudaMemcpy(host_idx.data(), sample_idx, h->N * 4, cudaMemcpyDefault));
-      if (!h->file_idx_valid || h->cached_sample_idx != host_idx) {
-        build_file_idx_public(h, host_idx.data());
-        h->cached_sample_idx = host_idx;
-      }
-    } else if (!h->file_idx_valid || !h->cached_sample_idx.empty()) {
-      build_file_idx_public(h, nullptr);
-      h->cached_sample_idx.clear();
-    }
-  }
+  ensure_file_idx(h, sample_idx);
   const uint8_t* packed_d = packed;
   if (!is_device_pointer(packed)) {
     h->packed_dev.alloc((size_t)h->bs_max * row_stride);
@@ -362,19 +343,7 @@ static void s2_block_bgen8_bt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
   const int P = h->P, C = h->C, dp = h->bt_dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  {
-    std::vector<int32_t> host_idx;
-    if (sample_idx) {
-      host_idx.assign(sample_idx, sample_idx + h->N);
-      if (!h->file_idx_valid || h->cached_sample_idx != host_idx) {
-        build_file_idx_public(h, host_idx.data());
-        h->cached_sample_idx = host_idx;
-      }
-    } else if (!h->file_idx_valid || !h->cached_sample_idx.empty()) {
-      build_file_idx_public(h, nullptr);
-      h->cached_sample_idx.clear();
-    }
-  }
+  ensure_file_idx(h, sample_idx);
   const uint8_t *probs_d = probs, *miss_d = miss;
   if (!is_device_pointer(probs)) {
     h->probs_dev.alloc((size_t)h->bs_max * n_file * 2);
@@ -431,19 +400,7 @@ static void s2_block_bgen8_qt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
   const int P = h->P, C = h->C, dp = h->dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  {
-    std::vector<int32_t> host_idx;
-    if (sample_idx) {
-      host_idx.assign(sample_idx, sample_idx + h->N);
-      if (!h->file_idx_valid || h->cached_sample_idx != host_idx) {
-        build_file_idx_public(h, host_idx.data());
-        h->cached_sample_idx = host_idx;
-      }
-    } else if (!h->file_idx_valid || !h->cached_sample_idx.empty()) {
-      build_file_idx_public(h, nullptr);
-      h->cached_sample_idx.clear();
-    }
-  }
+  ensure_file_idx(h, sample_idx);
   const uint8_t *probs_d = probs, *miss_d = miss;
   if (!is_device_pointer(probs)) {
     h->probs_dev.alloc((size_t)h->bs_max * n_file * 2);
@@ -502,19 +459,7 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   const int P = h->P, C = h->C, dp = h->bt_dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  {
-    std::vector<int32_t> host_idx;
-    if (sample_idx) {
-      host_idx.assign(sample_idx, sample_idx + h->N);
-      if (!h->file_idx_valid || h->cached_sample_idx != host_idx) {
-        build_file_idx_public(h, host_idx.data());
-        h->cached_sample_idx = host_idx;
-      }
-    } else if (!h->file_idx_valid || !h->cached_sample_idx.empty()) {
-      build_file_idx_public(h, nullptr);
-      h->cached_sample_idx.clear();
-    }
-  }
+  ensure_file_idx(h, sample_idx);
   const uint8_t* packed_d = packed;
   if (!is_device_pointer(packed)) {
     h->packed_dev.alloc((size_t)h->bs_max * row_stride);
@@ -730,7 +675,7 @@ int rg_step2_create(const rg_step2_config* cfg, const double* X, const uint8_t* 
                     const uint8_t* in_analysis, rg_handle* out) {
   RG_API_BEGIN
   RG_CHECK(cfg && X && mask && in_analysis && out, "null argument");
-  require_gpu_public(cfg->device);
+  require_gpu(cfg->device);
   RG_CHECK(cfg->n_samples > 0 && cfg->n_cov > 0 && cfg->n_pheno > 0 && cfg->max_block_size > 0, "bad sizes");
   RG_CHECK(cfg->n_cov <= kMaxCov, "too many covariates for this build");
   std::unique_ptr<rg_ctx> h(new rg_ctx());

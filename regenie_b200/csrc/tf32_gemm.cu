@@ -16,8 +16,6 @@
 //                stage), then the epilogue: accumulators -> shared memory -> optional  C_in - acc  in FP64 -> hi/lo
 //                planes (and / or the transposed tile, and / or a plain FP32 plane), one thread per tile row
 //   warp 4     : TMA producer - 3-D boxes {32 floats, 128 rows, 2 planes} with 128B swizzle, mbarrier ring
-#include <stdlib.h>
-
 #include "kernels.cuh"
 #include "wgmma_sm90.cuh"
 
@@ -29,8 +27,9 @@ using namespace sm90;
 
 constexpr int TG_M = 128, TG_N = 128;
 constexpr int TG_KC = 32;                          // floats per K chunk = one 128-byte swizzle atom
-// TG_STAGES is a template parameter: 1 (default) = one 64 KiB stage per CTA and several co-resident CTAs per SM: the
-// tiles of this solver are short (K <= 1024) and the launches small, so latency is hidden across CTAs
+// one 64 KiB stage per CTA and several co-resident CTAs per SM: the tiles of this solver are short (K <= 1024) and the
+// launches small, so latency is hidden across CTAs
+constexpr int TG_STAGES = 1;
 constexpr int TG_PLANE_BYTES = TG_M * 128;         // 16 KiB
 constexpr int TG_OP_BYTES = 2 * TG_PLANE_BYTES;    // hi + lo
 constexpr int TG_STAGE_BYTES = 2 * TG_OP_BYTES;    // A + B = 64 KiB (also holds the 128 x 128 FP32 result tile)
@@ -39,8 +38,7 @@ constexpr int TG_THREADS = 160;
 }  // namespace
 
 // grid: (ntiles, batch); tile entry = (A row tile, B row tile, first K chunk, number of K chunks)
-template <int TG_STAGES>
-__global__ void __launch_bounds__(TG_THREADS, TG_STAGES == 1 ? 2 : 1)
+__global__ void __launch_bounds__(TG_THREADS, 2)
 tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmI,
                       const int4* __restrict__ tiles, Tf32GemmEpilogue ep) {
@@ -79,21 +77,9 @@ tf32x3_gemm_nt_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     if (lane == 0) {
       const int cmat = 2 * (ep.c_mat_div > 0 ? mat / ep.c_mat_div : mat);
       // chunk kc: (kc < ncc) C tile x identity, else A / B row tiles at column (tile.z + kc - ncc) * TG_KC
-      auto prefetch = [&](int kc) {
-        if (kc < ncc) {
-          tma_prefetch_3d(&tmC, tile.y * TG_N + kc * TG_KC, tile.x * TG_M, cmat);
-        } else {
-          const int col = (tile.z + kc - ncc) * TG_KC;
-          tma_prefetch_3d(&tmA, col, tile.x * TG_M, 2 * mat);
-          tma_prefetch_3d(&tmB, col, tile.y * TG_N, 2 * mat);
-        }
-      };
-      const int pf = ep.l2_prefetch;                        // chunks kept in flight towards L2 ahead of the stage
-      for (int kc = 1; kc <= pf && kc < nkc; ++kc) prefetch(kc);
       for (int kc = 0; kc < nkc; ++kc) {
         const int s = kc % TG_STAGES;
         const uint32_t ph = (kc / TG_STAGES) & 1;
-        if (pf > 0 && kc + pf + 1 <= nkc - 1) prefetch(kc + pf + 1);
         mbar_wait(empty_bar + 8 * s, ph ^ 1);
         mbar_expect_tx(full_bar + 8 * s, TG_STAGE_BYTES);
         if (kc < ncc) {
@@ -330,20 +316,10 @@ void launch_tf32x3_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const in
                         const Tf32GemmEpilogue& ep, cudaStream_t s, const CUtensorMap* tmC, const CUtensorMap* tmI) {
   RG_CHECK(ep.c_chunks == 0 || (tmC && tmI), "tf32 gemm: the C phase needs its tensor maps");
   if (ntiles <= 0 || batch <= 0) return;
-  // RG_B200_MX_STAGES = 1 (default: co-resident CTAs hide the TMA latency) | 2 | 3 (one CTA per SM with a deeper ring)
-  static const int nst = [] { const char* e = getenv("RG_B200_MX_STAGES"); const int v = e ? atoi(e) : 1; return (v == 2 || v == 3) ? v : 1; }();
-  const size_t smem = (size_t)nst * TG_STAGE_BYTES + 1024 + 128;
+  const size_t smem = (size_t)TG_STAGES * TG_STAGE_BYTES + 1024 + 128;
   dim3 grid(ntiles, batch);
-  if (nst == 1) {
-    ensure_dyn_smem(reinterpret_cast<const void*>(tf32x3_gemm_nt_kernel<1>), smem);
-    tf32x3_gemm_nt_kernel<1><<<grid, TG_THREADS, smem, s>>>(tmA, tmB, tmC ? *tmC : tmA, tmI ? *tmI : tmB, tiles, ep);
-  } else if (nst == 2) {
-    ensure_dyn_smem(reinterpret_cast<const void*>(tf32x3_gemm_nt_kernel<2>), smem);
-    tf32x3_gemm_nt_kernel<2><<<grid, TG_THREADS, smem, s>>>(tmA, tmB, tmC ? *tmC : tmA, tmI ? *tmI : tmB, tiles, ep);
-  } else {
-    ensure_dyn_smem(reinterpret_cast<const void*>(tf32x3_gemm_nt_kernel<3>), smem);
-    tf32x3_gemm_nt_kernel<3><<<grid, TG_THREADS, smem, s>>>(tmA, tmB, tmC ? *tmC : tmA, tmI ? *tmI : tmB, tiles, ep);
-  }
+  ensure_dyn_smem(reinterpret_cast<const void*>(tf32x3_gemm_nt_kernel), smem);
+  tf32x3_gemm_nt_kernel<<<grid, TG_THREADS, smem, s>>>(tmA, tmB, tmC ? *tmC : tmA, tmI ? *tmI : tmB, tiles, ep);
 }
 
 }  // namespace rg
