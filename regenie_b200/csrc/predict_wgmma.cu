@@ -11,9 +11,11 @@
 //
 // Orientation: samples are the MMA M dimension, the 5 x 50 digit rows are N (256, zero padded), the SNP/plane index
 // is K.  The digit rows are K-major in shared memory (wgmma B operand).  The genotype tile arrives samples-contiguous
-// (MN-major), which 8-bit wgmma cannot read from shared memory, so the A operand comes from registers: a thread loads
-// 4 consecutive samples at 4 consecutive k as four 32-bit words and transposes the 4 x 4 bytes with byte permutes.
-// Its four samples fill its fragment rows in the two m64 halves of the 128-sample tile.
+// (MN-major), which 8-bit wgmma cannot read from shared memory, so the A operand comes from registers.  Each consumer
+// warpgroup owns one 64-sample half of the tile and all 256 digit rows (m64n256k32).  The two threads of a lane pair
+// (lane, lane ^ 4) share 4 consecutive samples: each loads them at 4 consecutive k (one of the two k quads of the
+// fragment) as four 32-bit words, transposes the 4 x 4 bytes with byte permutes, keeps its own two samples and trades
+// the other two with its partner.  The fragments of stage s + 1 are built while the MMAs of stage s run.
 #include <stdlib.h>
 
 #include "kernels.cuh"
@@ -28,11 +30,11 @@ using namespace sm90;
 constexpr int PT_BM = 128;            // samples per CTA
 constexpr int PT_BK = 128;            // Z rows per stage
 constexpr int PI_BN = 256;            // digit rows (5 limbs x 50 outputs, zero padded)
-constexpr int PI_STAGES = 3;
+constexpr int PI_STAGES = 4;
 constexpr int PI_A_BYTES = PT_BK * PT_BM;          // 16 KiB: 128 k-rows x 128 samples
 constexpr int PI_B_BYTES = PI_BN * PT_BK;          // 32 KiB: 256 digit rows x 128 k bytes
 constexpr int PI_STAGE_BYTES = PI_A_BYTES + PI_B_BYTES;
-constexpr int PI_THREADS = 288;                    // 2 consumer warpgroups (digit rows 0-127 / 128-255), 1 TMA warp
+constexpr int PI_THREADS = 288;                    // 2 consumer warpgroups (samples 0-63 / 64-127), 1 TMA warp
 constexpr int PI_QH = kLimbQI8 / 2;                // outputs per epilogue thread (25)
 constexpr int PI_LDE = PI_BN + 1;                  // row stride (int32) of the staged accumulator tile
 static_assert(kLimbsI8 * kLimbQI8 <= PI_BN && kLimbQI8 % 2 == 0, "INT8 prediction layout");
@@ -139,54 +141,73 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
     return;
   }
 
-  // ===== consumers: warpgroup wg = digit rows 128 wg .. 128 wg + 127; acc[m] = fragment rows of m64 half m =====
-  // Thread (warp w of the warpgroup, lane l) owns samples sb .. sb + 3, sb = 4 (8 w + l / 4): fragment row
-  // 16 w + l / 4 (+8) of half m is sample sb + 2 m (+1).
-  const int wg = warp >> 2, w = warp & 3, t4 = lane & 3;
-  const int sb = 4 * (8 * w + (lane >> 2));
-  int32_t acc[2][64];
+  // ===== consumers: warpgroup wg = samples 64 wg .. 64 wg + 63 x all 256 digit rows =====
+  // Thread (warp w of the warpgroup, lane l, r = l / 4, t4 = l % 4) holds fragment rows 16 w + r and 16 w + r + 8, which
+  // are samples 64 wg + 16 w + 2 r and the next one.  The pair (r, r ^ 1) shares the 4 samples from sq = 64 wg + 16 w +
+  // 4 (r / 2): the even thread loads them at the k quad 4 t4 .. +3 of each MMA, the odd one at 16 + 4 t4 .. +3.
+  const int wg = warp >> 2, w = warp & 3, r = lane >> 2, t4 = lane & 3;
+  const bool odd = r & 1;
+  const int sq = 64 * wg + 16 * w + 4 * (r >> 1);
+  // The 8 lanes reading one 16-byte sample chunk take the 4 k rows of their quad in rotated orders (rot = 0..3), so each
+  // load instruction of the warp meets 8 distinct swizzle phases, i.e. 32 distinct banks.  rsel undoes the rotation.
+  const int rot = 2 * odd + (t4 >> 1);
+  const uint32_t rsel = (0x32103210u >> (16 - 4 * rot)) & 0xFFFFu;
+  int aoff[4];                                      // byte offset of load i inside a 32-k slice of the A stage
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[0][i] = acc[1][i] = 0;
-  fence_regs(acc[0]);
-  fence_regs(acc[1]);
+  for (int i = 0; i < 4; ++i) {
+    const int kr = 16 * odd + 4 * t4 + ((i + rot) & 3);          // row of the 128B-swizzled tile
+    aoff[i] = kr * 128 + ((((sq >> 4) ^ (kr & 7)) << 4) | (sq & 15));
+  }
   const uint8_t* gA = gen_base;                     // generic view of the A stages
+
+  // A fragment of MMA kk of stage s: {row, row + 8} x {k 4 t4 .. +3, k 16 + 4 t4 .. +3} of the stage's 32-k slice kk
+  auto build = [&](int s, int kk, uint32_t (&af)[4]) {
+    uint32_t wv[4], v[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      wv[i] = *reinterpret_cast<const uint32_t*>(gA + s * PI_A_BYTES + kk * 32 * 128 + aoff[i]);
+    transpose4x4(wv, v);                            // v[j] = sample sq + j at the quad's k, rotated by rot bytes
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = __byte_perm(v[j], 0, rsel);
+    const uint32_t x0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 4);
+    const uint32_t x1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 4);
+    af[0] = odd ? x0 : v[0];
+    af[1] = odd ? x1 : v[1];
+    af[2] = odd ? v[2] : x0;
+    af[3] = odd ? v[3] : x1;
+  };
+  // One commit group per MMA, two fragment register sets: while MMA u runs, MMA u - 1 is retired (freeing its fragment
+  // registers, and at the first MMA of a stage the previous stage's buffers) and the fragment of MMA u + 1 is built.
+  // Double-buffering whole stages would need 32 fragment registers beside the 128 accumulators, more than the 168 a
+  // thread gets at 288 threads per SM.
+  int32_t acc[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0;
+  fence_regs(acc);
+  uint32_t afr[2][4];
+  mbar_wait(full_bar, 0);
+  build(0, 0, afr[0]);
   for (int kb = 0; kb < nkb; ++kb) {
     const int s = kb % PI_STAGES;
-    const uint32_t ph = (kb / PI_STAGES) & 1;
-    mbar_wait(full_bar + 8 * s, ph);
-    // A fragments of the stage's 4 MMAs: afr[kk][m] = {row, row + 8} x {k 4 t4 .. +3, k 16 + 4 t4 .. +3}
-    uint32_t afr[PT_BK / 32][2][4];
+    const uint64_t db = desc_k128(sB + s * PI_B_BYTES);
 #pragma unroll
     for (int kk = 0; kk < PT_BK / 32; ++kk) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t wv[4], v[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int kr = kk * 32 + h * 16 + 4 * t4 + i;          // row of the 128B-swizzled tile
-          wv[i] = *reinterpret_cast<const uint32_t*>(gA + s * PI_A_BYTES + kr * 128 + ((((sb >> 4) ^ (kr & 7)) << 4) | (sb & 15)));
-        }
-        transpose4x4(wv, v);
-        afr[kk][0][2 * h] = v[0];
-        afr[kk][0][2 * h + 1] = v[1];
-        afr[kk][1][2 * h] = v[2];
-        afr[kk][1][2 * h + 1] = v[3];
+      wgmma_fence();
+      // +32 bytes (K of one MMA) inside the 128-byte swizzle atom: +2 in 16-byte units
+      wgmma_s8_rs_n256(acc, afr[kk & 1], db + (uint64_t)(2 * kk));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (kk == 0 && kb > 0 && w == 0 && lane == 0) mbar_arrive(empty_bar + 8 * ((kb - 1) % PI_STAGES));
+      if (kk + 1 < PT_BK / 32) {
+        build(s, kk + 1, afr[(kk + 1) & 1]);
+      } else if (kb + 1 < nkb) {
+        mbar_wait(full_bar + 8 * ((kb + 1) % PI_STAGES), ((kb + 1) / PI_STAGES) & 1);
+        build((kb + 1) % PI_STAGES, 0, afr[0]);
       }
     }
-    const uint64_t db = desc_k128(sB + s * PI_B_BYTES + wg * (128 * PT_BK));
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < PT_BK / 32; ++kk) {
-      // +32 bytes (K of one MMA) inside the 128-byte swizzle atom: +2 in 16-byte units
-      wgmma_s8_rs_n128(acc[0], afr[kk][0], db + (uint64_t)(2 * kk));
-      wgmma_s8_rs_n128(acc[1], afr[kk][1], db + (uint64_t)(2 * kk));
-    }
-    wgmma_commit();
-    wgmma_wait<0>();                                // also frees the A registers for the next stage
-    if (w == 0 && lane == 0) mbar_arrive(empty_bar + 8 * s);
   }
-  fence_regs(acc[0]);
-  fence_regs(acc[1]);
+  wgmma_wait<0>();
+  fence_regs(acc);
 
   // ===== epilogue: accumulators -> shared memory tile E[sample][digit row] (the stage buffers are free once every
   // consumer is past its last MMA) -> thread = (sample, half of the outputs).  Limb sums are exact int32 multiples of 8;
@@ -194,13 +215,11 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
   named_sync(1, 256);
   int32_t* E = reinterpret_cast<int32_t*>(gen_base);
 #pragma unroll
-  for (int m = 0; m < 2; ++m)
-#pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      const int smp = sb + 2 * m + ((i >> 1) & 1);
-      const int col = wg * 128 + 8 * (i >> 2) + 2 * t4 + (i & 1);
-      E[smp * PI_LDE + col] = acc[m][i];
-    }
+  for (int i = 0; i < 128; ++i) {
+    const int smp = 64 * wg + 16 * w + 2 * r + ((i >> 1) & 1);
+    const int col = 8 * (i >> 2) + 2 * t4 + (i & 1);
+    E[smp * PI_LDE + col] = acc[i];
+  }
   named_sync(1, 256);
   {
     const int ct = threadIdx.x;                    // 0..255
