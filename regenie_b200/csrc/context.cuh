@@ -78,6 +78,7 @@ struct rg_ctx {
     rg::DevBuf<double*> wraw_tab;     // [P] per-phenotype base pointers into wraw (same addressing as W_tab with col0 = 0)
     rg::DevBuf<double> dscale;        // [K][Qp] column scales
     std::map<int, CUtensorMap> dmaps; // digit-matrix tensor maps keyed by rows_p
+    std::map<int, CUtensorMap> gmaps; // 2-bit row (gp) tensor maps of the INT8 prediction, keyed by rows_p
     // dense FP64 route for real-valued genotypes (l0_dense.cu)
     rg::DevBuf<uint8_t> dense_in;                 // staged host input (probability / ploidy bytes or FP64 rows)
     rg::DevBuf<double> gd, dpart, dpart_y;        // [bs][Npad] G~; chunk partials of G G^T and G Y

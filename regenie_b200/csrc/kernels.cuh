@@ -189,13 +189,17 @@ struct PredictTcArgs {
   double* part;
 };
 void make_byte_tensor_map(CUtensorMap* tm, const uint8_t* basep, int64_t inner, int64_t rows);
+void make_gp_tensor_map(CUtensorMap* tm, const uint32_t* gp, int64_t words_per_row, int64_t rows);
 int launch_l0_colsum(double* const* W, int64_t npad, int col0, int P, int Q, int Qp, double* part,
                      cudaStream_t s);
 // INT8 digits: 5 radix-254 digit rows per output, s8 x s8 -> s32 wgmma
 size_t predict_i8_dig_bytes(int K, int ngroups, int rows_p);
-void launch_l0_gamma_limbs_i8(const double* gam, const double* gmu, int Qp, int Q, int bs, int rows_p, int K,
-                              double* scale, uint8_t* dig, int ngroups, cudaStream_t s);
-void launch_l0_predict_i8(const CUtensorMap& tmZ, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
+// gam, gmu, cvec, scales and digit rows of every (output, fold) from the solutions, one CTA each
+void launch_l0_coef_i8(const double* cm, int64_t cm_stride, int ldc, int nC, int R, int P, int Q, int Qp, int bs,
+                       int rows_p, int K, const double* mu, const double* inv_sd, const double* Bv, int C, double* gam,
+                       double* gmu, double* cvec, double* scale, uint8_t* dig, int ngroups, cudaStream_t s);
+// A operand from the 2-bit rows (tmG over gp), digit rows (tmD); raw predictions to a.W, per-tile column sums to a.part
+void launch_l0_predict_i8(const CUtensorMap& tmG, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
                           cudaStream_t s);
 
 // ---- l1_kernels.cu

@@ -2,20 +2,22 @@
 //
 //   pred[t, q] = sum_i gamma[i,q] g0(i,t) + sum_i (gamma mu)[i,q] miss(i,t) - x_t . cvec_q
 // (reference: `beta.transpose() * Gmat.block(...)`, src/Step1_Models.cpp:503 - 2 P R bs N flops/block).
-// The genotype operand is the same plane pair Z = [G0; Miss] the Gram kernel consumes: its bytes are 8 x dosage as int8
-// (bed_expand_fp8_kernel).  The real-valued coefficients are split into FIVE balanced radix-254 digits
+// The genotype operand is the plane pair [G0; Miss] the Gram kernel consumes (8 x dosage and 8 x missing as int8, the
+// bytes bed_expand_fp8_kernel writes), but the kernel builds it in registers from the block's padded 2-bit rows: one
+// 32-bit word holds both planes of 16 samples, an eighth of the bytes of the int8 planes.  The real-valued coefficients
+// are split into FIVE balanced radix-254 digits
 //   gamma[i,q] = (s_q / 127) * sum_l d_l[i,q] 254^-l,   d_l in {-127..127}  (int8),
 // so the s8 x s8 -> s32 MMAs accumulate exact integer sums (|sum| <= K2 * 16 * 127 < 2^24 for K2 <= 4096) and the FP64
 // epilogue reassembles the prediction to s_q 254^-5 = 9.4e-13 s_q per coefficient (the last limb is rounded to within 1/2,
 // and one unit of it is worth (s_q / 127) 254^-4), far inside the 1e-5 parity budget.
 //
 // Orientation: samples are the MMA M dimension, the 5 x 50 digit rows are N (256, zero padded), the SNP/plane index
-// is K.  The digit rows are K-major in shared memory (wgmma B operand).  The genotype tile arrives samples-contiguous
-// (MN-major), which 8-bit wgmma cannot read from shared memory, so the A operand comes from registers.  Each consumer
-// warpgroup owns one 64-sample half of the tile and all 256 digit rows (m64n256k32).  The two threads of a lane pair
-// (lane, lane ^ 4) share 4 consecutive samples: each loads them at 4 consecutive k (one of the two k quads of the
-// fragment) as four 32-bit words, transposes the 4 x 4 bytes with byte permutes, keeps its own two samples and trades
-// the other two with its partner.  The fragments of stage s + 1 are built while the MMAs of stage s run.
+// is K: all G0 k-blocks, then all Miss k-blocks (the same 2-bit tiles again, mostly from L2).  The digit rows are K-major
+// in shared memory (wgmma B operand); the A operand comes from registers.  Each consumer warpgroup owns one 64-sample
+// half of the tile and all 256 digit rows (m64n256k32).  A warp's 16 samples are one 2-bit word of each SNP row: a thread
+// loads the words of the 8 k rows of its fragment, keeps the nibble of its two samples from each and turns the codes into
+// plane bytes with a few bit operations.  The fragments of MMA u + 1 are built while MMA u runs.
+// The epilogue also leaves per-tile column sums (sum, sum of squares) of the raw predictions for the standardisation.
 #include <stdlib.h>
 
 #include "kernels.cuh"
@@ -28,42 +30,65 @@ namespace {
 using namespace sm90;
 
 constexpr int PT_BM = 128;            // samples per CTA
-constexpr int PT_BK = 128;            // Z rows per stage
+constexpr int PT_BK = 128;            // SNP rows of one plane per stage
 constexpr int PI_BN = 256;            // digit rows (5 limbs x 50 outputs, zero padded)
 constexpr int PI_STAGES = 4;
-constexpr int PI_A_BYTES = PT_BK * PT_BM;          // 16 KiB: 128 k-rows x 128 samples
+constexpr int PI_A_WORDS = PT_BM / 16;             // 2-bit words per SNP row of a sample tile
+constexpr int PI_A_BYTES = PT_BK * PI_A_WORDS * 4; // 4 KiB: 128 SNP rows x 128 samples of 2-bit codes
 constexpr int PI_B_BYTES = PI_BN * PT_BK;          // 32 KiB: 256 digit rows x 128 k bytes
 constexpr int PI_STAGE_BYTES = PI_A_BYTES + PI_B_BYTES;
 constexpr int PI_THREADS = 288;                    // 2 consumer warpgroups (samples 0-63 / 64-127), 1 TMA warp
 constexpr int PI_QH = kLimbQI8 / 2;                // outputs per epilogue thread (25)
 constexpr int PI_LDE = PI_BN + 1;                  // row stride (int32) of the staged accumulator tile
+constexpr int PI_LDV = PT_BM + 1;                  // row stride (double) of the staged prediction tile
+constexpr int PI_MAX_ROWS = 2048;                  // rows_p bound of the INT8 route (2 rows_p <= 4096)
 static_assert(kLimbsI8 * kLimbQI8 <= PI_BN && kLimbQI8 % 2 == 0, "INT8 prediction layout");
 static_assert(PT_BM * PI_LDE * 4 <= PI_STAGES * PI_STAGE_BYTES, "the accumulator tile reuses the stage buffers");
-
-// 4 words W_i = bytes (k = i; samples 0..3)  ->  V_j = bytes (k = 0..3; sample j)
-__device__ __forceinline__ void transpose4x4(const uint32_t (&w)[4], uint32_t (&v)[4]) {
-  const uint32_t t0 = __byte_perm(w[0], w[1], 0x5140), t1 = __byte_perm(w[0], w[1], 0x7362);
-  const uint32_t t2 = __byte_perm(w[2], w[3], 0x5140), t3 = __byte_perm(w[2], w[3], 0x7362);
-  v[0] = __byte_perm(t0, t2, 0x5410);
-  v[1] = __byte_perm(t0, t2, 0x7632);
-  v[2] = __byte_perm(t1, t3, 0x5410);
-  v[3] = __byte_perm(t1, t3, 0x7632);
-}
+static_assert((kLimbQI8 * PI_LDV + 4 * kLimbQI8) * 8 <= PI_STAGES * PI_STAGE_BYTES, "so does the prediction tile");
 
 }  // namespace
 
-// digit rows  dig[f][g][l*50 + qq][k]  (int8), scales s[f][q].  grid: (Qp, K folds), block 256.
+// Everything the INT8 prediction needs from the solution column of one output q = r P + p and fold f, in one CTA:
+//   gam[f][i][q] = beta[m=(f,r)][p][i] * inv_sd[i],  gmu = gam * mu   (rows bs..rows_p zero),
+//   cvec[f][q][c] = sum_i gam[f][i][q] Bv[i][c]                       (256-thread stride loop, fixed-order tree),
+//   scale[f][q] = s = the largest |gam|, |gmu| of the column (1 if it is all zero),
+//   dig[f][g][l*50 + qq][k] = the balanced radix-254 digits l of 127 v / s, v = gam (k < rows_p) or gmu (k >= rows_p).
+// The values, the order of every sum and the digits are those of l0_gamma_kernel + l0_cvec_kernel, which the FP64 route
+// still runs.  grid: (Q, K folds), block 256.
 __global__ void __launch_bounds__(256)
-l0_gamma_limbs_i8_kernel(const double* __restrict__ gam, const double* __restrict__ gmu, int Qp, int Q, int bs,
-                         int rows_p, double* __restrict__ scale, uint8_t* __restrict__ dig, int ngroups) {
+l0_coef_i8_kernel(const double* __restrict__ cm, int64_t cm_stride, int ldc, int nC, int R, int P, int Qp, int bs,
+                  int rows_p, const double* __restrict__ mu, const double* __restrict__ inv_sd,
+                  const double* __restrict__ Bv, int C, double* __restrict__ gam, double* __restrict__ gmu,
+                  double* __restrict__ cvec, double* __restrict__ scale, uint8_t* __restrict__ dig, int ngroups) {
+  __shared__ double sg[PI_MAX_ROWS], sm[PI_MAX_ROWS];
   __shared__ double red[256];
   const int q = blockIdx.x, f = blockIdx.y;
-  if (q >= Q) return;
-  const double* gcol = gam + (int64_t)f * rows_p * Qp + q;
-  const double* mcol = gmu + (int64_t)f * rows_p * Qp + q;
+  const int r = q / P, p = q % P;
+  const double* x = cm + (int64_t)(f * R + r) * cm_stride + (int64_t)(nC + p) * ldc;
+  double* gcol = gam + (int64_t)f * rows_p * Qp + q;
+  double* mcol = gmu + (int64_t)f * rows_p * Qp + q;
   double mx = 0.0;
-  for (int i = threadIdx.x; i < bs; i += 256)
-    mx = fmax(mx, fmax(fabs(gcol[(int64_t)i * Qp]), fabs(mcol[(int64_t)i * Qp])));
+  for (int i = threadIdx.x; i < rows_p; i += 256) {
+    const double v = i < bs ? x[i] * inv_sd[i] : 0.0;
+    const double vm = v * mu[i];
+    gcol[(int64_t)i * Qp] = v;
+    mcol[(int64_t)i * Qp] = vm;
+    sg[i] = v;
+    sm[i] = vm;
+    if (i < bs) mx = fmax(mx, fmax(fabs(v), fabs(vm)));
+  }
+  for (int c = 0; c < C; ++c) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < bs; i += 256) s += sg[i] * Bv[(int64_t)i * C + c];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+      if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) cvec[((int64_t)f * Qp + q) * C + c] = red[0];
+    __syncthreads();
+  }
   red[threadIdx.x] = mx;
   __syncthreads();
   for (int o = 128; o > 0; o >>= 1) {
@@ -78,7 +103,7 @@ l0_gamma_limbs_i8_kernel(const double* __restrict__ gam, const double* __restric
   for (int k = threadIdx.x; k < K2; k += 256) {
     const int plane = k >= rows_p, i = plane ? k - rows_p : k;
     double v = 0.0;
-    if (i < bs) v = (plane ? mcol[(int64_t)i * Qp] : gcol[(int64_t)i * Qp]) / s * 127.0;
+    if (i < bs) v = (plane ? sm[i] : sg[i]) / s * 127.0;
 #pragma unroll
     for (int l = 0; l < kLimbsI8; ++l) {
       const double d = rint(v);                    // |v| <= 127: the remainder (<= 1/2) x 254 stays in range
@@ -90,34 +115,41 @@ l0_gamma_limbs_i8_kernel(const double* __restrict__ gam, const double* __restric
 
 // grid: (Npad / 128 sample tiles, q groups); 288 threads.
 __global__ void __launch_bounds__(PI_THREADS, 1)
-l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_constant__ CUtensorMap tmD, PredictTcArgs a) {
+l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmD, PredictTcArgs a) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gen_base = smem_raw + (base - raw);
-  const uint32_t sA = base;                                         // [NST][16 KiB]
-  const uint32_t sB = base + PI_STAGES * PI_A_BYTES;                // [NST][32 KiB]
+  const uint32_t sB = base;                                         // [NST][32 KiB], 1 KiB aligned (128B swizzle)
+  const uint32_t sA = base + PI_STAGES * PI_B_BYTES;                // [NST][4 KiB]
   uint64_t* bars = reinterpret_cast<uint64_t*>(gen_base + PI_STAGES * PI_STAGE_BYTES);
   const uint32_t full_bar = smem_u32(bars);
   const uint32_t empty_bar = smem_u32(bars + PI_STAGES);
   double* s_scale = reinterpret_cast<double*>(bars + 2 * PI_STAGES);   // [kLimbQI8]
   double* s_cvec = s_scale + kLimbQI8;                                  // [kLimbQI8][C]
+  double** s_dst = reinterpret_cast<double**>(s_cvec + kLimbQI8 * a.C);                     // [kLimbQI8] W columns
+  const uint8_t** s_msk = reinterpret_cast<const uint8_t**>(s_cvec + kLimbQI8 * (a.C + 1));  // [kLimbQI8] mask rows
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role
   const int tile = blockIdx.x, g = blockIdx.y;
   const int f = a.tile_fold[tile];
-  const int nkb = (2 * a.rows_p) / PT_BK;
+  const int nkh = a.rows_p / PT_BK;                 // k-blocks per plane
+  const int nkb = 2 * nkh;
   const int q0 = g * kLimbQI8;
   const int nq = min(kLimbQI8, a.Q - q0);
 
   if (warp == 8 && lane == 0) {
     for (int s = 0; s < PI_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }
     fence_barrier_init();
-    prefetch_tmap(&tmZ);
+    prefetch_tmap(&tmG);
     prefetch_tmap(&tmD);
   }
-  for (int e = threadIdx.x; e < kLimbQI8; e += PI_THREADS)
-    s_scale[e] = (e < nq) ? a.scale[(int64_t)f * a.Qp + q0 + e] / 127.0 : 0.0;
+  for (int e = threadIdx.x; e < kLimbQI8; e += PI_THREADS) {
+    const int q = q0 + e, r = q / a.P, p = q % a.P;
+    s_scale[e] = (e < nq) ? a.scale[(int64_t)f * a.Qp + q] / 127.0 : 0.0;
+    s_dst[e] = (e < nq) ? a.W[p] + (int64_t)(a.col0 + r) * a.npad : nullptr;
+    s_msk[e] = (e < nq) ? a.mask + (int64_t)p * a.npad : nullptr;
+  }
   for (int e = threadIdx.x; e < kLimbQI8 * a.C; e += PI_THREADS) {
     const int qq = e / a.C, c = e % a.C;
     s_cvec[e] = (qq < nq) ? a.cvec[((int64_t)f * a.Qp + q0 + qq) * a.C + c] : 0.0;
@@ -126,14 +158,15 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
 
   if (warp == 8) {
     if (lane == 0) {
-      // ===== TMA producer: A = 128 plane rows x 128 samples; B = 256 digit rows x 128 k bytes =====
+      // ===== TMA producer: A = 128 SNP rows x 8 words (128 samples) of 2-bit codes, the G0 rows and then the same rows
+      // for the Miss plane; B = 256 digit rows x 128 k bytes =====
       const int drow0 = (f * a.ngroups + g) * PI_BN;
       for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb % PI_STAGES;
         const uint32_t ph = (kb / PI_STAGES) & 1;
         mbar_wait(empty_bar + 8 * s, ph ^ 1);
         mbar_expect_tx(full_bar + 8 * s, PI_STAGE_BYTES);
-        tma_load_2d(sA + s * PI_A_BYTES, &tmZ, full_bar + 8 * s, tile * PT_BM, kb * PT_BK);
+        tma_load_2d(sA + s * PI_A_BYTES, &tmG, full_bar + 8 * s, tile * PI_A_WORDS, (kb % nkh) * PT_BK);
         tma_load_2d(sB + s * PI_B_BYTES, &tmD, full_bar + 8 * s, kb * PT_BK, drow0);
         tma_load_2d(sB + s * PI_B_BYTES + 16384, &tmD, full_bar + 8 * s, kb * PT_BK, drow0 + 128);
       }
@@ -142,39 +175,40 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
   }
 
   // ===== consumers: warpgroup wg = samples 64 wg .. 64 wg + 63 x all 256 digit rows =====
-  // Thread (warp w of the warpgroup, lane l, r = l / 4, t4 = l % 4) holds fragment rows 16 w + r and 16 w + r + 8, which
-  // are samples 64 wg + 16 w + 2 r and the next one.  The pair (r, r ^ 1) shares the 4 samples from sq = 64 wg + 16 w +
-  // 4 (r / 2): the even thread loads them at the k quad 4 t4 .. +3 of each MMA, the odd one at 16 + 4 t4 .. +3.
+  // Thread (warp w of the warpgroup, lane l, r = l / 4, t4 = l % 4) holds fragment rows r and r + 8 of its warp's 16,
+  // which are the samples 2 r and 2 r + 1 of the warp's 16 (from 64 wg + 16 w): the nibble at bit 4 r of word 4 wg + w
+  // of each SNP row.  Its k are the quads 4 t4 .. +3 and 16 + 4 t4 .. +3 of each MMA's 32.  At load j, lane t4 reads row
+  // 4 t4 + (j + t4) % 4 of its quad, so the four t4 of an instruction meet four distinct banks and the eight lanes of
+  // each t4 read one word (broadcast); qsel undoes the rotation.
   const int wg = warp >> 2, w = warp & 3, r = lane >> 2, t4 = lane & 3;
-  const bool odd = r & 1;
-  const int sq = 64 * wg + 16 * w + 4 * (r >> 1);
-  // The 8 lanes reading one 16-byte sample chunk take the 4 k rows of their quad in rotated orders (rot = 0..3), so each
-  // load instruction of the warp meets 8 distinct swizzle phases, i.e. 32 distinct banks.  rsel undoes the rotation.
-  const int rot = 2 * odd + (t4 >> 1);
-  const uint32_t rsel = (0x32103210u >> (16 - 4 * rot)) & 0xFFFFu;
-  int aoff[4];                                      // byte offset of load i inside a 32-k slice of the A stage
+  int aoff[4];                                      // byte offset of load j inside a 16-row quad slice of the A stage
+  uint32_t qsel = 0;                                // byte k of a quad comes from load (k - t4) % 4
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int kr = 16 * odd + 4 * t4 + ((i + rot) & 3);          // row of the 128B-swizzled tile
-    aoff[i] = kr * 128 + ((((sq >> 4) ^ (kr & 7)) << 4) | (sq & 15));
+  for (int j = 0; j < 4; ++j) {
+    aoff[j] = (4 * t4 + ((j + t4) & 3)) * (PI_A_WORDS * 4) + (4 * wg + w) * 4;
+    const int src = (j - t4) & 3;                   // for byte k = j
+    qsel |= (uint32_t)((src & 1) | ((src >> 1) << 2)) << (4 * j);
   }
-  const uint8_t* gA = gen_base;                     // generic view of the A stages
+  const uint32_t bsel = (uint32_t)(r >> 1) | ((uint32_t)(4 + (r >> 1)) << 4);   // byte r / 2 of two words
+  const int nsh = 4 * (r & 1);                                                   // nibble of that byte
+  const uint8_t* gA = gen_base + PI_STAGES * PI_B_BYTES;   // generic view of the A stages
 
-  // A fragment of MMA kk of stage s: {row, row + 8} x {k 4 t4 .. +3, k 16 + 4 t4 .. +3} of the stage's 32-k slice kk
-  auto build = [&](int s, int kk, uint32_t (&af)[4]) {
-    uint32_t wv[4], v[4];
+  // A fragment of MMA kk of stage s: {sample 2 r, 2 r + 1} x {k 4 t4 .. +3, k 16 + 4 t4 .. +3} of the stage's 32-k slice
+  // kk, as the plane bytes of bed_expand_fp8_kernel: G0 = 8 x code (0 for code 3), Miss = 8 x (code == 3).
+  auto build = [&](int s, int kk, bool miss, uint32_t (&af)[4]) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
-      wv[i] = *reinterpret_cast<const uint32_t*>(gA + s * PI_A_BYTES + kk * 32 * 128 + aoff[i]);
-    transpose4x4(wv, v);                            // v[j] = sample sq + j at the quad's k, rotated by rot bytes
+    for (int h = 0; h < 2; ++h) {
+      const uint8_t* src = gA + s * PI_A_BYTES + (kk * 32 + 16 * h) * (PI_A_WORDS * 4);
+      uint32_t t[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = __byte_perm(v[j], 0, rsel);
-    const uint32_t x0 = __shfl_xor_sync(0xffffffffu, odd ? v[0] : v[2], 4);
-    const uint32_t x1 = __shfl_xor_sync(0xffffffffu, odd ? v[1] : v[3], 4);
-    af[0] = odd ? x0 : v[0];
-    af[1] = odd ? x1 : v[1];
-    af[2] = odd ? v[2] : x0;
-    af[3] = odd ? v[3] : x1;
+      for (int j = 0; j < 4; ++j) t[j] = *reinterpret_cast<const uint32_t*>(src + aoff[j]);
+      // byte k: the codes of samples 2 r (bits 0-1) and 2 r + 1 (bits 2-3) at k, other samples' codes above
+      const uint32_t y = __byte_perm(__byte_perm(t[0], t[1], bsel), __byte_perm(t[2], t[3], bsel), qsel) >> nsh;
+      const uint32_t c0 = y & 0x03030303u, c1 = (y >> 2) & 0x03030303u;
+      const uint32_t m0 = c0 & (c0 >> 1), m1 = c1 & (c1 >> 1);     // 1 in the bytes of missing calls (code 3)
+      af[2 * h] = miss ? m0 << 3 : (c0 ^ (m0 * 3u)) << 3;
+      af[2 * h + 1] = miss ? m1 << 3 : (c1 ^ (m1 * 3u)) << 3;
+    }
   };
   // One commit group per MMA, two fragment register sets: while MMA u runs, MMA u - 1 is retired (freeing its fragment
   // registers, and at the first MMA of a stage the previous stage's buffers) and the fragment of MMA u + 1 is built.
@@ -186,9 +220,10 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
   fence_regs(acc);
   uint32_t afr[2][4];
   mbar_wait(full_bar, 0);
-  build(0, 0, afr[0]);
+  build(0, 0, false, afr[0]);
   for (int kb = 0; kb < nkb; ++kb) {
     const int s = kb % PI_STAGES;
+    const bool miss = kb >= nkh;
     const uint64_t db = desc_k128(sB + s * PI_B_BYTES);
 #pragma unroll
     for (int kk = 0; kk < PT_BK / 32; ++kk) {
@@ -199,10 +234,10 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
       wgmma_wait<1>();
       if (kk == 0 && kb > 0 && w == 0 && lane == 0) mbar_arrive(empty_bar + 8 * ((kb - 1) % PI_STAGES));
       if (kk + 1 < PT_BK / 32) {
-        build(s, kk + 1, afr[(kk + 1) & 1]);
+        build(s, kk + 1, miss, afr[(kk + 1) & 1]);
       } else if (kb + 1 < nkb) {
         mbar_wait(full_bar + 8 * ((kb + 1) % PI_STAGES), ((kb + 1) / PI_STAGES) & 1);
-        build((kb + 1) % PI_STAGES, 0, afr[0]);
+        build((kb + 1) % PI_STAGES, 0, kb + 1 >= nkh, afr[0]);
       }
     }
   }
@@ -214,6 +249,8 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
   // FP64 Horner from the lowest limb up.
   named_sync(1, 256);
   int32_t* E = reinterpret_cast<int32_t*>(gen_base);
+  double* V = reinterpret_cast<double*>(gen_base);           // [kLimbQI8][PI_LDV], written once E is read
+  double* Vs = V + kLimbQI8 * PI_LDV;                          // [2 sample halves][kLimbQI8][2]
 #pragma unroll
   for (int i = 0; i < 128; ++i) {
     const int smp = 64 * wg + 16 * w + 2 * r + ((i >> 1) & 1);
@@ -221,11 +258,19 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
     E[smp * PI_LDE + col] = acc[i];
   }
   named_sync(1, 256);
+  const int ct = threadIdx.x;                      // 0..255
+  const int half = ct >> 7;                        // warps 0-3: outputs 0-24, warps 4-7: outputs 25-49
   {
-    const int ct = threadIdx.x;                    // 0..255
-    const int smp = ct & 127, half = ct >> 7;
+    const int smp = ct & 127;
     const int t = tile * PT_BM + smp;
     const int32_t* er = E + smp * PI_LDE + half * PI_QH;
+    // every global load of the epilogue is issued here, ahead of the stores below, so that the 25 mask rows cost one
+    // memory latency rather than one each (the compiler may not move a load across a store through another pointer)
+    uint32_t mk[PI_QH];
+#pragma unroll
+    for (int j = 0; j < PI_QH; ++j) mk[j] = (half * PI_QH + j < nq) ? s_msk[half * PI_QH + j][t] : 0u;
+    double xr[kMaxCov];
+    for (int c = 0; c < a.C; ++c) xr[c] = a.xy[(int64_t)t * a.cpp + c];
     const double inv254 = 1.0 / 254.0;
     double accd[PI_QH];
 #pragma unroll
@@ -235,25 +280,47 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
 #pragma unroll
       for (int j = 0; j < PI_QH; ++j) accd[j] = fma(accd[j], inv254, (double)(er[l * kLimbQI8 + j] >> 3));
     }
-    double xr[kMaxCov];
-    for (int c = 0; c < a.C; ++c) xr[c] = a.xy[(int64_t)t * a.cpp + c];
 #pragma unroll
     for (int j = 0; j < PI_QH; ++j) {
       const int qq = half * PI_QH + j;
+      double val = 0.0;
       if (qq < nq) {
-        const int q = q0 + qq;
-        const int r = q / a.P, p = q % a.P;
-        double val = accd[j] * s_scale[qq];
+        val = accd[j] * s_scale[qq];
         for (int c = 0; c < a.C; ++c) val -= xr[c] * s_cvec[qq * a.C + c];
-        val *= (double)a.mask[(int64_t)p * a.npad + t];
-        a.W[p][(int64_t)(a.col0 + r) * a.npad + t] = val;
+        val *= (double)mk[j];
+        s_dst[qq][t] = val;
       }
+      accd[j] = val;
     }
+    // column sums of the tile (sum, sum of squares) in a fixed order: the values go through shared memory (over E, once
+    // every thread has read its row), transposed to V[output][sample]; thread (output, half of the samples) sums 64 of
+    // them in sample order, and the two halves are added
+    named_sync(1, 256);
+#pragma unroll
+    for (int j = 0; j < PI_QH; ++j) V[(half * PI_QH + j) * PI_LDV + smp] = accd[j];
+  }
+  named_sync(1, 256);
+  if (ct < 2 * kLimbQI8) {
+    const int qq = ct % kLimbQI8, sh = ct / kLimbQI8;
+    const double* v = V + qq * PI_LDV + sh * (PT_BM / 2);
+    double s1 = 0.0, s2 = 0.0;
+#pragma unroll 8
+    for (int i = 0; i < PT_BM / 2; ++i) {
+      s1 += v[i];
+      s2 = fma(v[i], v[i], s2);
+    }
+    Vs[(sh * kLimbQI8 + qq) * 2 + 0] = s1;
+    Vs[(sh * kLimbQI8 + qq) * 2 + 1] = s2;
+  }
+  named_sync(1, 256);
+  if (ct < nq) {
+    a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 0] = Vs[ct * 2 + 0] + Vs[(kLimbQI8 + ct) * 2 + 0];
+    a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 1] = Vs[ct * 2 + 1] + Vs[(kLimbQI8 + ct) * 2 + 1];
   }
 }
 
-// Column sums of the raw predictions for the standardisation: part[chunk][q] = (sum, sum of squares) over
-// a chunk of 8192 samples, fixed-order tree reduction.  grid: (Q, nchunks), block 256.
+// Column sums of predictions that no prediction kernel summed (the dense route of l0_dense.cu): part[chunk][q] =
+// (sum, sum of squares) over a chunk of 8192 samples, fixed-order tree reduction.  grid: (Q, nchunks), block 256.
 __global__ void __launch_bounds__(256)
 l0_colsum_kernel(double* const* __restrict__ W, int64_t npad, int col0, int P, int Qp,
                  double* __restrict__ part) {
@@ -318,18 +385,34 @@ void make_byte_tensor_map(CUtensorMap* tm, const uint8_t* basep, int64_t inner, 
 
 size_t predict_i8_dig_bytes(int K, int ngroups, int rows_p) { return (size_t)K * ngroups * PI_BN * 2 * rows_p; }
 
-void launch_l0_gamma_limbs_i8(const double* gam, const double* gmu, int Qp, int Q, int bs, int rows_p, int K,
-                              double* scale, uint8_t* dig, int ngroups, cudaStream_t s) {
-  dim3 grid(Qp, K);
-  l0_gamma_limbs_i8_kernel<<<grid, 256, 0, s>>>(gam, gmu, Qp, Q, bs, rows_p, scale, dig, ngroups);
+// 2-bit rows [rows][words_per_row] (uint32) with an 8-word x 128-row box (128 samples x 128 SNPs), no swizzle
+void make_gp_tensor_map(CUtensorMap* tm, const uint32_t* gp, int64_t words_per_row, int64_t rows) {
+  const cuuint64_t gdim[2] = {(cuuint64_t)words_per_row, (cuuint64_t)rows};
+  const cuuint64_t gstride[1] = {(cuuint64_t)words_per_row * 4};
+  const cuuint32_t box[2] = {(cuuint32_t)PI_A_WORDS, (cuuint32_t)PT_BK};
+  const cuuint32_t estr[2] = {1, 1};
+  CUresult r = pt_encode_fn()(tm, CU_TENSOR_MAP_DATA_TYPE_UINT32, 2, const_cast<uint32_t*>(gp), gdim, gstride, box,
+                              estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  RG_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")");
 }
 
-void launch_l0_predict_i8(const CUtensorMap& tmZ, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
+void launch_l0_coef_i8(const double* cm, int64_t cm_stride, int ldc, int nC, int R, int P, int Q, int Qp, int bs,
+                       int rows_p, int K, const double* mu, const double* inv_sd, const double* Bv, int C, double* gam,
+                       double* gmu, double* cvec, double* scale, uint8_t* dig, int ngroups, cudaStream_t s) {
+  RG_CHECK(rows_p <= PI_MAX_ROWS, "INT8 prediction: rows_p <= 2048");
+  dim3 grid(Q, K);
+  l0_coef_i8_kernel<<<grid, 256, 0, s>>>(cm, cm_stride, ldc, nC, R, P, Qp, bs, rows_p, mu, inv_sd, Bv, C, gam, gmu, cvec,
+                                         scale, dig, ngroups);
+}
+
+void launch_l0_predict_i8(const CUtensorMap& tmG, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
                           cudaStream_t s) {
   RG_CHECK(2 * a.rows_p <= 4096, "INT8 prediction: 2 * rows_p <= 4096 (int32 Horner bound)");
-  const size_t smem = (size_t)PI_STAGES * PI_STAGE_BYTES + 1024 + 128 + ((size_t)kLimbQI8 * (1 + a.C)) * sizeof(double);
+  const size_t smem = (size_t)PI_STAGES * PI_STAGE_BYTES + 1024 + 128 +
+                      ((size_t)kLimbQI8 * (3 + a.C)) * sizeof(double);   // scales, cvec, 2 pointers
   ensure_dyn_smem(reinterpret_cast<const void*>(l0_predict_i8_kernel), smem);
-  l0_predict_i8_kernel<<<dim3(ntiles, a.ngroups), PI_THREADS, smem, s>>>(tmZ, tmD, a);
+  l0_predict_i8_kernel<<<dim3(ntiles, a.ngroups), PI_THREADS, smem, s>>>(tmG, tmD, a);
 }
 
 }  // namespace rg

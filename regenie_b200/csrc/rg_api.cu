@@ -399,8 +399,6 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
   const int C = h->C, P = h->P, K = h->K, R = h->R;
   const int64_t Npad = h->Npad;
   ScopedTimer t(h, "l0_predict", s);
-  launch_l0_gamma(xsrc, xstride, xld, xrow0, R, P, d.Qp, d.bs, d.rows_p, K, L.mu.p, L.inv_sd.p, L.Bv.p, C,
-                  L.gam.p, L.gmu.p, L.cvec.p, s);
   // raw predictions go to the lane's LOCAL scratch; the standardisation pass reads them there and writes the finished
   // columns into W - the owner's HBM, which may be another GPU's (then only plain stores cross NVLink)
   if (L.wraw.n < (size_t)P * R * Npad) {
@@ -416,14 +414,17 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
   pa.col0 = 0; pa.npad = Npad; pa.words_per_row = Npad / 16;
   pa.gp = L.gp.p; pa.tile_fold = h->tile_fold.p; pa.gam = L.gam.p; pa.gmu = L.gmu.p;
   pa.cvec = L.cvec.p; pa.xy = h->xy.p; pa.mask = h->mask.p; pa.W = L.wraw_tab.p; pa.part = L.part.p;
-  int nparts = d.ntiles_s;
-  // INT8 tensor cores (s8 wgmma, 5 radix-254 limbs) up to 2 rows_p = 4096; the FP64 CUDA-core kernel beyond (bsize > 2048)
+  // INT8 tensor cores (s8 wgmma, 5 radix-254 limbs) up to 2 rows_p = 4096; the FP64 CUDA-core kernel beyond (bsize > 2048).
+  // Both leave per-tile column sums in L.part.
   const bool use_i8 = 2 * d.rows_p <= 4096;
   L.last_pred_i8 = use_i8 ? 1 : 0;
   if (!use_i8) {
+    launch_l0_gamma(xsrc, xstride, xld, xrow0, R, P, d.Qp, d.bs, d.rows_p, K, L.mu.p, L.inv_sd.p, L.Bv.p, C,
+                    L.gam.p, L.gmu.p, L.cvec.p, s);
     launch_l0_predict(pa, d.ntiles_s, s);
+    h->launches += 3;
   } else {
-    // exact tensor-core path: digit rows of gamma against the genotype operand planes
+    // exact tensor-core path: digit rows of gamma against the genotype planes, decoded from the 2-bit rows
     const int ngroups = (int)ceil_div(d.Q, kLimbQI8);
     const int drows_per_group = 256;
     const size_t need = predict_i8_dig_bytes(K, ngroups, h->rows_p_max);
@@ -438,18 +439,23 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
       make_byte_tensor_map(&tm, L.dig.p, 2 * d.rows_p, (int64_t)K * ngroups * drows_per_group);
       L.dmaps[d.rows_p] = tm;
     }
-    launch_l0_gamma_limbs_i8(L.gam.p, L.gmu.p, d.Qp, d.Q, d.bs, d.rows_p, K, L.dscale.p, L.dig.p, ngroups, s);
+    if (!L.gmaps.count(d.rows_p)) {
+      CUtensorMap tm;
+      make_gp_tensor_map(&tm, L.gp.p, Npad / 16, d.rows_p);
+      L.gmaps[d.rows_p] = tm;
+    }
+    launch_l0_coef_i8(xsrc, xstride, xld, xrow0, R, P, d.Q, d.Qp, d.bs, d.rows_p, K, L.mu.p, L.inv_sd.p, L.Bv.p, C,
+                      L.gam.p, L.gmu.p, L.cvec.p, L.dscale.p, L.dig.p, ngroups, s);
     PredictTcArgs ta;
     ta.rows_p = d.rows_p; ta.C = C; ta.P = P; ta.Q = d.Q; ta.Qp = d.Qp; ta.cpp = h->cpp; ta.col0 = 0; ta.ngroups = ngroups;
     ta.npad = Npad; ta.tile_fold = h->tile_fold.p; ta.scale = L.dscale.p; ta.cvec = L.cvec.p;
     ta.xy = h->xy.p; ta.mask = h->mask.p; ta.W = L.wraw_tab.p; ta.part = L.part.p;
-    launch_l0_predict_i8(L.tmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
-    nparts = launch_l0_colsum(L.wraw_tab.p, Npad, 0, P, d.Q, d.Qp, L.part.p, s);
+    launch_l0_predict_i8(L.gmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
     h->launches += 2;
   }
-  launch_l0_standardize(L.part.p, nparts, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, h->W_tab.p, Npad, d.col0,
+  launch_l0_standardize(L.part.p, d.ntiles_s, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, h->W_tab.p, Npad, d.col0,
                         h->is_real.p, s, L.wraw_tab.p, 0);
-  h->launches += 5;
+  h->launches += 2;
 }
 
 static BlockDims block_dims(const rg_ctx* h, int bs, int block_id) {
