@@ -15,8 +15,11 @@
 //     system streaming L once per sweep (mx_trisolve_kernel); a refinement step is one FP64 residual pass + one such solve.
 //
 // Storage per lane (n = round_up(bs, 128), nmat = K*R):
-//   Lp, Wp         : [nmat][2][n][n] FP32 hi/lo planes (L / P in place; diagonal tiles of Wp = M_k for the TRSM tiles)
-//   Lplain, Mplain : [nmat][n][n] L as one FP32 plane (off-diagonal tiles), [nmat][n/128][128][128] the M_k
+//   Lplain         : [nmat][n][n] FP32, the factor in place: tile (i,k), i >= k, holds P_ik and then L_ik; tile (k,i) above
+//                    the diagonal holds L_ik^T for the backward substitution.  The TF32 hi/lo pairs the tensor cores
+//                    multiply are formed from it inside the GEMM tiles and never stored.
+//   Mplain, MTplain: [nmat][n/128][128][128] the M_k = L_kk^-1 and their transposes
+//   Ap             : [K][n][n] the fold systems in FP32 (the C operand of the update tiles)
 //   Af             : [K][n][n] FP64 full symmetric fold systems WITHOUT the ridge shift (l0_assemble_sym_kernel)
 //   bvec, xvec, rvec : [.][Pp][n] FP64 right-hand sides (per fold), solutions and residuals (per system)
 #include <algorithm>
@@ -49,26 +52,15 @@ __device__ __forceinline__ void blk_nt(float (&acc)[PB], const float* __restrict
   }
 }
 
-__device__ __forceinline__ float tf32_rn(float x) {
-  uint32_t t;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x));
-  return __uint_as_float(t);
-}
-__device__ __forceinline__ void split_store(const float4 v, float* hp, float* lp, float4& hi) {
-  hi = make_float4(tf32_rn(v.x), tf32_rn(v.y), tf32_rn(v.z), tf32_rn(v.w));
-  *reinterpret_cast<float4*>(hp) = hi;
-  *reinterpret_cast<float4*>(lp) = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
-}
-
 }  // namespace
 
 // Diagonal tile of panel step k:  L_kk = chol(P_kk)  and  M = L_kk^-1  (FP32), one CTA per system.
-//   in : Lp tile (k,k) = P_kk (hi + lo), lower part
-//   out: Lp tile (k,k) = L_kk (lower, zeros above);  Wp tile (k,k) = M;  Wt tile (k,k) = M^T   (hi / lo planes)
+//   in : Lplain tile (k,k) = P_kk, lower part
+//   out: Lplain tile (k,k) = L_kk (lower, zeros above);  Mplain tile k = M;  MTplain tile k = M^T
 // 256 threads = 8 warps; shared: S (P -> L, scratch above the diagonal blocks), Wm (M), Wq (M^T).
 __global__ void __launch_bounds__(256)
-potrf128_kernel(float* __restrict__ Lp, float* __restrict__ Wp, float* __restrict__ Mplain, float* __restrict__ MTplain,
-                int n, int k, unsigned int* __restrict__ fail_flag) {
+potrf128_kernel(float* __restrict__ Lplain, float* __restrict__ Mplain, float* __restrict__ MTplain, int n, int k,
+                unsigned int* __restrict__ fail_flag) {
   extern __shared__ float pt_sm[];
   float* S = pt_sm;
   float* Wm = pt_sm + PT * PLD;
@@ -76,17 +68,12 @@ potrf128_kernel(float* __restrict__ Lp, float* __restrict__ Wp, float* __restric
   float* dinv = pt_sm + 3 * PT * PLD;                    // reciprocal diagonal of L
   float* lcol = dinv + PT;                               // [2][PB] current column of the 32 x 32 register Cholesky
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t plane = (int64_t)n * n;
-  const int64_t moff = (int64_t)blockIdx.x * 2 * plane + (int64_t)k * PT * n + (int64_t)k * PT;
-  float* Lh = Lp + moff;
-  float* Ll = Lh + plane;
+  float* Lkk = Lplain + (int64_t)blockIdx.x * n * n + (int64_t)k * PT * n + (int64_t)k * PT;
 #pragma unroll
   for (int it = 0; it < PT * PT / 4 / 256; ++it) {          // 128-bit loads, all in flight before the first use
     const int e = threadIdx.x + 256 * it;
     const int r = e >> 5, c = (e & 31) * 4;
-    const float4 h4 = *reinterpret_cast<const float4*>(Lh + (int64_t)r * n + c);
-    const float4 l4 = *reinterpret_cast<const float4*>(Ll + (int64_t)r * n + c);
-    float4 v = make_float4(h4.x + l4.x, h4.y + l4.y, h4.z + l4.z, h4.w + l4.w);
+    float4 v = *reinterpret_cast<const float4*>(Lkk + (int64_t)r * n + c);
     if (c + 0 > r) v.x = 0.f;
     if (c + 1 > r) v.y = 0.f;
     if (c + 2 > r) v.z = 0.f;
@@ -224,9 +211,7 @@ potrf128_kernel(float* __restrict__ Lp, float* __restrict__ Wp, float* __restric
     }
     __syncthreads();
   }
-  // ---- write back as hi / lo planes
-  float* Wh = Wp + moff;
-  float* Wl = Wh + plane;
+  // ---- write back
   float* Mp = Mplain + ((int64_t)blockIdx.x * (n / PT) + k) * PT * PT;       // M_k / M_k^T as FP32 tiles for the substitutions
   float* MTp = MTplain + ((int64_t)blockIdx.x * (n / PT) + k) * PT * PT;
 #pragma unroll 4
@@ -238,11 +223,8 @@ potrf128_kernel(float* __restrict__ Lp, float* __restrict__ Wp, float* __restric
     if (c + 1 > r) vl.y = 0.f;
     if (c + 2 > r) vl.z = 0.f;
     if (c + 3 > r) vl.w = 0.f;
-    const float4 vw = *reinterpret_cast<const float4*>(Wm + r * PLD + c);
-    float4 hi;
-    split_store(vl, Lh + (int64_t)r * n + c, Ll + (int64_t)r * n + c, hi);
-    split_store(vw, Wh + (int64_t)r * n + c, Wl + (int64_t)r * n + c, hi);
-    *reinterpret_cast<float4*>(Mp + r * PT + c) = vw;
+    *reinterpret_cast<float4*>(Lkk + (int64_t)r * n + c) = vl;
+    *reinterpret_cast<float4*>(Mp + r * PT + c) = *reinterpret_cast<const float4*>(Wm + r * PLD + c);
     *reinterpret_cast<float4*>(MTp + r * PT + c) = *reinterpret_cast<const float4*>(Wq + r * PLD + c);
   }
 }
@@ -620,9 +602,10 @@ static void build_plan(MxPlan& pl, int n) {
 
 struct MixedSolver::Impl {
   int n = 0, nmat = 0, K = 0, R = 0, Pp = 0;
-  DevBuf<float> Lp, Wp, Lplain, Mplain, MTplain, Ap, Ident;
+  DevBuf<float> Lplain, Mplain, MTplain, Ap;
   DevBuf<unsigned int> conv;
-  CUtensorMap tmL, tmW, tmAp, tmI, tmLpl, tmMpl, tmMTpl;
+  CUtensorMap tmL, tmM, tmAp;             // 128-row operand tiles of the GEMM (Lplain, Mplain, Ap)
+  CUtensorMap tmLpl, tmMpl, tmMTpl;       // 32-row sub-tiles of the substitution sweeps
   MxPlan plan;
 };
 
@@ -642,25 +625,20 @@ void MixedSolver::prepare(int n, int K, int R, int Pp) {
   RG_CHECK(n % PT == 0 && n >= PT && ((n / PT) & (n / PT - 1)) == 0 && n <= 2048,
            "mixed solver: dimension must be 128 * 2^k <= 2048");
   d.n = n; d.nmat = nmat; d.K = K; d.R = R; d.Pp = Pp;
-  const size_t planes = (size_t)nmat * 2 * n * n;
-  d.Lp.alloc(planes); d.Wp.alloc(planes);
   d.Lplain.alloc((size_t)nmat * n * n);
   d.Mplain.alloc((size_t)nmat * n * PT);
   d.MTplain.alloc((size_t)nmat * n * PT);
   make_f32_rows_tensor_map(&d.tmLpl, d.Lplain.p, n, (int64_t)nmat * n, PT, TS_SUB);
   make_f32_rows_tensor_map(&d.tmMpl, d.Mplain.p, PT, (int64_t)nmat * n, PT, TS_SUB);
   make_f32_rows_tensor_map(&d.tmMTpl, d.MTplain.p, PT, (int64_t)nmat * n, PT, TS_SUB);
-  // tiles that nothing writes (upper triangle) are read by nothing either; zero once so stale data can never matter
-  RG_CUDA(cudaMemset(d.Lp.p, 0, planes * 4));
-  RG_CUDA(cudaMemset(d.Wp.p, 0, planes * 4));
+  // every tile is written before anything reads it; zero once so stale data can never matter
   RG_CUDA(cudaMemset(d.Lplain.p, 0, (size_t)nmat * n * n * 4));
   d.conv.alloc((size_t)(kMxMaxSteps + 1) * nmat * 2);
-  make_tf32_planes_tensor_map(&d.tmL, d.Lp.p, n, nmat);
-  make_tf32_planes_tensor_map(&d.tmW, d.Wp.p, n, nmat);
-  d.Ap.alloc((size_t)K * 2 * n * n);
-  RG_CUDA(cudaMemset(d.Ap.p, 0, (size_t)K * 2 * n * n * 4));
-  make_tf32_planes_tensor_map(&d.tmAp, d.Ap.p, n, K);
-  make_tf32_identity_planes(d.Ident, &d.tmI);
+  make_tf32_operand_tensor_map(&d.tmL, d.Lplain.p, n, n, nmat);
+  make_tf32_operand_tensor_map(&d.tmM, d.Mplain.p, PT, n, nmat);
+  d.Ap.alloc((size_t)K * n * n);
+  RG_CUDA(cudaMemset(d.Ap.p, 0, (size_t)K * n * n * 4));
+  make_tf32_operand_tensor_map(&d.tmAp, d.Ap.p, n, n, K);
   build_plan(d.plan, n);
 }
 
@@ -693,24 +671,22 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
   RG_CUDA(cudaMemsetAsync(d.conv.p, 0, d.conv.n * sizeof(unsigned int), s));
   const int4* tl = d.plan.tiles.p;
   Tf32GemmEpilogue e0{};
-  e0.n = n; e0.out_mat_stride = (int64_t)n * n;
+  e0.n = n; e0.out_mat_stride = (int64_t)n * n; e0.out = d.Lplain.p;
   // ---- factorisation: left-looking, 128-wide panels
   for (int k = 0; k < nt; ++k) {
     Tf32GemmEpilogue e = e0;
-    e.out = d.Lp.p;
-    // P_ik = (A_f + lambda_r I)_ik - L_i,0:k L_k,0:k^T: the A tile enters through the tensor pipe (A_planes x identity),
+    // P_ik = (A_f + lambda_r I)_ik - L_i,0:k L_k,0:k^T: the A tile enters through the tensor pipe (A tile x identity),
     // the product with A negated, the ridge shift on the diagonal in the epilogue - no epilogue loads at all
     e.c_chunks = 4; e.c_mat_div = d.R;
     e.diag_add = lambda; e.diag_mod = d.R;
     // panel step 0 has nothing to subtract: the assembler already wrote block column 0 of every system (first_col_ready)
-    if (!(k == 0 && first_col_ready)) launch_tf32x3_gemm(d.tmL, d.tmL, tl + d.plan.upd[k].x, d.plan.upd[k].y, nmat, e, s, &d.tmAp, &d.tmI);
-    potrf128_kernel<<<nmat, 256, potrf_smem, s>>>(d.Lp.p, d.Wp.p, d.Mplain.p, d.MTplain.p, n, k, fail_flag);
+    if (!(k == 0 && first_col_ready)) launch_tf32x3_gemm(d.tmL, d.tmL, tl + d.plan.upd[k].x, d.plan.upd[k].y, nmat, e, s, &d.tmAp);
+    potrf128_kernel<<<nmat, 256, potrf_smem, s>>>(d.Lplain.p, d.Mplain.p, d.MTplain.p, n, k, fail_flag);
     if (d.plan.trsm[k].y > 0) {
-      Tf32GemmEpilogue t = e0;
-      t.out = d.Lp.p;
-      t.out_plain = d.Lplain.p;                      // the same tiles as one FP32 plane, and their transposes in the upper
+      Tf32GemmEpilogue t = e0;                       // L_ik = P_ik M_k^T in place, and its transpose into the upper
       t.mirror = 1;                                  // triangle: what the two substitution sweeps stream
-      launch_tf32x3_gemm(d.tmL, d.tmW, tl + d.plan.trsm[k].x, d.plan.trsm[k].y, nmat, t, s);
+      t.b_cols_local = 1;
+      launch_tf32x3_gemm(d.tmL, d.tmM, tl + d.plan.trsm[k].x, d.plan.trsm[k].y, nmat, t, s);
     }
   }
   // ---- x0 = (L L^T)^-1 b, then  x += (L L^T)^-1 (b - A x)  by block substitution, one CTA per system
@@ -742,12 +718,10 @@ void MixedSolver::solve(const double* Af, const double* lambda, const double* bv
 }
 
 float* MixedSolver::a_planes() { return impl->Ap.p; }
-float* MixedSolver::l_planes() { return impl->Lp.p; }
+float* MixedSolver::l_planes() { return impl->Lplain.p; }
 
 const float* MixedSolver::debug_planes(int which) const {
   switch (which) {
-    case 0: return impl->Lp.p;
-    case 1: return impl->Wp.p;
     case 2: return impl->Lplain.p;
     case 3: return impl->Mplain.p;
     default: return nullptr;

@@ -45,8 +45,8 @@ struct AssembleArgs {
   double* cm;                // batched row-major lower systems
   int64_t cm_stride;
   int ldc;
-  float* planes = nullptr;   // l0_assemble_sym only: FP32 hi / lo planes [K][2][n][n] of the same matrices (tensor-core operand)
-  float* lplanes = nullptr;  // l0_assemble_sym only: factor planes [K*R][2][n][n] of the mixed solver; their first 128 columns
+  float* planes = nullptr;   // l0_assemble_sym only: the same matrices in FP32 [K][n][n] (tensor-core operand)
+  float* lplanes = nullptr;  // l0_assemble_sym only: factor matrices [K*R][n][n] of the mixed solver; their first 128 columns
                              // receive A_f + lambda_r I (panel step 0 of the left-looking factorisation has nothing to subtract)
 };
 
@@ -88,14 +88,13 @@ size_t chol_inv_elems(int nC, int batch);
 void launch_chol_rows_backsolve(double* cm, int64_t stride, int nC, int row0, int nrows, int batch,
                                 const double* inv, cudaStream_t s);
 
-// ---- tf32_gemm.cu: batched 128x128 "NT" tiles in 3xTF32 on wgmma (operands = hi/lo FP32 planes [batch][2][n][n])
+// ---- tf32_gemm.cu: batched 128x128 "NT" tiles in 3xTF32 on wgmma (operands = FP32 matrices, split into hi/lo in the kernel)
 struct Tf32GemmEpilogue {
-  int n;                      // matrix dimension = row stride of every output
-  int64_t out_mat_stride;     // elements per plane per matrix (n * n)
-  float* out;                 // D   as hi / lo planes [batch][2][n][n], or null
-  float* out_t;               // D^T as hi / lo planes, or null
-  float* out_plain;           // D   as one FP32 plane [batch][n][n], or null
-  int mirror;                 // out_plain: also store D^T (symmetric result computed on its lower tiles)
+  int n;                      // matrix dimension = row stride of the output
+  int64_t out_mat_stride;     // elements per matrix (n * n)
+  float* out;                 // D as FP32 [batch][n][n]
+  int mirror;                 // also store D^T into the mirror tile (what the backward substitution streams)
+  int b_cols_local;           // B is [batch][n][128]: its columns count from the tile's first chunk, not from tile.z
   int negate;                 // D = -acc
   int lower_only;             // zero the strict upper part of diagonal tiles
   const double* cin;          // D = (float)(cin - acc) with FP64 matrices cin[mat / cin_mat_div][row][col], or null
@@ -106,12 +105,10 @@ struct Tf32GemmEpilogue {
   int c_chunks;               // 0, or 4: leading K chunks  acc = C_tile * I  followed by the main chunks with A negated
   int c_mat_div;              // C matrix index = mat / c_mat_div
 };
-void make_tf32_planes_tensor_map(CUtensorMap* tm, const float* planes, int n, int batch);
-void make_tf32_identity_planes(DevBuf<float>& buf, CUtensorMap* tm);
+void make_tf32_operand_tensor_map(CUtensorMap* tm, const float* base, int cols, int rows, int batch);
 void make_f32_rows_tensor_map(CUtensorMap* tm, const float* base, int cols, int64_t rows, int box_cols, int box_rows);
 void launch_tf32x3_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const int4* tiles, int ntiles, int batch,
-                        const Tf32GemmEpilogue& ep, cudaStream_t s, const CUtensorMap* tmC = nullptr,
-                        const CUtensorMap* tmI = nullptr);
+                        const Tf32GemmEpilogue& ep, cudaStream_t s, const CUtensorMap* tmC = nullptr);
 
 // ---- chol_mixed.cu: tensor-core factorisation + FP64 iterative refinement of the level-0 ridge systems
 constexpr int kMxMaxSteps = 6;
@@ -123,14 +120,14 @@ class MixedSolver {
   MixedSolver& operator=(const MixedSolver&) = delete;
   static int dim_for(int bs);                 // 128 * 2^k >= bs, or 0 when the block is too large for this path
   void prepare(int n, int K, int R, int Pp);
-  // Af [K][n][n] FP64 full symmetric (no ridge shift) and its FP32 hi / lo planes Ap [K][2][n][n], lambda [R],
+  // Af [K][n][n] FP64 full symmetric (no ridge shift) and the same in FP32, Ap [K][n][n], lambda [R],
   // bvec [K][Pp][n]; xvec / rvec [K*R][Pp][n]
   float* a_planes();                          // where the assembler writes Ap (owned by the solver, valid after prepare)
-  float* l_planes();                          // factor planes: the assembler may fill block column 0 (first_col_ready)
+  float* l_planes();                          // the factor [K*R][n][n]: the assembler may fill block column 0 (first_col_ready)
   void solve(const double* Af, const double* lambda, const double* bvec, double* xvec, double* rvec, int P, int steps,
              float tol, unsigned int* fail_flag, cudaStream_t s, bool first_col_ready = false);
   static int launches_per_solve(int n, int steps, int P);
-  const float* debug_planes(int which) const;  // 0 L, 1 W, 2 W^T (hi/lo planes), 3 X
+  const float* debug_planes(int which) const;  // 2 the factor (L below, L^T above the diagonal tiles), 3 the M_k; else null
  private:
   struct Impl;
   Impl* impl;

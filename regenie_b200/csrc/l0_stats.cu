@@ -250,12 +250,6 @@ l0_assemble_kernel(AssembleArgs a) {
 }
 
 
-__device__ __forceinline__ float tf32_round(float x) {
-  uint32_t t;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(t) : "f"(x));
-  return __uint_as_float(t);
-}
-
 // Mixed-precision solver input (chol_mixed.cu): the K fold systems  A_f = GGt - G_folds[f]  WITHOUT the ridge shift, as
 // full symmetric FP64 matrices of dimension n = a.nC (128 * 2^k; rows >= bs carry the identity), so that the refinement
 // residual is a plain row-wise matrix-vector pass and the R ridge values of a fold share one matrix.
@@ -309,8 +303,7 @@ l0_assemble_sym_kernel(AssembleArgs a) {
   }
   for (int f = 0; f < K; ++f) {
     double* out = a.cm + (int64_t)f * a.cm_stride;
-    float* ph = a.planes ? a.planes + (int64_t)f * 2 * a.cm_stride : nullptr;      // hi plane, lo plane behind it
-    float* pl = ph ? ph + a.cm_stride : nullptr;
+    float* pf = a.planes ? a.planes + (int64_t)f * a.cm_stride : nullptr;
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
       const int il = threadIdx.y * 4 + r;
@@ -319,19 +312,10 @@ l0_assemble_sym_kernel(AssembleArgs a) {
       if (i >= j) v = (i < a.bs) ? gsum[r] - gf[r][f] : (i == j ? 1.0 : 0.0);
       if (i >= j) {
         out[(int64_t)i * a.ldc + j] = v;
-        if (ph) {
-          const float hi = tf32_round((float)v);
-          ph[(int64_t)i * a.ldc + j] = hi;
-          pl[(int64_t)i * a.ldc + j] = (float)v - hi;
-        }
+        if (pf) pf[(int64_t)i * a.ldc + j] = (float)v;
         if (a.lplanes && j < 128) {          // block column 0 of every ridge system of this fold: P_i0 = (A_f + lambda_r I)_i0
-          for (int r2 = 0; r2 < a.R; ++r2) {
-            const float w = (float)(i == j ? v + a.lambda[r2] : v);
-            const float hi = tf32_round(w);
-            float* lh = a.lplanes + (int64_t)(f * a.R + r2) * 2 * a.cm_stride + (int64_t)i * a.ldc + j;
-            lh[0] = hi;
-            lh[a.cm_stride] = w - hi;
-          }
+          for (int r2 = 0; r2 < a.R; ++r2)
+            a.lplanes[(int64_t)(f * a.R + r2) * a.cm_stride + (int64_t)i * a.ldc + j] = (float)(i == j ? v + a.lambda[r2] : v);
         }
       }
       tl[il][threadIdx.x] = v;
@@ -344,11 +328,7 @@ l0_assemble_sym_kernel(AssembleArgs a) {
       if (i2 > j2) {
         const double v = tl[threadIdx.x][jl];
         out[(int64_t)j2 * a.ldc + i2] = v;
-        if (ph) {
-          const float hi = tf32_round((float)v);
-          ph[(int64_t)j2 * a.ldc + i2] = hi;
-          pl[(int64_t)j2 * a.ldc + i2] = (float)v - hi;
-        }
+        if (pf) pf[(int64_t)j2 * a.ldc + i2] = (float)v;
       }
     }
     __syncthreads();

@@ -1231,19 +1231,9 @@ int rg_dbg_mixed_solve(int32_t device, int32_t n, int32_t K, int32_t R, int32_t 
   RG_CUDA(cudaMemset(dfail.p, 0, 4));
   RG_CUDA(cudaMemcpy(dA.p, Af, dA.n * 8, cudaMemcpyHostToDevice));
   {
-    // FP32 hi / lo planes of the systems (the product path gets them from l0_assemble_sym_kernel)
-    std::vector<float> pl((size_t)K * 2 * n * n);
-    for (int f = 0; f < K; ++f)
-      for (size_t e = 0; e < (size_t)n * n; ++e) {
-        const float v = (float)Af[(size_t)f * n * n + e];
-        uint32_t u;
-        memcpy(&u, &v, 4);
-        u = (u + 0x1000u) & 0xFFFFE000u;                      // round to nearest TF32 (ties away), like cvt.rna.tf32.f32
-        float hi;
-        memcpy(&hi, &u, 4);
-        pl[((size_t)f * 2) * n * n + e] = hi;
-        pl[((size_t)f * 2 + 1) * n * n + e] = v - hi;
-      }
+    // the systems in FP32 (the product path gets them from l0_assemble_sym_kernel)
+    std::vector<float> pl((size_t)K * n * n);
+    for (size_t e = 0; e < pl.size(); ++e) pl[e] = (float)Af[e];
     RG_CUDA(cudaMemcpy(mx.a_planes(), pl.data(), pl.size() * 4, cudaMemcpyHostToDevice));
   }
   RG_CUDA(cudaMemcpy(dl.p, lambda, R * 8, cudaMemcpyHostToDevice));
