@@ -65,6 +65,12 @@ struct rg_ctx {
     rg::DevBuf<uint32_t> gp;          // [rows_p][Npad/16]
     rg::DevBuf<uint8_t> z;            // [2 rows_p][Npad] int8
     rg::DevBuf<float> zz;             // [K][2 rows_p][2 rows_p]
+    // sparse Miss rows of zz (miss_gram.cu): missing-call total of the block (> miss_cap = dense tiles), list segments
+    // [K][rows_p] (offset, count), sample lists, the block as sample-major 2-bit rows [Npad][rows_p / 16]
+    rg::DevBuf<unsigned long long> miss_total;
+    rg::DevBuf<int2> miss_seg;
+    rg::DevBuf<int32_t> miss_list;
+    rg::DevBuf<uint32_t> gt;
     rg::DevBuf<float> tstat;          // [K][2 rows_p][stat_drows] exact digit sums of the statistics tiles
     rg::DevBuf<int32_t> cnt_part, cnt_fold;
     rg::DevBuf<double> sum_part, sum_fold;
@@ -93,6 +99,7 @@ struct rg_ctx {
     // kernels that produced this lane's last block (rg_debug_fetch "paths"): INT8 (1) or FP64 (0) prediction; the
     // mixed solver's dimension, or 0 when the FP64 Cholesky solved it
     int last_pred_i8 = 0, last_mx_n = 0;
+    bool last_gram_dense = false;                 // RG_B200_GRAM=dense: the Miss rows ran as dense tiles unconditionally
   };
   std::vector<std::unique_ptr<Lane>> lanes;
   int next_lane = 0, last_lane = 0;
@@ -192,6 +199,11 @@ struct rg_ctx {
   rg::DevBuf<int8_t> bt_ym, firth_cflag;
   rg::DevBuf<int2> bt_cnt_part;      // [chunk][rows_p] non-zero / hom-alt counts of the dosage statistics kernel
   rg::DevBuf<int32_t> firth_sel, firth_status;
+
+  // ---- Miss rows of the level-0 Gram: sparse sums up to miss_cap missing calls per block, or always the dense tiles
+  //      (RG_B200_GRAM=dense)
+  bool gram_dense = false;
+  int64_t miss_cap = 0;
 
   // ---- level-0 solver selection (RG_B200_SOLVER = mixed | f64) and its counters
   int solver_mixed = 1;

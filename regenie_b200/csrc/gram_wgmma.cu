@@ -15,6 +15,8 @@
 //                in registers, int32) and stores them, times out_scale, as FP32 straight from the fragments
 //   warp 8     : TMA producer (cp.async.bulk.tensor 2D, 128B swizzle, 4-stage mbarrier ring)
 // K loop = the fold's samples in 128-byte (= 128-sample) swizzle atoms, 4 MMAs per atom.
+// Tiles of rows >= 128 miss_tile0 (the Miss rows of the Z Z^T Gram) return at once when the block's missing calls fit
+// the sparse path's list (*miss_total <= miss_cap): miss_gram.cu writes those rows then.
 #include "kernels.cuh"
 #include "wgmma_sm90.cuh"
 
@@ -39,7 +41,8 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 gram_s8_wgmma_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_constant__ CUtensorMap tmB,
                       const int2* __restrict__ tiles,
                       const int2* __restrict__ fold_k, float* __restrict__ out, int ldo,
-                      int64_t fold_stride, float out_scale) {
+                      int64_t fold_stride, float out_scale, const unsigned long long* __restrict__ miss_total,
+                      unsigned long long miss_cap, int miss_tile0) {
   constexpr int B_BYTES = BN * BK;
   constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int NACC = BN / 2;
@@ -56,6 +59,7 @@ gram_s8_wgmma_kernel(const __grid_constant__ CUtensorMap tmZ, const __grid_const
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role
   const int2 tile = tiles[blockIdx.x];          // (m tile of 128 rows, n tile of BN rows)
+  if (miss_total && tile.x >= miss_tile0 && *miss_total <= miss_cap) return;
   const int2 fk = fold_k[blockIdx.y];           // (first K block, number of K blocks)
   const int nkb = fk.y;
 
@@ -183,15 +187,18 @@ void gram_tile_list(int rows2, std::vector<int2>& tiles) {
 }
 
 void launch_gram_wgmma(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
-                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn) {
+                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn,
+                         const unsigned long long* miss_total, int64_t miss_cap, int miss_tile0) {
   RG_CHECK(bn == 256 || bn == 128, "gram tiles are 128 x 256 or 128 x 128");
   dim3 grid(ntiles, K);
   if (bn == 256) {
     ensure_dyn_smem(reinterpret_cast<const void*>(gram_s8_wgmma_kernel<256>), gram_smem_bytes(256));
-    gram_s8_wgmma_kernel<256><<<grid, NTHREADS, gram_smem_bytes(256), s>>>(tm, tmB, tiles, fold_k, out, ldo, fold_stride, out_scale);
+    gram_s8_wgmma_kernel<256><<<grid, NTHREADS, gram_smem_bytes(256), s>>>(tm, tmB, tiles, fold_k, out, ldo, fold_stride, out_scale,
+                                                                                     miss_total, miss_cap, miss_tile0);
   } else {
     ensure_dyn_smem(reinterpret_cast<const void*>(gram_s8_wgmma_kernel<128>), gram_smem_bytes(128));
-    gram_s8_wgmma_kernel<128><<<grid, NTHREADS, gram_smem_bytes(128), s>>>(tm, tmB, tiles, fold_k, out, ldo, fold_stride, out_scale);
+    gram_s8_wgmma_kernel<128><<<grid, NTHREADS, gram_smem_bytes(128), s>>>(tm, tmB, tiles, fold_k, out, ldo, fold_stride, out_scale,
+                                                                                     miss_total, miss_cap, miss_tile0);
   }
 }
 

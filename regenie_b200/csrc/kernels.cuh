@@ -70,11 +70,23 @@ void launch_l0_stats_finish(const float* T, int ldt, int64_t t_fold_stride, cons
                             int64_t zz_fold_stride, int rows_p, int cpp, int ncol, int K, const double* scale,
                             int32_t* cnt_fold, double* sum_fold, cudaStream_t s);
 void gram_tile_list(int rows2, std::vector<int2>& tiles);
+// miss_total != null: tiles of m tile >= miss_tile0 return at once when *miss_total <= miss_cap (miss_gram.cu)
 void launch_gram_wgmma(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
-                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256);
+                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256,
+                         const unsigned long long* miss_total = nullptr, int64_t miss_cap = 0, int miss_tile0 = 0);
 // operand-plane bytes of the Step-1 block (bed_expand_fp8_kernel): dosage d -> 8 d as int8
 constexpr float kZScaleGram = 1.f / 64;   // Z Z^T tiles: both operands carry 8
 constexpr float kZScaleStat = 1.f / 8;    // Z [X|Y]-digit tiles: the digit rows are plain int8 integers
+// ---- miss_gram.cu: the Miss rows of the Z Z^T Gram from per-(SNP, fold) lists of the missing calls
+// missing calls per block (as a fraction of bs_max x analysed samples) up to which the sparse sums run: the crossover
+// of tools/miss_rate_sweep.py (DESIGN.md section 3)
+constexpr double kMissSparseRate = 0.015;
+void launch_miss_list(const uint32_t* gp, int64_t npad, int rows_p, const int2* fold_k, int K, unsigned long long* total,
+                      int64_t cap, int2* seg, int32_t* list, cudaStream_t s);
+void launch_miss_transpose(const uint32_t* gp, int64_t npad, int rows_p, const unsigned long long* total, int64_t cap,
+                           uint32_t* gt, cudaStream_t s);
+void launch_miss_sparse(const uint32_t* gt, int rows_p, const int2* seg, const int32_t* list, int K,
+                        const unsigned long long* total, int64_t cap, float* zz, int64_t fold_stride, cudaStream_t s);
 void launch_gram_reference(const uint8_t* z, int64_t npad, int rows2, int k0, int k1, float* out, int ldo,
                            cudaStream_t s);
 

@@ -209,6 +209,15 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
       make_gram_tensor_map(&h->tmD, h->xyD.p, h->Npad, h->stat_drows);
     }
   }
+  // Miss rows of the Gram as sparse sums while a block has at most kMissSparseRate missing calls (miss_gram.cu)
+  {
+    // RG_B200_GRAM=dense: always the dense tiles; =sparse: a list for every call (tools/miss_rate_sweep.py)
+    const char* e = getenv("RG_B200_GRAM");
+    const std::string mode = e ? e : "";
+    h->gram_dense = mode == "dense";
+    const double rate = mode == "sparse" ? 1.0 : kMissSparseRate;
+    h->miss_cap = std::min<int64_t>((int64_t)(rate * h->bs_max * h->n_analyzed), INT32_MAX);
+  }
   RG_CUDA(cudaStreamSynchronize(s));   // host vectors go out of scope
 }
 
@@ -625,10 +634,26 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     }
     const rg_ctx::TileList& tl =
         cached_tiles(h->tile_lists, rows_p, [&](std::vector<int2>& tiles) { gram_tile_list(2 * rows_p, tiles); });
+    const int64_t zz_stride = (int64_t)4 * rows_p * rows_p;
     ScopedTimer t(h, "gram_wgmma", s);
-    launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], tl.buf.p, tl.count, h->fold_k.p, K,
-                      L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, kZScaleGram, s);
-    h->launches += 1;
+    if (h->gram_dense) {
+      launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], tl.buf.p, tl.count, h->fold_k.p, K,
+                        L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s);
+      h->launches += 1;
+    } else {
+      // the Miss rows: the device picks the sparse sums or the dense tiles from the block's missing-call count
+      L.miss_total.alloc(1);
+      L.miss_seg.alloc((size_t)K * h->rows_p_max);
+      L.miss_list.alloc((size_t)std::max<int64_t>(h->miss_cap, 1));
+      L.gt.alloc((size_t)Npad * (h->rows_p_max / 16));
+      launch_miss_list(L.gp.p, Npad, rows_p, h->fold_k.p, K, L.miss_total.p, h->miss_cap, L.miss_seg.p, L.miss_list.p, s);
+      launch_miss_transpose(L.gp.p, Npad, rows_p, L.miss_total.p, h->miss_cap, L.gt.p, s);
+      launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], tl.buf.p, tl.count, h->fold_k.p, K,
+                        L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
+      launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, L.miss_list.p, K, L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
+      h->launches += 5;
+    }
+    L.last_gram_dense = h->gram_dense;
   }
   if (h->stats_tc) {
     // Z [X | Y]-digits: one more column tile per row tile of the same kernel, then the FP64 Horner
@@ -818,6 +843,20 @@ static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
   if (n == "dims") {
     const int64_t v[8] = {h->Npad, rp, h->last_nC, h->last_n_aug, h->last_nmat, h->K, h->cpp, h->nchunks};
     return host_view(v, 8);
+  }
+  if (n == "gram_path") {
+    // how the Miss rows of the last block's Gram were computed: 1 = sparse sums, 0 = dense tiles; the block's
+    // missing calls (-1 when RG_B200_GRAM=dense skipped the count) and the sparse path's capacity
+    int64_t v[3] = {0, -1, h->miss_cap};
+    if (!L.last_gram_dense) {
+      RG_CHECK(L.miss_total.p, "debug buffer not filled yet: gram_path");
+      unsigned long long tot = 0;
+      RG_CUDA(cudaStreamSynchronize(L.stream));
+      RG_CUDA(cudaMemcpy(&tot, L.miss_total.p, sizeof(tot), cudaMemcpyDeviceToHost));
+      v[0] = (int64_t)tot <= h->miss_cap ? 1 : 0;
+      v[1] = (int64_t)tot;
+    }
+    return host_view(v, 3);
   }
   if (n == "pad_of") return host_view(h->pad_of.data(), h->N);
   if (n == "zz_ref") {
