@@ -16,19 +16,6 @@
 #include "context.cuh"
 #include "inflate_core.h"
 
-#define RG_API_BEGIN try {
-#define RG_API_END                         \
-  }                                        \
-  catch (const rg::Error& e) {             \
-    rg::set_last_error(e.msg);             \
-    return 1;                              \
-  }                                        \
-  catch (const std::exception& e) {        \
-    rg::set_last_error(e.what());          \
-    return 1;                              \
-  }                                        \
-  return 0;
-
 namespace rg {
 
 constexpr int kInflateWarps = 8;           // streams per CTA; 3.3 KB of decode tables each in shared memory

@@ -177,7 +177,7 @@ struct rg_ctx {
   // binary traits / dosages
   int bt_mode = 0, bt_dp = 0, bt_ncol = 0;   // bt_ncol: used feature columns of the bt_dp padded ones
   int s2_fcols = 0;                           // the same for the quantitative-trait feature rows (dp)
-  bool bt_chr_set = false;
+  bool s2_chr_set = false, bt_chr_set = false;   // rg_s2_set_chr / rg_s2_set_chr_bt has run
   int s2_last_bs = 0;                // variants resident in dz (for rg_s2_firth)
   // shape of the sums the last block left (rg_debug_fetch "s2_sums" / "bt_sums"): padded rows, and the row width of bt_sums
   int s2_sums_rows = 0, bt_sums_rows = 0, bt_sums_dp = 0;
@@ -229,3 +229,17 @@ void sync_lanes(rg_ctx* h);
 // throws when a kernel of rg_pgen_decode flagged a malformed record (pgen_decode.cu)
 void pgen_check_errors(rg_ctx* h);
 }
+
+// body of every C ABI entry point: an exception becomes return code 1 and the message of rg_last_error
+#define RG_API_BEGIN try {
+#define RG_API_END                         \
+  }                                        \
+  catch (const rg::Error& e) {             \
+    rg::set_last_error(e.msg);             \
+    return 1;                              \
+  }                                        \
+  catch (const std::exception& e) {        \
+    rg::set_last_error(e.what());          \
+    return 1;                              \
+  }                                        \
+  return 0;

@@ -9,21 +9,6 @@
 
 using namespace rg;
 
-#define RG_API_BEGIN try {
-#define RG_API_END                         \
-  }                                        \
-  catch (const rg::Error& e) {             \
-    rg::set_last_error(e.msg);             \
-    return 1;                              \
-  }                                        \
-  catch (const std::exception& e) {        \
-    rg::set_last_error(e.what());          \
-    return 1;                              \
-  }                                        \
-  return 0;
-
-
-
 static void l1_setup_chunks(rg_ctx* h, int nC, int ldp) {
   cudaStream_t s = h->stream;
   const int K = h->K;

@@ -16,19 +16,6 @@
 #include "context.cuh"
 #include "pgen_core.h"
 
-#define RG_API_BEGIN try {
-#define RG_API_END                         \
-  }                                        \
-  catch (const rg::Error& e) {             \
-    rg::set_last_error(e.msg);             \
-    return 1;                              \
-  }                                        \
-  catch (const std::exception& e) {        \
-    rg::set_last_error(e.what());          \
-    return 1;                              \
-  }                                        \
-  return 0;
-
 namespace rg {
 
 struct PgenMeta {                 // device views into the block's metadata blob

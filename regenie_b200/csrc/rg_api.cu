@@ -901,19 +901,6 @@ static int64_t copy_debug_view(const DebugView& v, const std::string& n, void* o
 
 using namespace rg;
 
-#define RG_API_BEGIN try {
-#define RG_API_END                         \
-  }                                        \
-  catch (const rg::Error& e) {             \
-    rg::set_last_error(e.msg);             \
-    return 1;                              \
-  }                                        \
-  catch (const std::exception& e) {        \
-    rg::set_last_error(e.what());          \
-    return 1;                              \
-  }                                        \
-  return 0;
-
 extern "C" {
 
 const char* rg_last_error(void) { return rg::g_last_error.c_str(); }

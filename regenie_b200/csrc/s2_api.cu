@@ -8,19 +8,6 @@
 
 using namespace rg;
 
-#define RG_API_BEGIN try {
-#define RG_API_END                         \
-  }                                        \
-  catch (const rg::Error& e) {             \
-    rg::set_last_error(e.msg);             \
-    return 1;                              \
-  }                                        \
-  catch (const std::exception& e) {        \
-    rg::set_last_error(e.what());          \
-    return 1;                              \
-  }                                        \
-  return 0;
-
 static void s2_create(rg_ctx* h, const rg_step2_config* cfg, const double* X, const uint8_t* mask,
                       const uint8_t* in_analysis) {
   h->kind = 2;
@@ -170,6 +157,7 @@ static void s2_set_chr(rg_ctx* h, const double* res, const double* scf_sv) {
   RG_CUDA(cudaMemcpyAsync(h->s2_male_tot.p, male_tot.data(), (1 + P) * 8, cudaMemcpyHostToDevice, h->stream));
   s2_build_digits(h, h->F.p, dp, base + (with_sex ? 1 + P : 0));
   RG_CUDA(cudaStreamSynchronize(h->stream));
+  h->s2_chr_set = true;
 }
 
 // per-variant non-PAR flags set by rg_s2_set_non_par apply to exactly one block call
@@ -196,13 +184,25 @@ static void s2_wait_stage(rg_ctx* h, const void* in, cudaStream_t s) {
 }
 }
 
+// Packed per-variant outputs of a block, laid out alike in s2_out_d / s2_out_i and in their pinned host mirrors: f64 slabs
+// af, mac, stat, beta, se, chisq [bs_max x P], then af_all, mac_all, scale_fac [bs_max]; i32 slabs ns [bs_max x P], then
+// ns_all, flags [bs_max].
+static size_t s2_out_f64(const rg_ctx* h) { return (size_t)h->bs_max * (6 * (size_t)h->P + 3); }
+static size_t s2_out_i32(const rg_ctx* h) { return (size_t)h->bs_max * ((size_t)h->P + 2); }
+static rg_s2_out s2_out_at(const rg_ctx* h, double* d, int32_t* i) {
+  const size_t bp = (size_t)h->bs_max * h->P, b1 = h->bs_max;
+  rg_s2_out o;
+  o.af = d; o.mac = d + bp; o.stat = d + 2 * bp; o.beta = d + 3 * bp; o.se = d + 4 * bp; o.chisq = d + 5 * bp;
+  o.af_all = d + 6 * bp; o.mac_all = d + 6 * bp + b1; o.scale_fac = d + 6 * bp + 2 * b1;
+  o.ns = i; o.ns_all = i + bp; o.flags = i + bp + b1;
+  return o;
+}
+
 // Results of a block back to the caller: the packed f64 / i32 output buffers cross PCIe as TWO copies into pinned mirrors
 // (instead of twelve copies into whatever memory the caller's arrays live in) and are handed out with memcpy after the
 // stream has drained - the block calls are synchronous, so every microsecond of this tail is exposed.
 static void s2_copy_out(rg_ctx* h, int bs, const rg_s2_out* out, double* info_out, const double* info_dev, cudaStream_t s) {
-  const int P = h->P;
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  const size_t nd = 6 * bp + 3 * b1, ni = bp + 2 * b1;
+  const size_t bp = (size_t)h->bs_max * h->P, nd = s2_out_f64(h), ni = s2_out_i32(h);
   if (h->s2_host_cap < nd + bp) {
     if (h->s2_hd) RG_CUDA(cudaFreeHost(h->s2_hd));
     if (h->s2_hi) RG_CUDA(cudaFreeHost(h->s2_hi));
@@ -212,42 +212,76 @@ static void s2_copy_out(rg_ctx* h, int bs, const rg_s2_out* out, double* info_ou
   }
   RG_CUDA(cudaMemcpyAsync(h->s2_hd, h->s2_out_d.p, nd * sizeof(double), cudaMemcpyDeviceToHost, s));
   RG_CUDA(cudaMemcpyAsync(h->s2_hi, h->s2_out_i.p, ni * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (info_out) RG_CUDA(cudaMemcpyAsync(h->s2_hd + nd, info_dev, (size_t)bs * P * 8, cudaMemcpyDeviceToHost, s));
+  if (info_out) RG_CUDA(cudaMemcpyAsync(h->s2_hd + nd, info_dev, (size_t)bs * h->P * 8, cudaMemcpyDeviceToHost, s));
   RG_CUDA(cudaStreamSynchronize(s));
-  const double* d = h->s2_hd;
-  const int32_t* ii = h->s2_hi;
-  const size_t vp = (size_t)bs * P * 8, v1 = (size_t)bs * 8;
-  auto cp = [](void* dst, const void* src, size_t bytes) { if (dst) memcpy(dst, src, bytes); };
-  cp(out->af, d, vp); cp(out->mac, d + bp, vp); cp(out->stat, d + 2 * bp, vp); cp(out->beta, d + 3 * bp, vp);
-  cp(out->se, d + 4 * bp, vp); cp(out->chisq, d + 5 * bp, vp); cp(out->af_all, d + 6 * bp, v1);
-  cp(out->mac_all, d + 6 * bp + b1, v1); cp(out->scale_fac, d + 6 * bp + 2 * b1, v1);
-  cp(out->ns, ii, (size_t)bs * P * 4); cp(out->ns_all, ii + bp, (size_t)bs * 4); cp(out->flags, ii + bp + b1, (size_t)bs * 4);
-  cp(info_out, d + nd, vp);
+  const rg_s2_out m = s2_out_at(h, h->s2_hd, h->s2_hi);
+  const size_t vp = (size_t)bs * h->P, v1 = bs;
+  auto cp = [](auto* dst, const auto* src, size_t n) { if (dst) memcpy(dst, src, n * sizeof(*src)); };
+  cp(out->af, m.af, vp); cp(out->mac, m.mac, vp); cp(out->stat, m.stat, vp); cp(out->beta, m.beta, vp); cp(out->se, m.se, vp);
+  cp(out->chisq, m.chisq, vp); cp(out->af_all, m.af_all, v1); cp(out->mac_all, m.mac_all, v1); cp(out->scale_fac, m.scale_fac, v1);
+  cp(out->ns, m.ns, vp); cp(out->ns_all, m.ns_all, v1); cp(out->flags, m.flags, v1);
+  cp(info_out, h->s2_hd + nd, vp);
+}
+
+// What every block route does first: the handle, block-size and chromosome-state checks (quantitative-trait routes need
+// rg_s2_set_chr, binary-trait routes rg_s2_set_chr_bt), then the device, the staged copies of the block's inputs, the
+// sample index map and the packed output buffers.
+static void s2_block_begin(rg_ctx* h, bool bt, int bs, const int32_t* sample_idx, const void* in, const void* in2 = nullptr) {
+  RG_CHECK(h->kind == 2, "handle is not a Step-2 handle");
+  RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
+  if (bt) RG_CHECK(h->bt_chr_set, "rg_s2_set_chr_bt has not been called");
+  else RG_CHECK(h->s2_chr_set, "rg_s2_set_chr has not been called");
+  RG_CUDA(cudaSetDevice(h->device));
+  s2_wait_stage(h, in, h->stream);
+  s2_wait_stage(h, in2, h->stream);
+  ensure_file_idx(h, sample_idx);
+  h->s2_out_d.alloc(s2_out_f64(h));
+  h->s2_out_i.alloc(s2_out_i32(h));
+}
+
+// 2-bit rows of the block on the device: a device pointer as it is, host rows through packed_dev
+static const uint8_t* s2_rows_in(rg_ctx* h, const uint8_t* packed, int64_t row_stride, int bs) {
+  if (is_device_pointer(packed)) return packed;
+  h->packed_dev.alloc((size_t)h->bs_max * row_stride);
+  copy_to_device(h->packed_dev.p, packed, (size_t)bs * row_stride, h->stream);
+  return h->packed_dev.p;
+}
+
+// 8-bit probability pairs and ploidy / missing bytes of the block on the device, likewise through probs_dev / miss_dev
+static void s2_probs_in(rg_ctx* h, const uint8_t** probs, const uint8_t** miss, int64_t n_file, int bs) {
+  if (is_device_pointer(*probs)) return;
+  h->probs_dev.alloc((size_t)h->bs_max * n_file * 2);
+  copy_to_device(h->probs_dev.p, *probs, (size_t)bs * n_file * 2, h->stream);
+  *probs = h->probs_dev.p;
+  if (*miss) {
+    h->miss_dev.alloc((size_t)h->bs_max * n_file);
+    copy_to_device(h->miss_dev.p, *miss, (size_t)bs * n_file, h->stream);
+    *miss = h->miss_dev.p;
+  }
+}
+
+// the fields S2FinalizeArgs and S2BtFinalizeArgs share, the packed outputs included; consumes the block's non-PAR flags
+template <typename Args>
+static void s2_finalize_args(rg_ctx* h, Args& a, int bs, int dp, double min_mac, const double* sums, int col_male) {
+  a.bs = bs; a.C = h->C; a.P = h->P; a.dp = dp;
+  a.n_analyzed = h->n_analyzed; a.n_samples = h->N; a.min_mac = min_mac; a.numtol = 1e-6;
+  a.sums = sums; a.non_par = take_non_par(h, bs); a.col_male = col_male;
+  const rg_s2_out o = s2_out_at(h, h->s2_out_d.p, h->s2_out_i.p);
+  a.af = o.af; a.mac = o.mac; a.stat = o.stat; a.beta = o.beta; a.se = o.se; a.chisq = o.chisq;
+  a.af_all = o.af_all; a.mac_all = o.mac_all; a.scale_fac = o.scale_fac;
+  a.ns = o.ns; a.ns_all = o.ns_all; a.flags = o.flags;
 }
 
 static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, int bs, const int32_t* sample_idx,
                          int ref_first, double min_mac, const rg_s2_out* out) {
-  RG_CHECK(h->kind == 2, "handle is not a Step-2 handle");
-  RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
-  RG_CUDA(cudaSetDevice(h->device));
+  s2_block_begin(h, false, bs, sample_idx, packed);
   cudaStream_t s = h->stream;
-  s2_wait_stage(h, packed, s);
-  const int P = h->P, C = h->C;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  ensure_file_idx(h, sample_idx);
-  const uint8_t* packed_d = packed;
-  if (!is_device_pointer(packed)) {
-    h->packed_dev.alloc((size_t)h->bs_max * row_stride);
-    copy_to_device(h->packed_dev.p, packed, (size_t)bs * row_stride, s);
-    packed_d = h->packed_dev.p;
-  }
+  const uint8_t* packed_d = s2_rows_in(h, packed, row_stride, bs);
   h->gp.alloc((size_t)h->rows_p_max * (Npad / 16));
   if (!h->s2_tc) h->s2_part.alloc((size_t)h->nchunks * h->rows_p_max * 3 * h->dp);
   h->s2_sums.alloc((size_t)h->rows_p_max * 3 * h->dp);
-  const size_t nd = (size_t)h->bs_max * (7 * (size_t)P + 3), ni = (size_t)h->bs_max * ((size_t)P + 2);
-  h->s2_out_d.alloc(nd);
-  h->s2_out_i.alloc(ni);
   launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, h->gp.p, Npad, s);
   if (h->s2_tc) {
     s2_tensor_sums(h, rows_p, s);
@@ -257,17 +291,9 @@ static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     launch_s2_stats(h->gp.p, Npad, h->F.p, h->dp, h->chunks.p, h->nchunks, rows_p, h->s2_part.p, h->s2_sums.p, s);
   }
   S2FinalizeArgs a;
-  a.bs = bs; a.C = C; a.P = P; a.dp = h->dp; a.strict = h->strict;
-  a.n_analyzed = h->n_analyzed; a.n_samples = h->N; a.min_mac = min_mac; a.numtol = 1e-6;
-  a.sums = h->s2_sums.p; a.mask_count = h->s2_maskcount.p; a.YtX = h->s2_YtX.p; a.XmX = h->s2_XmX.p;
-  a.scf_sv = h->s2_scf.p;
-  a.non_par = take_non_par(h, bs); a.col_male = h->s2_col_male; a.male_tot = h->s2_male_tot.p;
-  double* d = h->s2_out_d.p;
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  a.af = d; a.mac = d + bp; a.stat = d + 2 * bp; a.beta = d + 3 * bp; a.se = d + 4 * bp; a.chisq = d + 5 * bp;
-  a.af_all = d + 6 * bp; a.mac_all = d + 6 * bp + b1; a.scale_fac = d + 6 * bp + 2 * b1;
-  int32_t* ii = h->s2_out_i.p;
-  a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
+  s2_finalize_args(h, a, bs, h->dp, min_mac, h->s2_sums.p, h->s2_col_male);
+  a.strict = h->strict; a.mask_count = h->s2_maskcount.p; a.YtX = h->s2_YtX.p; a.XmX = h->s2_XmX.p; a.scf_sv = h->s2_scf.p;
+  a.male_tot = h->s2_male_tot.p;
   launch_s2_finalize(a, s);
   h->launches += 4;
   h->s2_sums_rows = rows_p;
@@ -330,56 +356,34 @@ static void s2_set_chr_bt(rg_ctx* h, const rg_s2_bt_chr* st) {
   h->bt_chr_set = true;
 }
 
+// the per-variant buffers of the binary-trait finish (S2BtFinalizeArgs), which rg_s2_firth / rg_s2_spa read back
+static void s2_bt_outputs(rg_ctx* h, S2BtFinalizeArgs& a) {
+  const size_t bp = (size_t)h->bs_max * h->P;
+  h->bt_xtwg.alloc(bp * h->C); h->bt_mu.alloc(h->bs_max); h->bt_info.alloc(bp); h->bt_den.alloc(bp);
+  a.with_flip = 1; a.col_tot = h->bt_coltot.p; a.xwy = h->bt_xwy.p; a.nz_count = h->bt_nnz.p; a.n510 = h->bt_n510.p;
+  a.info = h->bt_info.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.den = h->bt_den.p;
+}
+
 static void s2_block_bgen8_bt(rg_ctx* h, const uint8_t* probs, const uint8_t* miss, int64_t n_file, int bs,
                               const int32_t* sample_idx, int ref_first, double min_mac, const rg_s2_out* out,
                               double* info_out) {
-  RG_CHECK(h->kind == 2, "handle is not a Step-2 handle");
-  RG_CHECK(h->bt_chr_set, "rg_s2_set_chr_bt has not been called");
-  RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
-  RG_CUDA(cudaSetDevice(h->device));
+  s2_block_begin(h, true, bs, sample_idx, probs, miss);
   cudaStream_t s = h->stream;
-  s2_wait_stage(h, probs, s);
-  s2_wait_stage(h, miss, s);
-  const int P = h->P, C = h->C, dp = h->bt_dp;
+  const int dp = h->bt_dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  ensure_file_idx(h, sample_idx);
-  const uint8_t *probs_d = probs, *miss_d = miss;
-  if (!is_device_pointer(probs)) {
-    h->probs_dev.alloc((size_t)h->bs_max * n_file * 2);
-    copy_to_device(h->probs_dev.p, probs, (size_t)bs * n_file * 2, s);
-    probs_d = h->probs_dev.p;
-    if (miss) {
-      h->miss_dev.alloc((size_t)h->bs_max * n_file);
-      copy_to_device(h->miss_dev.p, miss, (size_t)bs * n_file, s);
-      miss_d = h->miss_dev.p;
-    }
-  }
+  s2_probs_in(h, &probs, &miss, n_file, bs);
   h->dz.alloc((size_t)h->rows_p_max * Npad);
   h->bt_part.alloc((size_t)h->nchunks * h->rows_p_max * 4 * dp);
   h->bt_sums.alloc((size_t)h->rows_p_max * 4 * dp);
   h->bt_nnz.alloc(h->rows_p_max); h->bt_n510.alloc(h->rows_p_max);
-  h->bt_xtwg.alloc((size_t)h->bs_max * P * C); h->bt_mu.alloc(h->bs_max); h->bt_info.alloc((size_t)h->bs_max * P);
-  h->bt_den.alloc((size_t)h->bs_max * P);
-  const size_t nd = (size_t)h->bs_max * (7 * (size_t)P + 3), ni = (size_t)h->bs_max * ((size_t)P + 2);
-  h->s2_out_d.alloc(nd);
-  h->s2_out_i.alloc(ni);
-  launch_dosage_relayout(probs_d, miss_d, n_file, bs, rows_p, h->file_idx_pad.p, ref_first, h->dz.p, Npad, s);
   h->bt_cnt_part.alloc((size_t)h->nchunks * h->rows_p_max);
+  launch_dosage_relayout(probs, miss, n_file, bs, rows_p, h->file_idx_pad.p, ref_first, h->dz.p, Npad, s);
   launch_dosage_stats(h->dz.p, Npad, h->bt_F.p, dp, h->chunks.p, h->nchunks, rows_p, h->bt_part.p, h->bt_cnt_part.p, h->bt_sums.p,
                       h->bt_nnz.p, h->bt_n510.p, s, h->bt_ncol);
   S2BtFinalizeArgs a;
-  a.bs = bs; a.C = C; a.P = P; a.dp = dp; a.with_flip = 1;
-  a.n_analyzed = h->n_analyzed; a.n_samples = h->N; a.min_mac = min_mac; a.numtol = 1e-6;
-  a.sums = h->bt_sums.p; a.col_tot = h->bt_coltot.p; a.xwy = h->bt_xwy.p; a.nz_count = h->bt_nnz.p; a.n510 = h->bt_n510.p;
-  a.non_par = take_non_par(h, bs); a.col_male = h->bt_col_male;
-  double* d = h->s2_out_d.p;
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  a.af = d; a.mac = d + bp; a.stat = d + 2 * bp; a.beta = d + 3 * bp; a.se = d + 4 * bp; a.chisq = d + 5 * bp;
-  a.af_all = d + 6 * bp; a.mac_all = d + 6 * bp + b1; a.scale_fac = d + 6 * bp + 2 * b1;
-  a.info = h->bt_info.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.den = h->bt_den.p;
-  int32_t* ii = h->s2_out_i.p;
-  a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
+  s2_bt_outputs(h, a);
+  s2_finalize_args(h, a, bs, dp, min_mac, h->bt_sums.p, h->bt_col_male);
   launch_s2_bt_finalize(a, s);
   h->launches += 5;
   h->s2_last_bs = bs;
@@ -391,54 +395,28 @@ static void s2_block_bgen8_bt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
 static void s2_block_bgen8_qt(rg_ctx* h, const uint8_t* probs, const uint8_t* miss, int64_t n_file, int bs,
                               const int32_t* sample_idx, int ref_first, double min_mac, const rg_s2_out* out,
                               double* info_out) {
-  RG_CHECK(h->kind == 2, "handle is not a Step-2 handle");
-  RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
-  RG_CUDA(cudaSetDevice(h->device));
+  s2_block_begin(h, false, bs, sample_idx, probs, miss);
   cudaStream_t s = h->stream;
-  s2_wait_stage(h, probs, s);
-  s2_wait_stage(h, miss, s);
-  const int P = h->P, C = h->C, dp = h->dp;
+  const int dp = h->dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  ensure_file_idx(h, sample_idx);
-  const uint8_t *probs_d = probs, *miss_d = miss;
-  if (!is_device_pointer(probs)) {
-    h->probs_dev.alloc((size_t)h->bs_max * n_file * 2);
-    copy_to_device(h->probs_dev.p, probs, (size_t)bs * n_file * 2, s);
-    probs_d = h->probs_dev.p;
-    if (miss) {
-      h->miss_dev.alloc((size_t)h->bs_max * n_file);
-      copy_to_device(h->miss_dev.p, miss, (size_t)bs * n_file, s);
-      miss_d = h->miss_dev.p;
-    }
-  }
+  s2_probs_in(h, &probs, &miss, n_file, bs);
   h->dz.alloc((size_t)h->rows_p_max * Npad);
   h->bt_part.alloc((size_t)h->nchunks * h->rows_p_max * 4 * dp);
   h->bt_sums.alloc((size_t)h->rows_p_max * 4 * dp);
   h->bt_nnz.alloc(h->rows_p_max); h->bt_n510.alloc(h->rows_p_max);
   h->s2_sums.alloc((size_t)h->rows_p_max * 3 * dp);
   h->bt_xtwg.alloc((size_t)h->rows_p_max * dp);            // Se in dosage units
-  h->bt_info.alloc((size_t)h->bs_max * P);
-  const size_t nd = (size_t)h->bs_max * (7 * (size_t)P + 3), ni = (size_t)h->bs_max * ((size_t)P + 2);
-  h->s2_out_d.alloc(nd);
-  h->s2_out_i.alloc(ni);
-  launch_dosage_relayout(probs_d, miss_d, n_file, bs, rows_p, h->file_idx_pad.p, ref_first, h->dz.p, Npad, s);
+  h->bt_info.alloc((size_t)h->bs_max * h->P);
   h->bt_cnt_part.alloc((size_t)h->nchunks * h->rows_p_max);
+  launch_dosage_relayout(probs, miss, n_file, bs, rows_p, h->file_idx_pad.p, ref_first, h->dz.p, Npad, s);
   launch_dosage_stats(h->dz.p, Npad, h->F.p, dp, h->chunks.p, h->nchunks, rows_p, h->bt_part.p, h->bt_cnt_part.p, h->bt_sums.p,
                       h->bt_nnz.p, h->bt_n510.p, s, h->s2_fcols);
   launch_dosage_scale(h->bt_sums.p, rows_p, dp, h->s2_sums.p, h->bt_xtwg.p, s);
   S2FinalizeArgs a;
-  a.bs = bs; a.C = C; a.P = P; a.dp = dp; a.strict = h->strict;
-  a.n_analyzed = h->n_analyzed; a.n_samples = h->N; a.min_mac = min_mac; a.numtol = 1e-6;
-  a.sums = h->s2_sums.p; a.mask_count = h->s2_maskcount.p; a.YtX = h->s2_YtX.p; a.XmX = h->s2_XmX.p;
-  a.scf_sv = h->s2_scf.p; a.nz_count = h->bt_nnz.p; a.info_sums = h->bt_xtwg.p; a.info = h->bt_info.p;
-  a.non_par = take_non_par(h, bs); a.col_male = h->s2_col_male; a.male_tot = h->s2_male_tot.p;
-  double* d = h->s2_out_d.p;
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  a.af = d; a.mac = d + bp; a.stat = d + 2 * bp; a.beta = d + 3 * bp; a.se = d + 4 * bp; a.chisq = d + 5 * bp;
-  a.af_all = d + 6 * bp; a.mac_all = d + 6 * bp + b1; a.scale_fac = d + 6 * bp + 2 * b1;
-  int32_t* ii = h->s2_out_i.p;
-  a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
+  s2_finalize_args(h, a, bs, dp, min_mac, h->s2_sums.p, h->s2_col_male);
+  a.strict = h->strict; a.mask_count = h->s2_maskcount.p; a.YtX = h->s2_YtX.p; a.XmX = h->s2_XmX.p; a.scf_sv = h->s2_scf.p;
+  a.male_tot = h->s2_male_tot.p; a.nz_count = h->bt_nnz.p; a.info_sums = h->bt_xtwg.p; a.info = h->bt_info.p;
   launch_s2_finalize(a, s);
   h->launches += 6;
   h->s2_sums_rows = rows_p;
@@ -449,49 +427,26 @@ static void s2_block_bgen8_qt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
 // binary traits on 2-bit hard calls (.bed / .pgen): tensor-core sums, then the same finish as the dosage path
 static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride, int bs, const int32_t* sample_idx,
                             int ref_first, double min_mac, const rg_s2_out* out) {
-  RG_CHECK(h->kind == 2, "handle is not a Step-2 handle");
-  RG_CHECK(h->bt_chr_set, "rg_s2_set_chr_bt has not been called");
+  s2_block_begin(h, true, bs, sample_idx, packed);
   RG_CHECK(h->s2_tc, "rg_s2_block_bed_bt needs the tensor-core statistics (RG_B200_S2_STATS=f64 disables them)");
-  RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
-  RG_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
-  s2_wait_stage(h, packed, s);
-  const int P = h->P, C = h->C, dp = h->bt_dp;
+  const int dp = h->bt_dp;
   const int rows_p = (int)round_up(bs, kRowPad);
   const int64_t Npad = h->Npad;
-  ensure_file_idx(h, sample_idx);
-  const uint8_t* packed_d = packed;
-  if (!is_device_pointer(packed)) {
-    h->packed_dev.alloc((size_t)h->bs_max * row_stride);
-    copy_to_device(h->packed_dev.p, packed, (size_t)bs * row_stride, s);
-    packed_d = h->packed_dev.p;
-  }
+  const uint8_t* packed_d = s2_rows_in(h, packed, row_stride, bs);
   h->gp.alloc((size_t)h->rows_p_max * (Npad / 16));
   h->dz.alloc((size_t)h->rows_p_max * Npad);
   h->bt_sums.alloc((size_t)h->rows_p_max * 4 * dp);
   h->bt_nnz.alloc(h->rows_p_max); h->bt_n510.alloc(h->rows_p_max);
-  h->bt_xtwg.alloc((size_t)h->bs_max * P * C); h->bt_mu.alloc(h->bs_max); h->bt_info.alloc((size_t)h->bs_max * P);
-  h->bt_den.alloc((size_t)h->bs_max * P);
-  const size_t nd = (size_t)h->bs_max * (7 * (size_t)P + 3), ni = (size_t)h->bs_max * ((size_t)P + 2);
-  h->s2_out_d.alloc(nd);
-  h->s2_out_i.alloc(ni);
   launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, h->gp.p, Npad, s);
   s2_tensor_sums(h, rows_p, s);
   launch_s2_bt_bed_finish(h->s2_T.p, h->s2_drows, (int64_t)3 * rows_p * h->s2_drows, h->s2_nchunk, rows_p, dp, h->s2_ncol,
                           h->s2_Fscale.p, h->bt_sums.p, h->bt_nnz.p, h->bt_n510.p, s);
   launch_gp_to_dz(h->gp.p, rows_p, h->dz.p, Npad, s);               // what rg_s2_firth / rg_s2_spa read
   S2BtFinalizeArgs a;
-  a.bs = bs; a.C = C; a.P = P; a.dp = dp; a.with_flip = 1; a.unit = 1.0;
-  a.n_analyzed = h->n_analyzed; a.n_samples = h->N; a.min_mac = min_mac; a.numtol = 1e-6;
-  a.sums = h->bt_sums.p; a.col_tot = h->bt_coltot.p; a.xwy = h->bt_xwy.p; a.nz_count = h->bt_nnz.p; a.n510 = h->bt_n510.p;
-  a.non_par = take_non_par(h, bs); a.col_male = h->bt_col_male;
-  double* d = h->s2_out_d.p;
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  a.af = d; a.mac = d + bp; a.stat = d + 2 * bp; a.beta = d + 3 * bp; a.se = d + 4 * bp; a.chisq = d + 5 * bp;
-  a.af_all = d + 6 * bp; a.mac_all = d + 6 * bp + b1; a.scale_fac = d + 6 * bp + 2 * b1;
-  a.info = h->bt_info.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.den = h->bt_den.p;
-  int32_t* ii = h->s2_out_i.p;
-  a.ns = ii; a.ns_all = ii + bp; a.flags = ii + bp + b1;
+  s2_bt_outputs(h, a);
+  s2_finalize_args(h, a, bs, dp, min_mac, h->bt_sums.p, h->bt_col_male);
+  a.unit = 1.0;
   launch_s2_bt_finalize(a, s);
   h->launches += 7;
   h->s2_last_bs = bs;
@@ -499,69 +454,65 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   s2_copy_out(h, bs, out, nullptr, nullptr, s);
 }
 
-static void s2_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* beta, double* se,
-                     double* lrt, int32_t* status) {
-  RG_CHECK(h->kind == 2 && h->bt_chr_set && h->s2_last_bs > 0, "rg_s2_firth needs a resident dosage block");
+// Firth and SPA on (variant, trait) selections of the block left resident by a binary-trait route, kSelBatch at a time.
+// `batch(o, nb)` fills its kernel's arguments for selections o .. o + nb (uploaded to firth_sel), launches the kernel and
+// queues the copies of its results; the batch is complete when this returns to the loop.
+constexpr int kSelBatch = 256;
+template <typename Batch>
+static void s2_selections(rg_ctx* h, const char* call, int n_sel, const int32_t* var_idx, const int32_t* trait_idx,
+                          Batch&& batch) {
+  RG_CHECK(h->kind == 2 && h->bt_chr_set && h->s2_last_bs > 0, std::string(call) + " needs a resident dosage block");
   RG_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
-  const int P = h->P, C = h->C;
   for (int k = 0; k < n_sel; ++k)
-    RG_CHECK(var_idx[k] >= 0 && var_idx[k] < h->s2_last_bs && trait_idx[k] >= 0 && trait_idx[k] < P, "selection out of range");
-  const int kBatch = 256;
-  h->firth_gvec.alloc((size_t)kBatch * h->Npad); h->firth_cflag.alloc((size_t)kBatch * h->Npad);
-  h->firth_sel.alloc(2 * kBatch); h->firth_status.alloc(kBatch); h->firth_out.alloc(3 * kBatch);
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  for (int o = 0; o < n_sel; o += kBatch) {
-    const int nb = std::min(kBatch, n_sel - o);
+    RG_CHECK(var_idx[k] >= 0 && var_idx[k] < h->s2_last_bs && trait_idx[k] >= 0 && trait_idx[k] < h->P, "selection out of range");
+  h->firth_gvec.alloc((size_t)kSelBatch * h->Npad); h->firth_cflag.alloc((size_t)kSelBatch * h->Npad);
+  h->firth_sel.alloc(2 * kSelBatch); h->firth_status.alloc(kSelBatch); h->firth_out.alloc(3 * kSelBatch);
+  for (int o = 0; o < n_sel; o += kSelBatch) {
+    const int nb = std::min(kSelBatch, n_sel - o);
     RG_CUDA(cudaMemcpyAsync(h->firth_sel.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
-    RG_CUDA(cudaMemcpyAsync(h->firth_sel.p + kBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
-    FirthArgs a;
-    a.n_sel = nb; a.C = C; a.P = P; a.dp = h->bt_dp; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;
-    a.npad = h->Npad; a.sel_var = h->firth_sel.p; a.sel_trait = h->firth_sel.p + kBatch;
-    a.dz = h->dz.p; a.F = h->bt_F.p; a.w = h->bt_w.p; a.gs = h->bt_gs.p; a.xw = h->bt_xw.p; a.off = h->bt_off.p;
-    a.ym = h->bt_ym.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.mac = h->s2_out_d.p + bp;
-    a.flags = h->s2_out_i.p + bp + b1;
-    a.gvec = h->firth_gvec.p; a.cflag = h->firth_cflag.p;
-    a.beta = h->firth_out.p; a.se = h->firth_out.p + kBatch; a.lrt = h->firth_out.p + 2 * kBatch;
-    a.status = h->firth_status.p;
-    launch_s2_firth(a, s);
+    RG_CUDA(cudaMemcpyAsync(h->firth_sel.p + kSelBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+    batch(o, nb);
     h->launches += 1;
-    RG_CUDA(cudaMemcpyAsync(beta + o, a.beta, nb * 8, cudaMemcpyDeviceToHost, s));
-    RG_CUDA(cudaMemcpyAsync(se + o, a.se, nb * 8, cudaMemcpyDeviceToHost, s));
-    RG_CUDA(cudaMemcpyAsync(lrt + o, a.lrt, nb * 8, cudaMemcpyDeviceToHost, s));
-    RG_CUDA(cudaMemcpyAsync(status + o, a.status, nb * 4, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaStreamSynchronize(s));
   }
 }
 
+static void s2_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* beta, double* se,
+                     double* lrt, int32_t* status) {
+  s2_selections(h, "rg_s2_firth", n_sel, var_idx, trait_idx, [&](int o, int nb) {
+    cudaStream_t s = h->stream;
+    const rg_s2_out d = s2_out_at(h, h->s2_out_d.p, h->s2_out_i.p);
+    FirthArgs a;
+    a.n_sel = nb; a.C = h->C; a.P = h->P; a.dp = h->bt_dp; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;
+    a.npad = h->Npad; a.sel_var = h->firth_sel.p; a.sel_trait = h->firth_sel.p + kSelBatch;
+    a.dz = h->dz.p; a.F = h->bt_F.p; a.w = h->bt_w.p; a.gs = h->bt_gs.p; a.xw = h->bt_xw.p; a.off = h->bt_off.p;
+    a.ym = h->bt_ym.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.mac = d.mac; a.flags = d.flags;
+    a.gvec = h->firth_gvec.p; a.cflag = h->firth_cflag.p;
+    a.beta = h->firth_out.p; a.se = h->firth_out.p + kSelBatch; a.lrt = h->firth_out.p + 2 * kSelBatch;
+    a.status = h->firth_status.p;
+    launch_s2_firth(a, s);
+    RG_CUDA(cudaMemcpyAsync(beta + o, a.beta, nb * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(se + o, a.se, nb * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(lrt + o, a.lrt, nb * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(status + o, a.status, nb * 4, cudaMemcpyDeviceToHost, s));
+  });
+}
+
 static void s2_spa(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* pval, int32_t* status) {
-  RG_CHECK(h->kind == 2 && h->bt_chr_set && h->s2_last_bs > 0, "rg_s2_spa needs a resident dosage block");
-  RG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
-  const int P = h->P, C = h->C;
-  for (int k = 0; k < n_sel; ++k)
-    RG_CHECK(var_idx[k] >= 0 && var_idx[k] < h->s2_last_bs && trait_idx[k] >= 0 && trait_idx[k] < P, "selection out of range");
-  const int kBatch = 256;
-  h->firth_gvec.alloc((size_t)kBatch * h->Npad); h->firth_cflag.alloc((size_t)kBatch * h->Npad);
-  h->firth_sel.alloc(2 * kBatch); h->firth_status.alloc(kBatch); h->firth_out.alloc(3 * kBatch);
-  const size_t bp = (size_t)h->bs_max * P, b1 = h->bs_max;
-  for (int o = 0; o < n_sel; o += kBatch) {
-    const int nb = std::min(kBatch, n_sel - o);
-    RG_CUDA(cudaMemcpyAsync(h->firth_sel.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
-    RG_CUDA(cudaMemcpyAsync(h->firth_sel.p + kBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+  s2_selections(h, "rg_s2_spa", n_sel, var_idx, trait_idx, [&](int o, int nb) {
+    cudaStream_t s = h->stream;
+    const rg_s2_out d = s2_out_at(h, h->s2_out_d.p, h->s2_out_i.p);
     SpaArgs a;
-    a.n_sel = nb; a.C = C; a.P = P; a.dp = h->bt_dp; a.niter = 1000; a.tol = 1.220703125e-4;   // eps^(1/4), src/Regenie.hpp:330
-    a.npad = h->Npad; a.sel_var = h->firth_sel.p; a.sel_trait = h->firth_sel.p + kBatch;
+    a.n_sel = nb; a.C = h->C; a.P = h->P; a.dp = h->bt_dp; a.niter = 1000; a.tol = 1.220703125e-4;   // eps^(1/4), src/Regenie.hpp:330
+    a.npad = h->Npad; a.sel_var = h->firth_sel.p; a.sel_trait = h->firth_sel.p + kSelBatch;
     a.dz = h->dz.p; a.F = h->bt_F.p; a.w = h->bt_w.p; a.gs = h->bt_gs.p; a.xw = h->bt_xw.p; a.phat = h->bt_phat.p;
-    a.ym = h->bt_ym.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.stat = h->s2_out_d.p + 2 * bp; a.den = h->bt_den.p;
-    a.flags = h->s2_out_i.p + bp + b1;
+    a.ym = h->bt_ym.p; a.xtwg = h->bt_xtwg.p; a.mu = h->bt_mu.p; a.stat = d.stat; a.den = h->bt_den.p; a.flags = d.flags;
     a.gvec = h->firth_gvec.p; a.cflag = h->firth_cflag.p; a.pval = h->firth_out.p; a.status = h->firth_status.p;
     launch_s2_spa(a, s);
-    h->launches += 1;
     RG_CUDA(cudaMemcpyAsync(pval + o, a.pval, nb * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(status + o, a.status, nb * 4, cudaMemcpyDeviceToHost, s));
-    RG_CUDA(cudaStreamSynchronize(s));
-  }
+  });
 }
 
 extern "C" {

@@ -947,6 +947,25 @@ struct S2Writers {
   }
 };
 
+// Per-variant results of one Step-2 block call for up to bsz variants and P traits: the arrays behind an rg_s2_out
+struct S2Results {
+  std::vector<double> af, mac, stat, beta, se, chisq, info, af_all, mac_all, scale_fac;
+  std::vector<int32_t> ns, ns_all, flags;
+  void init(int bsz, int P) {
+    const size_t bp = (size_t)bsz * P;
+    for (auto* v : {&af, &mac, &stat, &beta, &se, &chisq, &info}) v->resize(bp);
+    for (auto* v : {&af_all, &mac_all, &scale_fac}) v->resize(bsz);
+    ns.resize(bp); ns_all.resize(bsz); flags.resize(bsz);
+  }
+  rg_s2_out out() { return out(*this); }
+  // the test columns (scale_fac, stat, beta, se, chisq) into those of `t`: the --test recode pass writes the test of the
+  // recoded genotypes over the additive one and keeps its own counts
+  rg_s2_out out(S2Results& t) {
+    return rg_s2_out{af.data(), ns.data(), mac.data(), af_all.data(), ns_all.data(), mac_all.data(), flags.data(),
+                     t.scale_fac.data(), t.stat.data(), t.beta.data(), t.se.data(), t.chisq.data()};
+  }
+};
+
 // --no-split prints N_RR N_RA N_AA of all analysed samples (src/Geno.cpp:2480-2486).  For hard calls they follow from two
 // allele sums the kernels already return: a pass over the block recoded as "recessive" (1 -> 0, 2 -> 1) counts the
 // homozygotes, N_AA = sum of the recoded genotypes; with S = 2 N A1FREQ the additive sum, N_RA = S - 2 N_AA and
@@ -955,19 +974,14 @@ struct GenoCounts {
   bool on = false;
   Recode rec;
   std::vector<uint8_t> rows;
-  std::vector<double> af, mac, af_all, mac_all, stat, beta, se, chisq, scale;
-  std::vector<int32_t> ns, ns_all, flags;
+  S2Results r;
   std::vector<long> n_aa;
-  rg_s2_out out;
   GenoCounts(bool on_, int bsz, int P, size_t row_bytes, bool ref_first) : on(on_), rec(2, ref_first) {
     if (on) {
       rows.resize((size_t)bsz * row_bytes);
-      const size_t bp = (size_t)bsz * P;
-      af.resize(bp); mac.resize(bp); stat.resize(bp); beta.resize(bp); se.resize(bp); chisq.resize(bp); ns.resize(bp);
-      af_all.resize(bsz); mac_all.resize(bsz); scale.resize(bsz); ns_all.resize(bsz); flags.resize(bsz); n_aa.resize(bsz);
+      r.init(bsz, P);
+      n_aa.resize(bsz);
     }
-    out = rg_s2_out{af.data(), ns.data(), mac.data(), af_all.data(), ns_all.data(), mac_all.data(), flags.data(),
-                    scale.data(), stat.data(), beta.data(), se.data(), chisq.data()};
   }
   // `call(rows, &out)` runs the block entry point on the recoded copy with the MAC filter off
   template <typename Call>
@@ -975,8 +989,9 @@ struct GenoCounts {
     if (!on) return;
     memcpy(rows.data(), src, nbytes);
     rec.bed(rows.data(), nbytes);
+    const rg_s2_out out = r.out();
     call(rows.data(), &out);
-    for (int v = 0; v < bs; ++v) n_aa[v] = std::lround(2.0 * af_all[v] * ns_all[v]);
+    for (int v = 0; v < bs; ++v) n_aa[v] = std::lround(2.0 * r.af_all[v] * r.ns_all[v]);
   }
   // N_RR, N_RA, N_AA of variant v given the additive pass
   void counts(int v, double af_add, int n, long& n_rr, long& n_ra, long& n_aa_out) const {
@@ -1159,244 +1174,295 @@ std::vector<uint8_t> male_vector(const std::vector<int>& sex_file, const std::ve
   return m;
 }
 
-void run_step2_qt(const Params& p, Log& log) {
-  const bool use_bgen = !p.bgen.empty();
+// The Step-2 input of either trait kind: the genotype file (BGEN, or .bed / .pgen rows) after --range, the samples,
+// phenotypes, covariates and LOCO predictions, the blocks, and their prefetch.  Blocks are fetched (file read / threaded
+// BGEN inflate) one block ahead of the GPU call into two slots, block b in slot b & 1: the rg_s2_block_* calls return
+// with the results on the host, so the slot of block b is free again when block b + 2 is fetched.  The fetch thread also
+// derives from each block what its rows print:
+// - the INFO over all analysed samples (--minINFO drops a variant whose INFO is too low, src/Geno.cpp:2074) and the
+//   dosage genotype counts of --no-split, from the inflated bytes;
+// - the --htp genotype counts per trait (update_genocounts, src/Geno.cpp:2986-3018): thresholded from the inflated bytes
+//   (BgenFile::trait_counts) or popcounts over the 2-bit rows (BedTraitCounts).  A binary trait counts its cases and
+//   controls apart, a quantitative trait all its samples as one class.
+struct S2Input {
+  const Params& p;
+  const bool binary, use_bgen;
   BedFile g;
   BgenFile gg;
-  const auto excl = read_id_list(p.exclude, 1), extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2),
-             keepl = read_id_list(p.keep, 2);
-  if (use_bgen) {
-    gg.sex_specific = p.sex_specific;
-    gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keepl, p.chrs, p.bgi);
-    if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
-    log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
-  } else {
-    open_rows(p, g, excl, extr, rem, keepl, log);
-  }
-  apply_range(p, gg.snps);
-  apply_range(p, g.snps);
-  if (g.pg) apply_range(p, g.pg->snps);
-  if (p.set_range && (use_bgen ? gg.snps : g.snps).empty()) throw Fail("no variant left to include in analysis.");
-  const std::vector<Snp>& snps = use_bgen ? gg.snps : g.snps;
-  const std::vector<std::string>& keys = use_bgen ? gg.keys : g.keys;
-  const std::vector<int32_t>& sample_idx = use_bgen ? gg.sample_idx : g.sample_idx;
-  const size_t n_file = use_bgen ? gg.n_file : g.keys_file.size();
-  const SampleSet ss{keys, use_bgen ? gg.key_to_ind : g.key_to_ind};
+  const std::vector<Snp>& snps;
+  const std::vector<int32_t>& sample_idx;
+  const SampleSet ss;
+  size_t n_file = 0;
+  bool subset = false;                                       // the file holds samples that are not analysed
   Pheno ph;
   std::vector<Loco> locos;
-  load_step2_inputs(p, ss, use_bgen ? gg.ids_file : g.ids_file, sample_idx, ph, locos, log);
-  const int64_t N = ph.N;
-  const int P = ph.P;
-  const auto blocks = set_blocks(snps, p.bsize);
-  log << " * # blocks            : [" << blocks.size() << "]\n";
-
-  rg_step2_config cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.device = p.gpu; cfg.n_samples = N; cfg.n_cov = ph.C; cfg.n_pheno = P; cfg.max_block_size = p.bsize;
-  cfg.n_analyzed = ph.n_analyzed; cfg.strict_mode = ph.strict;
-  rg_handle h = nullptr;
-  HandleGuard guard{h};
-  require_device();
-  rg_check(rg_step2_create(&cfg, ph.X.data(), ph.mask.data(), ph.in_analysis.data(), &h));
-
-  S2Writers w;
-  w.open(p, ph, use_bgen);
-  std::vector<std::string>& obuf = w.obuf;                   // rows of the current block, one buffer per trait
-  std::string head_s;
-  const int bsz = p.bsize;
-  GenoCounts gc(p.no_split, bsz, P, use_bgen ? 0 : g.row_stride, p.ref_first);
-  // input blocks are fetched (file read / threaded BGEN inflate) one block ahead of the GPU call: the rg_s2_block_*
-  // calls return with the results on the host, so the buffer of block b is free again when block b+2 is fetched
-  std::vector<uint8_t> rows[2], probs[2], pmiss[2];
-  for (int k = 0; k < 2; ++k) {
-    if (use_bgen) { probs[k].resize((size_t)bsz * n_file * 2); pmiss[k].resize((size_t)bsz * n_file); }
-    else rows[k].resize((size_t)bsz * g.row_stride);
-  }
-  const int threads = p.threads > 0 ? p.threads : (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
-  // --minINFO also drops a variant whose INFO over all analysed samples is too low (src/Geno.cpp:2074): computed from the
-  // inflated bytes on the host, in the fetch thread
-  const bool use_info1 = use_bgen && (p.min_info > 0 || p.no_split);   // --no-split prints it and the dosage genotype counts
-  // --htp on dosages: thresholded genotype counts per trait (update_genocounts, src/Geno.cpp:2986-3018) from the inflated
-  // bytes, in the fetch thread (BgenFile::trait_counts)
-  // hard calls: the same counts by popcounts over the 2-bit rows (BedTraitCounts).  Both run in the fetch thread.
-  const bool htp_bgen = use_bgen && p.htp;
-  std::vector<uint8_t> htp_cls, htp_npf[2];
-  const std::vector<uint8_t> htp_male = p.htp ? male_vector(use_bgen ? gg.sex_file : g.sex_file, sample_idx) : std::vector<uint8_t>();
-  std::vector<long> htp_cnt[2];
-  BedTraitCounts btc;
-  if (p.htp) {
-    htp_cls.resize((size_t)P * N);
-    for (size_t e = 0; e < htp_cls.size(); ++e) htp_cls[e] = ph.mask[e] ? 1 : 0;
-    for (int k = 0; k < 2; ++k) htp_cnt[k].resize((size_t)bsz * P * 6);
-    if (!use_bgen) btc.init(P, false, p.ref_first, n_file, sample_idx, htp_cls.data(), htp_male.data());
-  }
-  const bool dev_inflate = use_bgen && p.gpu_inflate && gg.compression == 1 && p.test_type == 0 && !use_info1 && !htp_bgen;
-  if (use_bgen && p.gpu_inflate)
-    log << (dev_inflate ? " * bgen genotype blocks are inflated on the GPU\n"
-                        : "   -WARNING: --gpu-inflate needs zlib-compressed payloads, the additive test and no --minINFO / --no-split / --htp; inflating on the host.\n");
-  std::vector<uint8_t> comp[2];
+  std::vector<Block> blocks;
+  size_t b_first = 0;                                        // --starting-block
+  std::vector<uint8_t> male;                                 // params.sex == 1 of the kept samples
+  int threads = 1;
+  bool use_info1 = false, htp_bgen = false, dev_inflate = false, pgen_dev = false;
+  std::vector<uint8_t> rows[2], probs[2], pmiss[2], comp[2];
   std::vector<uint64_t> comp_offs[2];
-  std::vector<double> info1[2];
-  std::vector<long> d_rr[2], d_aa[2];
-  if (use_info1) for (int k = 0; k < 2; ++k) { info1[k].resize(bsz); d_rr[k].resize(bsz); d_aa[k].resize(bsz); }
-  // .pgen records are expanded on the GPU unless an option edits the rows on the host (see pgen_on_device)
-  const bool pgen_dev = !use_bgen && g.pg && pgen_on_device() && !p.no_split && !p.htp && p.test_type == 0;
-  if (pgen_dev) log << " * pgen records are decoded on the GPU\n";
   PgenBatch pbatch[2];
+  std::vector<double> info1[2];
+  std::vector<long> d_rr[2], d_aa[2], htp_cnt[2];
+  std::vector<uint8_t> htp_cls, htp_npf[2], npf;
+  BedTraitCounts btc;
   std::future<void> pending;
-  auto fetch = [&](size_t b) {
-    return std::async(std::launch::async, [&, b] {
-      if (dev_inflate) gg.read_block_compressed(blocks[b].first, blocks[b].size, comp[b & 1], comp_offs[b & 1]);
+
+  S2Input(const Params& p_, bool binary_, Log& log)
+      : p(p_), binary(binary_), use_bgen(!p_.bgen.empty()), snps(use_bgen ? gg.snps : g.snps),
+        sample_idx(use_bgen ? gg.sample_idx : g.sample_idx),
+        ss{use_bgen ? gg.keys : g.keys, use_bgen ? gg.key_to_ind : g.key_to_ind} {
+    const auto excl = read_id_list(p.exclude, 1), extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2),
+               keep = read_id_list(p.keep, 2);
+    if (use_bgen) {
+      gg.sex_specific = p.sex_specific;
+      gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keep, p.chrs, p.bgi);
+      if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
+      log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
+    } else {
+      open_rows(p, g, excl, extr, rem, keep, log);
+    }
+    apply_range(p, gg.snps);
+    apply_range(p, g.snps);
+    if (g.pg) apply_range(p, g.pg->snps);
+    if (p.set_range && snps.empty()) throw Fail("no variant left to include in analysis.");
+    n_file = use_bgen ? gg.n_file : g.keys_file.size();
+    subset = ss.keys.size() != n_file;
+    load_step2_inputs(p, ss, use_bgen ? gg.ids_file : g.ids_file, sample_idx, ph, locos, log);
+    blocks = set_blocks(snps, p.bsize);
+    log << " * # blocks            : [" << blocks.size() << "]\n";
+    male = male_vector(use_bgen ? gg.sex_file : g.sex_file, sample_idx);
+  }
+
+  // a Step-2 handle over the analysed samples with the per-trait sample masks `mask` [P][N]
+  void create_handle(const uint8_t* mask, bool strict, rg_handle* h) const {
+    rg_step2_config cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.device = p.gpu; cfg.n_samples = ph.N; cfg.n_cov = ph.C; cfg.n_pheno = ph.P; cfg.max_block_size = p.bsize;
+    cfg.n_analyzed = ph.n_analyzed; cfg.strict_mode = strict;
+    rg_check(rg_step2_create(&cfg, ph.X.data(), mask, ph.in_analysis.data(), h));
+  }
+
+  // buffers, the decode choices and the fetch of the first block; runs once the handles exist
+  void start(Log& log) {
+    const int bsz = p.bsize, P = ph.P;
+    threads = p.threads > 0 ? p.threads : (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
+    for (int k = 0; k < 2; ++k) {
+      if (use_bgen) { probs[k].resize((size_t)bsz * n_file * 2); pmiss[k].resize((size_t)bsz * n_file); }
+      else rows[k].resize((size_t)bsz * g.row_stride);
+    }
+    use_info1 = use_bgen && (p.min_info > 0 || p.no_split);   // --no-split prints it and the dosage genotype counts
+    htp_bgen = use_bgen && p.htp;
+    if (p.htp) {
+      htp_cls.resize((size_t)P * ph.N);                      // 0 = not in the trait, 1 = in it (a control), 2 = a case
+      for (size_t e = 0; e < htp_cls.size(); ++e) htp_cls[e] = !ph.mask[e] ? 0 : (binary && ph.Y_raw[e] == 1.0) ? 2 : 1;
+      for (int k = 0; k < 2; ++k) htp_cnt[k].resize((size_t)bsz * P * 6);
+      if (!use_bgen) btc.init(P, binary, p.ref_first, n_file, sample_idx, htp_cls.data(), male.data());
+    }
+    dev_inflate = use_bgen && p.gpu_inflate && gg.compression == 1 && p.test_type == 0 && !use_info1 && !htp_bgen;
+    if (use_bgen && p.gpu_inflate)
+      log << (dev_inflate ? " * bgen genotype blocks are inflated on the GPU\n"
+                          : "   -WARNING: --gpu-inflate needs zlib-compressed payloads, the additive test and no --minINFO / --no-split / --htp; inflating on the host.\n");
+    if (use_info1) for (int k = 0; k < 2; ++k) { info1[k].resize(bsz); d_rr[k].resize(bsz); d_aa[k].resize(bsz); }
+    // .pgen records are expanded on the GPU unless an option needs the rows on the host: --no-split and --htp count
+    // genotypes from them, --test recodes them, and the --af-cc handle of a binary trait reads them
+    pgen_dev = !use_bgen && g.pg && pgen_on_device() && !p.no_split && !p.htp && p.test_type == 0 && !(binary && p.af_cc);
+    if (pgen_dev) log << " * pgen records are decoded on the GPU\n";
+    if (blocks.empty()) throw Fail("no variant left to include in analysis.");
+    if (p.start_block > (int)blocks.size()) throw Fail("Starting block > number of blocks analyzed");   // src/Data.cpp:2863-2864
+    b_first = p.start_block > 1 ? (size_t)p.start_block - 1 : 0;
+    if (b_first) log << "    + skipping to block #" << p.start_block << "\n";
+    pending = fetch(b_first);
+  }
+
+  std::future<void> fetch(size_t b) {
+    return std::async(std::launch::async, [this, b] {
+      const Block& bl = blocks[b];
+      const int k = b & 1;
+      if (dev_inflate) gg.read_block_compressed(bl.first, bl.size, comp[k], comp_offs[k]);
       else if (use_bgen) {
-        gg.read_block(blocks[b].first, blocks[b].size, probs[b & 1].data(), pmiss[b & 1].data(), threads);
-        if (use_info1) gg.info_all(probs[b & 1].data(), pmiss[b & 1].data(), blocks[b].size, ph.in_analysis.data(), p.ref_first,
-                                   info1[b & 1].data(), threads, d_rr[b & 1].data(), d_aa[b & 1].data());
+        gg.read_block(bl.first, bl.size, probs[k].data(), pmiss[k].data(), threads);
+        if (use_info1) gg.info_all(probs[k].data(), pmiss[k].data(), bl.size, ph.in_analysis.data(), p.ref_first,
+                                   info1[k].data(), threads, d_rr[k].data(), d_aa[k].data());
         if (htp_bgen) {
-          const bool np = non_par_flags(p, snps, blocks[b], htp_npf[b & 1]);
-          gg.trait_counts(probs[b & 1].data(), pmiss[b & 1].data(), blocks[b].size, htp_cls.data(), P, false, p.ref_first,
-                          htp_cnt[b & 1].data(), threads, htp_male.data(), np ? htp_npf[b & 1].data() : nullptr);
+          const bool np = non_par_flags(p, snps, bl, htp_npf[k]);
+          gg.trait_counts(probs[k].data(), pmiss[k].data(), bl.size, htp_cls.data(), ph.P, binary, p.ref_first,
+                          htp_cnt[k].data(), threads, male.data(), np ? htp_npf[k].data() : nullptr);
         }
       }
-      else if (pgen_dev) g.pg->gather(blocks[b].first, blocks[b].size, pbatch[b & 1]);
+      else if (pgen_dev) g.pg->gather(bl.first, bl.size, pbatch[k]);
       else {
-        g.read_rows(blocks[b].first, blocks[b].size, rows[b & 1].data());
+        g.read_rows(bl.first, bl.size, rows[k].data());
         if (p.htp) {
-          const bool np = non_par_flags(p, snps, blocks[b], htp_npf[b & 1]);
-          btc.count(rows[b & 1].data(), g.row_stride, blocks[b].size, np ? htp_npf[b & 1].data() : nullptr, htp_cnt[b & 1].data(), threads);
+          const bool np = non_par_flags(p, snps, bl, htp_npf[k]);
+          btc.count(rows[k].data(), g.row_stride, bl.size, np ? htp_npf[k].data() : nullptr, htp_cnt[k].data(), threads);
         }
       }
     });
-  };
-  if (blocks.empty()) throw Fail("no variant left to include in analysis.");
-  if (p.start_block > (int)blocks.size()) throw Fail("Starting block > number of blocks analyzed");   // src/Data.cpp:2863-2864
-  const size_t b_first = p.start_block > 1 ? (size_t)p.start_block - 1 : 0;
-  if (b_first) log << "    + skipping to block #" << p.start_block << "\n";
-  if (!blocks.empty()) pending = fetch(b_first);
-  std::vector<double> info((size_t)bsz * P);
-  std::vector<double> af((size_t)bsz * P), mac((size_t)bsz * P), stat((size_t)bsz * P), beta((size_t)bsz * P),
-      se((size_t)bsz * P), chisq((size_t)bsz * P), af_all(bsz), mac_all(bsz), scale_fac(bsz);
-  std::vector<int32_t> ns((size_t)bsz * P), ns_all(bsz), flags(bsz);
-  rg_s2_out out{af.data(), ns.data(), mac.data(), af_all.data(), ns_all.data(), mac_all.data(), flags.data(),
-                scale_fac.data(), stat.data(), beta.data(), se.data(), chisq.data()};
-  const bool subset = keys.size() != n_file;
+  }
+
+  // waits for block b and starts the fetch of block b + 1
+  void next(size_t b) {
+    pending.get();
+    if (b + 1 < blocks.size()) pending = fetch(b + 1);
+  }
+
+  const int32_t* sidx() const { return subset ? sample_idx.data() : nullptr; }
+
+  void set_non_par(rg_handle h, size_t b) {
+    if (non_par_flags(p, snps, blocks[b], npf)) rg_check(rg_s2_set_non_par(h, npf.data(), blocks[b].size));
+  }
+
+  // the dosages of block b for the block calls: the fetched bytes, or the payloads inflated on the device
+  void dosages(rg_handle h, size_t b, const uint8_t** pd, const uint8_t** md) {
+    *pd = probs[b & 1].data();
+    *md = pmiss[b & 1].data();
+    if (dev_inflate) rg_check(rg_bgen_inflate(h, comp[b & 1].data(), comp_offs[b & 1].data(), (int64_t)n_file, blocks[b].size, pd, md));
+  }
+
+  // the 2-bit rows of block b for the block calls: the fetched rows, or the .pgen records decoded on the device
+  void hard_calls(rg_handle h, size_t b, const uint8_t** r, int64_t* stride) {
+    *r = rows[b & 1].data();
+    *stride = (int64_t)g.row_stride;
+    if (pgen_dev) pgen_rows_device(h, pbatch[b & 1], blocks[b].size, (int64_t)g.pg->n_file, (int)b, r, stride);
+  }
+
+  // --test dominant / recessive: the fetched bytes of block b recoded in place for the second pass
+  void recode(const Recode& rc, size_t b) {
+    if (use_bgen) rc.probs(probs[b & 1].data(), (size_t)blocks[b].size * n_file);
+    else rc.bed(rows[b & 1].data(), (size_t)blocks[b].size * g.row_stride);
+  }
+};
+
+// print_sum_stats_head / print_sum_stats_head_htp (src/Step2_Models.cpp:2410-2426) of variant v of block b into head_s
+// and, with --no-split, the start of its row (print_sum_stats_all :2441-2493)
+void s2_row_start(const S2Input& in, size_t b, int v, const S2Results& r, const GenoCounts& gc, S2Writers& w, std::string& head_s) {
+  const Params& p = in.p;
+  const Snp& s = in.snps[in.blocks[b].first + v];
+  if (p.htp) {
+    head_s = s.id + "\t" + std::to_string(s.chrom) + "\t" + std::to_string(s.pos) + "\t" + s.allele0 + "\t" + s.allele1 + "\t";
+  } else {
+    head_s.clear();
+    head_s += std::to_string(s.chrom); head_s += ' ';
+    head_s += std::to_string(s.pos); head_s += ' ';
+    head_s += s.id; head_s += ' ';
+    head_s += s.allele0; head_s += ' ';
+    head_s += s.allele1; head_s += ' ';
+  }
+  if (!p.no_split) return;
+  long n_rr, n_ra, n_aa;
+  if (in.use_bgen) { n_rr = in.d_rr[b & 1][v]; n_aa = in.d_aa[b & 1][v]; n_ra = r.ns_all[v] - n_rr - n_aa; }
+  else gc.counts(v, r.af_all[v], r.ns_all[v], n_rr, n_ra, n_aa);
+  append_sumstats_all_start(w.obuf_all, head_s, r.af_all[v], r.ns_all[v], n_rr, n_ra, n_aa, test_name(p.test_type), in.use_bgen,
+                            in.use_bgen ? in.info1[b & 1][v] : -1.0);
+}
+
+void run_step2_qt(const Params& p, Log& log) {
+  S2Input in(p, false, log);
+  const Pheno& ph = in.ph;
+  const int64_t N = ph.N;
+  const int P = ph.P;
+  rg_handle h = nullptr;
+  HandleGuard guard{h};
+  require_device();
+  in.create_handle(ph.mask.data(), ph.strict, &h);
+
+  S2Writers w;
+  w.open(p, ph, in.use_bgen);
+  std::vector<std::string>& obuf = w.obuf;                   // rows of the current block, one buffer per trait
+  std::string head_s;
+  GenoCounts gc(p.no_split, p.bsize, P, in.use_bgen ? 0 : in.g.row_stride, p.ref_first);
+  in.start(log);
+  // --test dominant / recessive: the second pass on the recoded genotypes keeps its counts in r2 (see Recode)
+  S2Results r, r2;
+  r.init(p.bsize, P);
+  if (p.test_type) r2.init(p.bsize, P);
+  const rg_s2_out out = r.out(), out2 = r2.out(r);
+  const Recode recode(p.test_type, p.ref_first);
   // --htp: test_string + wgr_string + correction_type (src/Data.cpp:2075-2102)
   const std::string htp_model = std::string(test_name(p.test_type)) + (p.ignore_pred ? "" : "-WGR") + "-LR";
-  // second pass of --test dominant / recessive: counts go to scratch, the test columns to the arrays that are printed
-  const Recode recode(p.test_type, p.ref_first);
-  std::vector<double> af2, mac2, af_all2, mac_all2, info2;
-  std::vector<int32_t> ns2, ns_all2, flags2;
-  if (p.test_type) {
-    af2.resize((size_t)bsz * P); mac2.resize((size_t)bsz * P); info2.resize((size_t)bsz * P); ns2.resize((size_t)bsz * P);
-    af_all2.resize(bsz); mac_all2.resize(bsz); ns_all2.resize(bsz); flags2.resize(bsz);
-  }
-  rg_s2_out out2{af2.data(), ns2.data(), mac2.data(), af_all2.data(), ns_all2.data(), mac_all2.data(), flags2.data(),
-                 scale_fac.data(), stat.data(), beta.data(), se.data(), chisq.data()};
   std::vector<double> res((size_t)N * P), scf(P);
-  std::vector<uint8_t> npf;
   int cur_chr = -1;
   size_t n_ignored = 0;
-  for (size_t b = b_first; b < blocks.size(); ++b) {
-    const int chrom = blocks[b].chrom;
+  for (size_t b = in.b_first; b < in.blocks.size(); ++b) {
+    const int chrom = in.blocks[b].chrom, bs = in.blocks[b].size;
     if (chrom != cur_chr) {
       cur_chr = chrom;
       log << "Chromosome " << chrom << "\n";
       // blup_read_chr + compute_res (src/Step2_Models.cpp:96-124, src/Data.cpp:2386-2404)
       for (int i = 0; i < P; ++i) {
-        const std::vector<double> blup = blup_for_chr(locos[i], ss, ph, i, chrom);
+        const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
         double ssq = 0.0;
         for (int64_t s = 0; s < N; ++s) {
-          const double r = (ph.Y[(size_t)i * N + s] - blup[s]) * ph.mask[(size_t)i * N + s];
-          res[(size_t)i * N + s] = r;
-          ssq += r * r;
+          const double rv = (ph.Y[(size_t)i * N + s] - blup[s]) * ph.mask[(size_t)i * N + s];
+          res[(size_t)i * N + s] = rv;
+          ssq += rv * rv;
         }
         const double psd = std::sqrt(ssq) / std::sqrt(ph.neff[i] - ph.C);
         for (int64_t s = 0; s < N; ++s) res[(size_t)i * N + s] /= psd;
         scf[i] = ph.scale_Y[i] * psd;
       }
-      const std::vector<uint8_t> male = male_vector(use_bgen ? gg.sex_file : g.sex_file, sample_idx);
-      rg_check(rg_s2_set_sex(h, chrom == 23 ? male.data() : nullptr));
+      rg_check(rg_s2_set_sex(h, chrom == 23 ? in.male.data() : nullptr));
       rg_check(rg_s2_set_chr(h, res.data(), scf.data()));
     }
-    pending.get();
-    if (b + 1 < blocks.size()) pending = fetch(b + 1);
-    if (!use_bgen)
-      gc.run(rows[b & 1].data(), (size_t)blocks[b].size * g.row_stride, blocks[b].size, [&](const uint8_t* r, const rg_s2_out* o) {
-        rg_check(rg_s2_block_bed(h, r, (int64_t)g.row_stride, blocks[b].size, subset ? sample_idx.data() : nullptr, p.ref_first, 0.0, o));
+    in.next(b);
+    if (!in.use_bgen)
+      gc.run(in.rows[b & 1].data(), (size_t)bs * in.g.row_stride, bs, [&](const uint8_t* rw, const rg_s2_out* o) {
+        rg_check(rg_s2_block_bed(h, rw, (int64_t)in.g.row_stride, bs, in.sidx(), p.ref_first, 0.0, o));
       });
-    if (non_par_flags(p, snps, blocks[b], npf)) rg_check(rg_s2_set_non_par(h, npf.data(), blocks[b].size));
-    if (use_bgen) {
-      const uint8_t *pd = probs[b & 1].data(), *md = pmiss[b & 1].data();
-      if (dev_inflate) rg_check(rg_bgen_inflate(h, comp[b & 1].data(), comp_offs[b & 1].data(), (int64_t)n_file, blocks[b].size, &pd, &md));
-      rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)n_file, blocks[b].size,
-                                 subset ? sample_idx.data() : nullptr, p.ref_first, p.min_mac, &out, info.data()));
+    in.set_non_par(h, b);
+    if (in.use_bgen) {
+      const uint8_t *pd, *md;
+      in.dosages(h, b, &pd, &md);
+      rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, p.min_mac, &out, r.info.data()));
       if (p.test_type) {
-        recode.probs(probs[b & 1].data(), (size_t)blocks[b].size * n_file);
-        rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)n_file, blocks[b].size, subset ? sample_idx.data() : nullptr, p.ref_first,
-                                   0.0, &out2, info2.data()));
+        in.recode(recode, b);
+        rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &out2, r2.info.data()));
       }
-    } else if (pgen_dev) {
-      const uint8_t* drows = nullptr;
-      int64_t dstride = 0;
-      pgen_rows_device(h, pbatch[b & 1], blocks[b].size, (int64_t)g.pg->n_file, (int)b, &drows, &dstride);
-      rg_check(rg_s2_block_bed(h, drows, dstride, blocks[b].size, subset ? sample_idx.data() : nullptr, p.ref_first, p.min_mac, &out));
     } else {
-      rg_check(rg_s2_block_bed(h, rows[b & 1].data(), (int64_t)g.row_stride, blocks[b].size,
-                               subset ? sample_idx.data() : nullptr, p.ref_first, p.min_mac, &out));
+      const uint8_t* rows;
+      int64_t stride;
+      in.hard_calls(h, b, &rows, &stride);
+      rg_check(rg_s2_block_bed(h, rows, stride, bs, in.sidx(), p.ref_first, p.min_mac, &out));
       if (p.test_type) {
-        recode.bed(rows[b & 1].data(), (size_t)blocks[b].size * g.row_stride);
-        rg_check(rg_s2_block_bed(h, rows[b & 1].data(), (int64_t)g.row_stride, blocks[b].size,
-                                 subset ? sample_idx.data() : nullptr, p.ref_first, 0.0, &out2));
+        in.recode(recode, b);
+        rg_check(rg_s2_block_bed(h, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &out2));
       }
     }
-    if (p.test_type) merge_recode_flags(blocks[b].size, flags.data(), flags2.data(), af_all2.data());
-    for (int v = 0; v < blocks[b].size; ++v) {
-      if (flags[v] & 3) { ++n_ignored; continue; }            // no row for ignored variants (split mode)
-      if (use_info1 && p.min_info > 0 && info1[b & 1][v] < p.min_info) { ++n_ignored; continue; }
-      const Snp& s = snps[blocks[b].first + v];
-      head_s.clear();                                        // print_sum_stats_head, src/Step2_Models.cpp:2410-2418
-      head_s += std::to_string(s.chrom); head_s += ' ';
-      head_s += std::to_string(s.pos); head_s += ' ';
-      head_s += s.id; head_s += ' ';
-      head_s += s.allele0; head_s += ' ';
-      head_s += s.allele1; head_s += ' ';
-      if (p.htp) {                                             // print_sum_stats_head_htp :2419-2426
-        head_s = s.id + "\t" + std::to_string(s.chrom) + "\t" + std::to_string(s.pos) + "\t" + s.allele0 + "\t" + s.allele1 + "\t";
-      }
-      if (p.no_split) {                                        // print_sum_stats_all :2441-2493
-        long n_rr, n_ra, n_aa;
-        if (use_bgen) { n_rr = d_rr[b & 1][v]; n_aa = d_aa[b & 1][v]; n_ra = ns_all[v] - n_rr - n_aa; }
-        else gc.counts(v, af_all[v], ns_all[v], n_rr, n_ra, n_aa);
-        append_sumstats_all_start(w.obuf_all, head_s, af_all[v], ns_all[v], n_rr, n_ra, n_aa, test_name(p.test_type), use_bgen,
-                                  use_bgen ? info1[b & 1][v] : -1.0);
-      }
+    if (p.test_type) merge_recode_flags(bs, r.flags.data(), r2.flags.data(), r2.af_all.data());
+    for (int v = 0; v < bs; ++v) {
+      if (r.flags[v] & 3) { ++n_ignored; continue; }          // no row for ignored variants (split mode)
+      if (in.use_info1 && p.min_info > 0 && in.info1[b & 1][v] < p.min_info) { ++n_ignored; continue; }
+      s2_row_start(in, b, v, r, gc, w, head_s);
       for (int i = 0; i < P; ++i) {
         const size_t e = (size_t)v * P + i;
-        const bool have = !(mac[e] < p.min_mac) &&             // ignored_trait (src/Geno.cpp:3102)
-                          !(use_bgen && info[e] < p.min_info);  // --minINFO (src/Geno.cpp:3142-3146)
-        if (p.no_split) { append_sumstats_all_trait(w.obuf_all, have, beta[e], se[e], chisq[e], get_logp(chisq[e]), true); continue; }
+        const bool have = !(r.mac[e] < p.min_mac) &&           // ignored_trait (src/Geno.cpp:3102)
+                          !(in.use_bgen && r.info[e] < p.min_info);   // --minINFO (src/Geno.cpp:3142-3146)
+        if (p.no_split) { append_sumstats_all_trait(w.obuf_all, have, r.beta[e], r.se[e], r.chisq[e], get_logp(r.chisq[e]), true); continue; }
         if (!have) continue;
         if (p.htp) {
-          // print_sum_stats_htp for a quantitative trait.  Genotype counts of the trait's samples (update_genocounts,
-          // src/Geno.cpp:2986-3003) counted on the host in the fetch thread (BedTraitCounts / BgenFile::trait_counts).
-          // SCORE / SKATV are the numerator and denominator of the statistic (dt_thr->scores / skat_var,
-          // src/Step2_Models.cpp:391-394, :421-424): se = scf / sqrt(denum), stat = num / sqrt(denum).
-          HtpRow r;
-          r.model = htp_model.c_str();
-          r.beta = beta[e]; r.se = se[e]; r.chisq = chisq[e]; r.logp = get_logp(chisq[e]); r.af = af[e]; r.mac = mac[e];
-          for (int k = 0; k < 3; ++k) r.gc[k] = htp_cnt[b & 1][e * 6 + k];
-          if (use_bgen) r.info = info[e];                      // dosages: the trait's INFO
-          const double sqrt_den = scf[i] / se[e];
-          r.score = stat[e] * sqrt_den; r.skat_var = sqrt_den * sqrt_den;
-          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, r);
+          // print_sum_stats_htp for a quantitative trait, with the genotype counts of the trait's samples.  SCORE / SKATV
+          // are the numerator and denominator of the statistic (dt_thr->scores / skat_var, src/Step2_Models.cpp:391-394,
+          // :421-424): se = scf / sqrt(denum), stat = num / sqrt(denum).
+          HtpRow hr;
+          hr.model = htp_model.c_str();
+          hr.beta = r.beta[e]; hr.se = r.se[e]; hr.chisq = r.chisq[e]; hr.logp = get_logp(r.chisq[e]); hr.af = r.af[e]; hr.mac = r.mac[e];
+          for (int k = 0; k < 3; ++k) hr.gc[k] = in.htp_cnt[b & 1][e * 6 + k];
+          if (in.use_bgen) hr.info = r.info[e];                // dosages: the trait's INFO
+          const double sqrt_den = scf[i] / r.se[e];
+          hr.score = r.stat[e] * sqrt_den; hr.skat_var = sqrt_den * sqrt_den;
+          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, hr);
           continue;
         }
-        append_sumstats_row(obuf[i], head_s, af[e], use_bgen, use_bgen ? info[e] : -1.0, ns[e], test_name(p.test_type), beta[e], se[e], chisq[e],
-                            get_logp(chisq[e]), true);   // print_sum_stats_single :2502-2540
+        append_sumstats_row(obuf[i], head_s, r.af[e], in.use_bgen, in.use_bgen ? r.info[e] : -1.0, r.ns[e], test_name(p.test_type),
+                            r.beta[e], r.se[e], r.chisq[e], get_logp(r.chisq[e]), true);   // print_sum_stats_single :2502-2540
       }
       if (p.no_split) w.obuf_all += " NA\n";
     }
     w.flush();
-    log << " block [" << b + 1 << "/" << blocks.size() << "] : done\n";
+    log << " block [" << b + 1 << "/" << in.blocks.size() << "] : done\n";
   }
   w.close();
   log << "\nNumber of ignored tests due to low MAC or low variance : " << n_ignored << "\n";
@@ -1406,35 +1472,10 @@ void run_step2_qt(const Params& p, Log& log) {
 // Control flow of Data::test_snps_fast for trait_mode 1 (src/Data.cpp:2230-2383): per chromosome the null
 // logistic / null Firth fits (host, O(N C^2)), per block the score test and the Firth fallback (GPU).
 void run_step2_bt(const Params& p, Log& log) {
-  const bool use_bgen = !p.bgen.empty();
-  BedFile gb;
-  BgenFile gg;
-  const auto excl = read_id_list(p.exclude, 1), extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2),
-             keep = read_id_list(p.keep, 2);
-  if (use_bgen) {
-    gg.sex_specific = p.sex_specific;
-    gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keep, p.chrs, p.bgi);
-    if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
-    log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
-  } else {
-    open_rows(p, gb, excl, extr, rem, keep, log);
-  }
-  apply_range(p, gg.snps);
-  apply_range(p, gb.snps);
-  if (gb.pg) apply_range(p, gb.pg->snps);
-  if (p.set_range && (use_bgen ? gg.snps : gb.snps).empty()) throw Fail("no variant left to include in analysis.");
-  const std::vector<Snp>& snps = use_bgen ? gg.snps : gb.snps;
-  const std::vector<std::string>& keys = use_bgen ? gg.keys : gb.keys;
-  const std::vector<int32_t>& sample_idx = use_bgen ? gg.sample_idx : gb.sample_idx;
-  const size_t n_file = use_bgen ? gg.n_file : gb.keys_file.size();
-  const SampleSet ss{keys, use_bgen ? gg.key_to_ind : gb.key_to_ind};
-  Pheno ph;
-  std::vector<Loco> locos;
-  load_step2_inputs(p, ss, use_bgen ? gg.ids_file : gb.ids_file, sample_idx, ph, locos, log);
+  S2Input in(p, true, log);
+  const Pheno& ph = in.ph;
   const int64_t N = ph.N;
   const int P = ph.P, C = ph.C;
-  const auto blocks = set_blocks(snps, p.bsize);
-  log << " * # blocks            : [" << blocks.size() << "]\n";
   const double z_thr = z_threshold(p.p_thresh);
   // --htp: test_string + wgr_string + correction_type (src/Data.cpp:2075-2102)
   const std::string htp_model = std::string(test_name(p.test_type)) + (p.ignore_pred ? "" : "-WGR") + (p.firth ? "-FIRTH" : p.spa ? "-SPA" : "-LOG");
@@ -1459,124 +1500,42 @@ void run_step2_bt(const Params& p, Log& log) {
   }
   if (p.spa) log << " * using SPA correction for logistic regression p-values less than " << p.p_thresh << "\n";
 
-  rg_step2_config cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.device = p.gpu; cfg.n_samples = N; cfg.n_cov = C; cfg.n_pheno = P; cfg.max_block_size = p.bsize;
-  cfg.n_analyzed = ph.n_analyzed; cfg.strict_mode = ph.strict;
   rg_handle h = nullptr;
   HandleGuard guard{h};
   require_device();
-  rg_check(rg_step2_create(&cfg, ph.X.data(), ph.mask.data(), ph.in_analysis.data(), &h));
+  in.create_handle(ph.mask.data(), ph.strict, &h);
 
   S2Writers w;
-  w.open(p, ph, use_bgen);
+  w.open(p, ph, in.use_bgen);
   std::vector<std::string>& obuf = w.obuf;                   // rows of the current block, one buffer per trait
   std::string head_s;
-  const int bsz = p.bsize;
-  GenoCounts gc(p.no_split, bsz, P, use_bgen ? 0 : gb.row_stride, p.ref_first);
+  GenoCounts gc(p.no_split, p.bsize, P, in.use_bgen ? 0 : in.g.row_stride, p.ref_first);
   // --af-cc (update_af_cc / compute_aaf_info, src/Geno.cpp:3069-3075, :3120-3127): a second handle whose sample masks are
   // the cases of each trait returns their allele frequency and count from the same block bytes; controls follow by
   // difference of the (exactly reconstructed) allele sums.
   rg_handle hc = nullptr;
   HandleGuard guard_cases{hc};
-  std::vector<double> afc, macc, afc_all, macc_all, statc, betac, sec, chisqc, scalec, infoc;
-  std::vector<int32_t> nsc, nsc_all, flagsc;
+  S2Results rc;
   if (p.af_cc) {
     std::vector<uint8_t> mask_case(ph.mask.size());
     for (size_t e = 0; e < mask_case.size(); ++e) mask_case[e] = ph.mask[e] && ph.Y_raw[e] == 1.0;
-    rg_step2_config cfgc = cfg;
-    cfgc.strict_mode = 0;                                    // per-trait masks differ from the analysis set here
-    rg_check(rg_step2_create(&cfgc, ph.X.data(), mask_case.data(), ph.in_analysis.data(), &hc));
+    in.create_handle(mask_case.data(), false, &hc);          // not strict: per-trait masks differ from the analysis set here
     const std::vector<double> zero((size_t)N * P, 0.0), one(P, 1.0);
     rg_check(rg_s2_set_chr(hc, zero.data(), one.data()));
-    const size_t bp = (size_t)bsz * P;
-    afc.resize(bp); macc.resize(bp); statc.resize(bp); betac.resize(bp); sec.resize(bp); chisqc.resize(bp); infoc.resize(bp); nsc.resize(bp);
-    afc_all.resize(bsz); macc_all.resize(bsz); scalec.resize(bsz); nsc_all.resize(bsz); flagsc.resize(bsz);
+    rc.init(p.bsize, P);
   }
-  rg_s2_out outc{afc.data(), nsc.data(), macc.data(), afc_all.data(), nsc_all.data(), macc_all.data(), flagsc.data(),
-                 scalec.data(), statc.data(), betac.data(), sec.data(), chisqc.data()};
-  const double unit = use_bgen ? 255.0 : 1.0;                // allele sums are multiples of 1 / unit
-  const int threads = p.threads > 0 ? p.threads : (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
-  std::vector<uint8_t> probs[2], pmiss[2], rows[2];          // fetched one block ahead of the GPU call, like the QT path
-  for (int k = 0; k < 2; ++k) {
-    if (use_bgen) { probs[k].resize((size_t)bsz * n_file * 2); pmiss[k].resize((size_t)bsz * n_file); }
-    else rows[k].resize((size_t)bsz * gb.row_stride);
-  }
-  const bool use_info1 = use_bgen && (p.min_info > 0 || p.no_split);   // variant-level --minINFO / --no-split, see run_step2_qt
-  // --htp on dosages: thresholded genotype counts of the cases and controls of each trait (BgenFile::trait_counts)
-  // hard calls: the same by popcounts over the 2-bit rows (BedTraitCounts)
-  const bool htp_bgen = use_bgen && p.htp;
-  std::vector<uint8_t> htp_cls, htp_npf[2];
-  const std::vector<uint8_t> htp_male = p.htp ? male_vector(use_bgen ? gg.sex_file : gb.sex_file, sample_idx) : std::vector<uint8_t>();
-  std::vector<long> htp_cnt[2];
-  BedTraitCounts btc;
-  if (p.htp) {
-    htp_cls.resize((size_t)P * N);
-    for (size_t e = 0; e < htp_cls.size(); ++e) htp_cls[e] = !ph.mask[e] ? 0 : ph.Y_raw[e] == 1.0 ? 2 : 1;
-    for (int k = 0; k < 2; ++k) htp_cnt[k].resize((size_t)bsz * P * 6);
-    if (!use_bgen) btc.init(P, true, p.ref_first, n_file, sample_idx, htp_cls.data(), htp_male.data());
-  }
-  const bool dev_inflate = use_bgen && p.gpu_inflate && gg.compression == 1 && p.test_type == 0 && !use_info1 && !htp_bgen;
-  if (use_bgen && p.gpu_inflate)
-    log << (dev_inflate ? " * bgen genotype blocks are inflated on the GPU\n"
-                        : "   -WARNING: --gpu-inflate needs zlib-compressed payloads, the additive test and no --minINFO / --no-split / --htp; inflating on the host.\n");
-  std::vector<uint8_t> comp[2];
-  std::vector<uint64_t> comp_offs[2];
-  std::vector<double> info1[2];
-  std::vector<long> d_rr[2], d_aa[2];
-  if (use_info1) for (int k = 0; k < 2; ++k) { info1[k].resize(bsz); d_rr[k].resize(bsz); d_aa[k].resize(bsz); }
-  const bool pgen_dev = !use_bgen && gb.pg && pgen_on_device() && !p.no_split && !p.htp && p.test_type == 0 && !hc;   // --htp counts on host rows
-  if (pgen_dev) log << " * pgen records are decoded on the GPU\n";
-  PgenBatch pbatch[2];
-  std::future<void> pending;
-  auto fetch = [&](size_t b) {
-    return std::async(std::launch::async, [&, b] {
-      if (dev_inflate) gg.read_block_compressed(blocks[b].first, blocks[b].size, comp[b & 1], comp_offs[b & 1]);
-      else if (use_bgen) {
-        gg.read_block(blocks[b].first, blocks[b].size, probs[b & 1].data(), pmiss[b & 1].data(), threads);
-        if (use_info1) gg.info_all(probs[b & 1].data(), pmiss[b & 1].data(), blocks[b].size, ph.in_analysis.data(), p.ref_first,
-                                   info1[b & 1].data(), threads, d_rr[b & 1].data(), d_aa[b & 1].data());
-        if (htp_bgen) {
-          const bool np = non_par_flags(p, snps, blocks[b], htp_npf[b & 1]);
-          gg.trait_counts(probs[b & 1].data(), pmiss[b & 1].data(), blocks[b].size, htp_cls.data(), P, true, p.ref_first,
-                          htp_cnt[b & 1].data(), threads, htp_male.data(), np ? htp_npf[b & 1].data() : nullptr);
-        }
-      }
-      else if (pgen_dev) gb.pg->gather(blocks[b].first, blocks[b].size, pbatch[b & 1]);
-      else {
-        gb.read_rows(blocks[b].first, blocks[b].size, rows[b & 1].data());
-        if (p.htp) {
-          const bool np = non_par_flags(p, snps, blocks[b], htp_npf[b & 1]);
-          btc.count(rows[b & 1].data(), gb.row_stride, blocks[b].size, np ? htp_npf[b & 1].data() : nullptr, htp_cnt[b & 1].data(), threads);
-        }
-      }
-    });
-  };
-  if (blocks.empty()) throw Fail("no variant left to include in analysis.");
-  if (p.start_block > (int)blocks.size()) throw Fail("Starting block > number of blocks analyzed");   // src/Data.cpp:2863-2864
-  const size_t b_first = p.start_block > 1 ? (size_t)p.start_block - 1 : 0;
-  if (b_first) log << "    + skipping to block #" << p.start_block << "\n";
-  if (!blocks.empty()) pending = fetch(b_first);
-  std::vector<double> af((size_t)bsz * P), mac((size_t)bsz * P), stat((size_t)bsz * P), beta((size_t)bsz * P),
-      se((size_t)bsz * P), chisq((size_t)bsz * P), info((size_t)bsz * P), af_all(bsz), mac_all(bsz), scale_fac(bsz);
-  std::vector<int32_t> ns((size_t)bsz * P), ns_all(bsz), flags(bsz);
-  rg_s2_out out{af.data(), ns.data(), mac.data(), af_all.data(), ns_all.data(), mac_all.data(), flags.data(),
-                scale_fac.data(), stat.data(), beta.data(), se.data(), chisq.data()};
-  const bool subset = keys.size() != n_file;
-  const Recode recode(p.test_type, p.ref_first);             // --test dominant / recessive: see run_step2_qt
-  std::vector<double> af2, mac2, af_all2, mac_all2, info2;
-  std::vector<int32_t> ns2, ns_all2, flags2;
-  if (p.test_type) {
-    af2.resize((size_t)bsz * P); mac2.resize((size_t)bsz * P); info2.resize((size_t)bsz * P); ns2.resize((size_t)bsz * P);
-    af_all2.resize(bsz); mac_all2.resize(bsz); ns_all2.resize(bsz); flags2.resize(bsz);
-  }
-  rg_s2_out out2{af2.data(), ns2.data(), mac2.data(), af_all2.data(), ns_all2.data(), mac_all2.data(), flags2.data(),
-                 scale_fac.data(), stat.data(), beta.data(), se.data(), chisq.data()};
-  std::vector<uint8_t> npf;
+  const rg_s2_out outc = rc.out();
+  const double unit = in.use_bgen ? 255.0 : 1.0;             // allele sums are multiples of 1 / unit
+  in.start(log);
+  S2Results r, r2;                                           // r2: counts of the --test recode pass, see run_step2_qt
+  r.init(p.bsize, P);
+  if (p.test_type) r2.init(p.bsize, P);
+  const rg_s2_out out = r.out(), out2 = r2.out(r);
+  const Recode recode(p.test_type, p.ref_first);
   int cur_chr = -1;
   size_t n_ignored = 0, n_firth = 0, n_fail = 0;
-  for (size_t b = b_first; b < blocks.size(); ++b) {
-    const int chrom = blocks[b].chrom, bs = blocks[b].size;
+  for (size_t b = in.b_first; b < in.blocks.size(); ++b) {
+    const int chrom = in.blocks[b].chrom, bs = in.blocks[b].size;
     if (chrom != cur_chr) {
       cur_chr = chrom;
       log << "Chromosome " << chrom << "\n";
@@ -1584,7 +1543,7 @@ void run_step2_bt(const Params& p, Log& log) {
       if (p.firth) off.resize((size_t)P * N);
       if (p.spa) yhat.resize((size_t)P * N);
       for (int i = 0; i < P; ++i) {
-        const std::vector<double> blup = blup_for_chr(locos[i], ss, ph, i, chrom);
+        const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
         // --use-null-firth: starting values of this chromosome from the Step-1 file (get_beta_start_firth, :1936-1980)
         std::vector<double> fstart;
         if (p.firth && !null_firth_files.empty() && !null_firth_files[i].empty()) {
@@ -1612,51 +1571,40 @@ void run_step2_bt(const Params& p, Log& log) {
         if (p.firth) std::copy(nm.firth_offset.begin(), nm.firth_offset.end(), off.begin() + (size_t)i * N);
         if (p.spa) std::copy(nm.y_hat_p.begin(), nm.y_hat_p.end(), yhat.begin() + (size_t)i * N);
       }
-      const std::vector<uint8_t> male = male_vector(use_bgen ? gg.sex_file : gb.sex_file, sample_idx);
-      rg_check(rg_s2_set_sex(h, chrom == 23 ? male.data() : nullptr));
+      rg_check(rg_s2_set_sex(h, chrom == 23 ? in.male.data() : nullptr));
       rg_s2_bt_chr st{gsm.data(), gs.data(), yres.data(), xg.data(), ph.Y_raw.data(), p.firth ? off.data() : nullptr,
                       p.spa ? yhat.data() : nullptr};
       rg_check(rg_s2_set_chr_bt(h, &st));
     }
-    pending.get();
-    if (b + 1 < blocks.size()) pending = fetch(b + 1);
-    if (!use_bgen)
-      gc.run(rows[b & 1].data(), (size_t)bs * gb.row_stride, bs, [&](const uint8_t* r, const rg_s2_out* o) {
-        rg_check(rg_s2_block_bed_bt(h, r, (int64_t)gb.row_stride, bs, subset ? sample_idx.data() : nullptr, p.ref_first, 0.0, o));
+    in.next(b);
+    if (!in.use_bgen)
+      gc.run(in.rows[b & 1].data(), (size_t)bs * in.g.row_stride, bs, [&](const uint8_t* rw, const rg_s2_out* o) {
+        rg_check(rg_s2_block_bed_bt(h, rw, (int64_t)in.g.row_stride, bs, in.sidx(), p.ref_first, 0.0, o));
       });
-    if (non_par_flags(p, snps, blocks[b], npf)) rg_check(rg_s2_set_non_par(h, npf.data(), bs));
-    if (use_bgen) {
-      const uint8_t *pd = probs[b & 1].data(), *md = pmiss[b & 1].data();
-      if (dev_inflate) rg_check(rg_bgen_inflate(h, comp[b & 1].data(), comp_offs[b & 1].data(), (int64_t)n_file, bs, &pd, &md));
-      rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)n_file, bs,
-                                    subset ? sample_idx.data() : nullptr, p.ref_first, p.min_mac, &out, info.data()));
-      if (hc) rg_check(rg_s2_block_bgen8(hc, pd, md, (int64_t)n_file, bs, subset ? sample_idx.data() : nullptr, p.ref_first, 0.0,
-                                         &outc, infoc.data()));
+    in.set_non_par(h, b);
+    if (in.use_bgen) {
+      const uint8_t *pd, *md;
+      in.dosages(h, b, &pd, &md);
+      rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, p.min_mac, &out, r.info.data()));
+      if (hc) rg_check(rg_s2_block_bgen8(hc, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &outc, rc.info.data()));
       if (p.test_type) {
-        recode.probs(probs[b & 1].data(), (size_t)bs * n_file);
-        rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)n_file, bs, subset ? sample_idx.data() : nullptr, p.ref_first, 0.0,
-                                      &out2, info2.data()));
+        in.recode(recode, b);
+        rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &out2, r2.info.data()));
       }
-    } else if (pgen_dev) {
-      const uint8_t* drows = nullptr;
-      int64_t dstride = 0;
-      pgen_rows_device(h, pbatch[b & 1], bs, (int64_t)gb.pg->n_file, (int)b, &drows, &dstride);
-      rg_check(rg_s2_block_bed_bt(h, drows, dstride, bs, subset ? sample_idx.data() : nullptr, p.ref_first, p.min_mac, &out));
     } else {
-      // hard calls go to the GPU as they are (2 bits per sample)
-      rg_check(rg_s2_block_bed_bt(h, rows[b & 1].data(), (int64_t)gb.row_stride, bs, subset ? sample_idx.data() : nullptr,
-                                  p.ref_first, p.min_mac, &out));
-      if (hc) rg_check(rg_s2_block_bed(hc, rows[b & 1].data(), (int64_t)gb.row_stride, bs, subset ? sample_idx.data() : nullptr,
-                                       p.ref_first, 0.0, &outc));
+      const uint8_t* rows;
+      int64_t stride;
+      in.hard_calls(h, b, &rows, &stride);
+      rg_check(rg_s2_block_bed_bt(h, rows, stride, bs, in.sidx(), p.ref_first, p.min_mac, &out));
+      if (hc) rg_check(rg_s2_block_bed(hc, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &outc));
       if (p.test_type) {
-        recode.bed(rows[b & 1].data(), (size_t)bs * gb.row_stride);
-        rg_check(rg_s2_block_bed_bt(h, rows[b & 1].data(), (int64_t)gb.row_stride, bs, subset ? sample_idx.data() : nullptr,
-                                    p.ref_first, 0.0, &out2));
+        in.recode(recode, b);
+        rg_check(rg_s2_block_bed_bt(h, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &out2));
       }
     }
-    if (p.test_type) merge_recode_flags(bs, flags.data(), flags2.data(), af_all2.data());
-    if (use_info1)                                           // ignored_snp: counts as one ignored variant, no Firth / SPA
-      for (int v = 0; v < bs; ++v) if (p.min_info > 0 && info1[b & 1][v] < p.min_info) flags[v] |= 1;
+    if (p.test_type) merge_recode_flags(bs, r.flags.data(), r2.flags.data(), r2.af_all.data());
+    if (in.use_info1)                                        // ignored_snp: counts as one ignored variant, no Firth / SPA
+      for (int v = 0; v < bs; ++v) if (p.min_info > 0 && in.info1[b & 1][v] < p.min_info) r.flags[v] |= 1;
     // Firth fallback for |z| above the --pThresh threshold (check_pval_snp, src/Step2_Models.cpp:1988-2041)
     std::vector<int32_t> sel_v, sel_t, fstatus;
     std::vector<double> fbeta, fse, flrt;
@@ -1664,10 +1612,10 @@ void run_step2_bt(const Params& p, Log& log) {
     std::map<std::pair<int, int>, double> spa_logp;
     if (p.firth || p.spa) {
       for (int v = 0; v < bs; ++v) {
-        if (flags[v] & (1 | 16)) continue;
+        if (r.flags[v] & (1 | 16)) continue;
         for (int i = 0; i < P; ++i) {
           const size_t e = (size_t)v * P + i;
-          if (mac[e] < p.min_mac || !(std::fabs(stat[e]) > z_thr)) continue;
+          if (r.mac[e] < p.min_mac || !(std::fabs(r.stat[e]) > z_thr)) continue;
           fidx[{v, i}] = (int)sel_v.size();
           sel_v.push_back(v); sel_t.push_back(i);
         }
@@ -1684,40 +1632,24 @@ void run_step2_bt(const Params& p, Log& log) {
           const size_t e = (size_t)sel_v[k] * P + sel_t[k];
           const double pval = std::max(10.0 * std::numeric_limits<double>::min(), pv[k]);
           flrt[k] = chisq1_from_pvalue(pval);
-          fse[k] = se[e];
-          fbeta[k] = (beta[e] < 0 ? -1.0 : 1.0) * std::sqrt(flrt[k]) * se[e];
+          fse[k] = r.se[e];
+          fbeta[k] = (r.beta[e] < 0 ? -1.0 : 1.0) * std::sqrt(flrt[k]) * r.se[e];
           spa_logp[{sel_v[k], sel_t[k]}] = -std::log10(pval);
         }
       }
       n_firth += nsel;
     }
     for (int v = 0; v < bs; ++v) {
-      if (flags[v] & (1 | 16)) { ++n_ignored; continue; }
-      const Snp& s = snps[blocks[b].first + v];
-      head_s.clear();                                        // print_sum_stats_head, src/Step2_Models.cpp:2410-2418
-      head_s += std::to_string(s.chrom); head_s += ' ';
-      head_s += std::to_string(s.pos); head_s += ' ';
-      head_s += s.id; head_s += ' ';
-      head_s += s.allele0; head_s += ' ';
-      head_s += s.allele1; head_s += ' ';
-      if (p.htp) {                                             // print_sum_stats_head_htp :2419-2426
-        head_s = s.id + "\t" + std::to_string(s.chrom) + "\t" + std::to_string(s.pos) + "\t" + s.allele0 + "\t" + s.allele1 + "\t";
-      }
-      if (p.no_split) {                                        // print_sum_stats_all :2441-2493
-        long n_rr, n_ra, n_aa;
-        if (use_bgen) { n_rr = d_rr[b & 1][v]; n_aa = d_aa[b & 1][v]; n_ra = ns_all[v] - n_rr - n_aa; }
-        else gc.counts(v, af_all[v], ns_all[v], n_rr, n_ra, n_aa);
-        append_sumstats_all_start(w.obuf_all, head_s, af_all[v], ns_all[v], n_rr, n_ra, n_aa, test_name(p.test_type), use_bgen,
-                                  use_bgen ? info1[b & 1][v] : -1.0);
-      }
+      if (r.flags[v] & (1 | 16)) { ++n_ignored; continue; }
+      s2_row_start(in, b, v, r, gc, w, head_s);
       for (int i = 0; i < P; ++i) {
         const size_t e = (size_t)v * P + i;
-        const bool have = !(mac[e] < p.min_mac) && !(use_bgen && info[e] < p.min_info);   // ignored_trait, --minINFO
+        const bool have = !(r.mac[e] < p.min_mac) && !(in.use_bgen && r.info[e] < p.min_info);   // ignored_trait, --minINFO
         if (!have) {
           if (p.no_split) append_sumstats_all_trait(w.obuf_all, false, 0, 0, 0, 0, false);
           continue;
         }
-        double bo = beta[e], so = se[e], co = chisq[e];
+        double bo = r.beta[e], so = r.se[e], co = r.chisq[e];
         bool pass = true;
         auto f = fidx.find({v, i});
         if (f != fidx.end()) {
@@ -1728,38 +1660,37 @@ void run_step2_bt(const Params& p, Log& log) {
         if (p.spa && pass && f != fidx.end()) lp = spa_logp[{v, i}];   // SPA reports -log10 of its own p-value
         AfCc cc;
         if (hc) {
-          const double s_all = std::round(af[e] * 2.0 * ns[e] * unit), s_case = std::round(afc[e] * 2.0 * nsc[e] * unit);
-          cc.ns_case = nsc[e];
-          cc.ns_control = ns[e] - nsc[e];
-          cc.af_case = afc[e];
+          const double s_all = std::round(r.af[e] * 2.0 * r.ns[e] * unit), s_case = std::round(rc.af[e] * 2.0 * rc.ns[e] * unit);
+          cc.ns_case = rc.ns[e];
+          cc.ns_control = r.ns[e] - rc.ns[e];
+          cc.af_case = rc.af[e];
           cc.af_control = (s_all - s_case) / unit / (2.0 * cc.ns_control);
         }
         if (p.htp) {
-          // print_sum_stats_htp for a binary trait (src/Step2_Models.cpp:2542-2646).  Genotype counts of the trait's cases
-          // and controls (update_genocounts, src/Geno.cpp:2986-3018) counted on the host in the fetch thread (BedTraitCounts /
-          // BgenFile::trait_counts).  SCORE / SKATV (compute_score_bt :523-526, :546): stats * sqrt(denum) with the sign of the minor-allele
-          // flip undone, and denum = 1 / se^2 of the score test; cal_factor (check_pval_snp :1993, :2027) = 1 without a
-          // correction, stats^2 / corrected chi-square with one.  After a FAILED correction the reference prints whatever
-          // cal_factor the thread held before (it returns before the assignment): 1 here.
-          HtpRow r;
-          r.model = htp_model.c_str(); r.bt = true; r.firth = p.firth;
-          r.beta = bo; r.se = so; r.chisq = co; r.logp = lp; r.af = af[e]; r.mac = mac[e]; r.test_pass = pass;
-          for (int k = 0; k < 6; ++k) r.gc[k] = htp_cnt[b & 1][e * 6 + k];
-          if (use_bgen) r.info = info[e];                      // dosages: the trait's INFO
-          const double sqrt_den = 1.0 / se[e];
-          r.score = stat[e] * sqrt_den * ((flags[v] & 8) ? -1.0 : 1.0); r.skat_var = sqrt_den * sqrt_den;
-          r.cal_factor = (f != fidx.end() && pass) ? (co == 0 ? 0.0 : stat[e] * stat[e] / co) : 1.0;
-          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, r);
+          // print_sum_stats_htp for a binary trait (src/Step2_Models.cpp:2542-2646), with the genotype counts of the
+          // trait's cases and controls.  SCORE / SKATV (compute_score_bt :523-526, :546): stats * sqrt(denum) with the
+          // sign of the minor-allele flip undone, and denum = 1 / se^2 of the score test; cal_factor (check_pval_snp
+          // :1993, :2027) = 1 without a correction, stats^2 / corrected chi-square with one.  After a FAILED correction
+          // the reference prints whatever cal_factor the thread held before (it returns before the assignment): 1 here.
+          HtpRow hr;
+          hr.model = htp_model.c_str(); hr.bt = true; hr.firth = p.firth;
+          hr.beta = bo; hr.se = so; hr.chisq = co; hr.logp = lp; hr.af = r.af[e]; hr.mac = r.mac[e]; hr.test_pass = pass;
+          for (int k = 0; k < 6; ++k) hr.gc[k] = in.htp_cnt[b & 1][e * 6 + k];
+          if (in.use_bgen) hr.info = r.info[e];                // dosages: the trait's INFO
+          const double sqrt_den = 1.0 / r.se[e];
+          hr.score = r.stat[e] * sqrt_den * ((r.flags[v] & 8) ? -1.0 : 1.0); hr.skat_var = sqrt_den * sqrt_den;
+          hr.cal_factor = (f != fidx.end() && pass) ? (co == 0 ? 0.0 : r.stat[e] * r.stat[e] / co) : 1.0;
+          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, hr);
           continue;
         }
         if (p.no_split) append_sumstats_all_trait(w.obuf_all, true, bo, so, co, lp, pass);
-        else append_sumstats_row(obuf[i], head_s, af[e], use_bgen, use_bgen ? info[e] : -1.0, ns[e], test_name(p.test_type), bo, so, co, lp, pass,
-                                 (hc && p.af_cc) ? &cc : nullptr);
+        else append_sumstats_row(obuf[i], head_s, r.af[e], in.use_bgen, in.use_bgen ? r.info[e] : -1.0, r.ns[e], test_name(p.test_type),
+                                 bo, so, co, lp, pass, (hc && p.af_cc) ? &cc : nullptr);
       }
       if (p.no_split) w.obuf_all += " NA\n";
     }
     w.flush();
-    log << " block [" << b + 1 << "/" << blocks.size() << "] : done\n";
+    log << " block [" << b + 1 << "/" << in.blocks.size() << "] : done\n";
   }
   w.close();
   log << "\nNumber of ignored tests due to low MAC or low variance : " << n_ignored << "\n";

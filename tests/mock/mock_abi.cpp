@@ -32,6 +32,7 @@ struct rg_ctx {
   std::vector<uint32_t> pgen_rows;
   std::vector<uint8_t> stage[4];                               // rg_s2_stage slots (host copies)
   int last_bs = 0;
+  bool qt_chr = false, bt_chr = false;                         // rg_s2_set_chr / rg_s2_set_chr_bt has run
 };
 
 namespace {
@@ -254,6 +255,7 @@ int rg_step2_create(const rg_step2_config* cfg, const double*, const uint8_t* ma
 int rg_s2_set_chr(rg_handle h, const double* res, const double* scf) {
   h->res.assign(res, res + (size_t)h->N * h->P);
   h->scf.assign(scf, scf + h->P);
+  h->qt_chr = true;
   return 0;
 }
 int rg_s2_set_sex(rg_handle h, const uint8_t* male) {
@@ -265,38 +267,47 @@ int rg_s2_set_chr_bt(rg_handle h, const rg_s2_bt_chr* st) {
   h->res.assign(st->yres, st->yres + (size_t)h->N * h->P);
   for (size_t e = 0; e < h->res.size(); ++e) h->res[e] *= 25.0 * st->gamma_sqrt_mask[e];   // enough |z| > threshold cases
   h->scf.assign(h->P, 1.0);
+  h->bt_chr = true;
   return 0;
 }
-static int block_common(rg_handle h, int bs, const rg_s2_out* o) {
+// each route needs its own chromosome call, like the library: a driver that calls the route of the other trait kind fails
+static int block_common(rg_handle h, bool bt, int bs) {
   if (h->kind != 2 || bs < 1 || bs > h->bs_max) return fail("mock: block size out of range");
-  if (h->res.empty()) return fail("mock: rg_s2_set_chr has not been called");
+  if (!(bt ? h->bt_chr : h->qt_chr)) return fail(bt ? "mock: rg_s2_set_chr_bt has not been called" : "mock: rg_s2_set_chr has not been called");
   h->last_bs = bs;
-  (void)o;
   return 0;
 }
-int rg_s2_block_bed(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
-                    double min_mac, const rg_s2_out* o) {
-  if (block_common(h, bs, o)) return 1;
+static int block_bed(rg_handle h, bool bt, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx,
+                     int32_t ref_first, double min_mac, const rg_s2_out* o) {
+  if (block_common(h, bt, bs)) return 1;
   for (int v = 0; v < bs; ++v) score(h, v, from_bed(h, packed + (size_t)v * row_stride, sample_idx, ref_first), h->res, min_mac, o, nullptr);
   h->nonpar.clear();
   return 0;
 }
-int rg_s2_block_bed_bt(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
-                       double min_mac, const rg_s2_out* o) {
-  return rg_s2_block_bed(h, packed, row_stride, bs, sample_idx, ref_first, min_mac, o);
-}
-int rg_s2_block_bgen8(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
-                      int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
-  if (block_common(h, bs, o)) return 1;
+static int block_bgen8(rg_handle h, bool bt, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
+                       int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
+  if (block_common(h, bt, bs)) return 1;
   for (int v = 0; v < bs; ++v)
     score(h, v, from_bgen(h, probs + (size_t)v * n_file * 2, pm ? pm + (size_t)v * n_file : nullptr, sample_idx, ref_first), h->res,
           min_mac, o, info);
   h->nonpar.clear();
   return 0;
 }
+int rg_s2_block_bed(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
+                    double min_mac, const rg_s2_out* o) {
+  return block_bed(h, false, packed, row_stride, bs, sample_idx, ref_first, min_mac, o);
+}
+int rg_s2_block_bed_bt(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
+                       double min_mac, const rg_s2_out* o) {
+  return block_bed(h, true, packed, row_stride, bs, sample_idx, ref_first, min_mac, o);
+}
+int rg_s2_block_bgen8(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
+                      int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
+  return block_bgen8(h, false, probs, pm, n_file, bs, sample_idx, ref_first, min_mac, o, info);
+}
 int rg_s2_block_bgen8_bt(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
                          int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
-  return rg_s2_block_bgen8(h, probs, pm, n_file, bs, sample_idx, ref_first, min_mac, o, info);
+  return block_bgen8(h, true, probs, pm, n_file, bs, sample_idx, ref_first, min_mac, o, info);
 }
 int rg_s2_firth(rg_handle h, int32_t n, const int32_t* vi, const int32_t* ti, double* beta, double* se, double* lrt, int32_t* status) {
   for (int k = 0; k < n; ++k) {

@@ -118,3 +118,35 @@ def test_staged_input_gives_the_same_rows(tmp_path):
     finally:
         capi.check(L.rg_host_free(hp))
     st.close()
+
+
+def test_block_routes_need_their_chromosome_call_and_count_their_launches():
+    """The quantitative-trait block routes refuse to run before rg_s2_set_chr, which fills the feature rows, YtX and the
+    scale factors they read; each of the four routes adds its fixed number of kernels to rg_launch_count."""
+    from regenie_b200 import capi
+    rng = np.random.default_rng(3)
+    N, P, C, bs = 1000, 2, 3, 32
+    X = np.asfortranarray(np.linalg.qr(np.hstack([np.ones((N, 1)), rng.standard_normal((N, C - 1))]))[0])
+    g = rng.integers(0, 3, (bs, N))
+    probs = np.stack([(g == 2) * 255, (g == 1) * 255], axis=2).astype(np.uint8)
+    packed = rng.integers(0, 256, (bs, (N + 3) // 4), dtype=np.uint8)
+    st = capi.Step2(X, np.ones((N, P), dtype=np.uint8), np.ones(N, dtype=np.uint8), N, bs)
+    for call in (lambda: st.block_bed(packed), lambda: st.block_bgen8(probs)):
+        with pytest.raises(capi.RgError, match="rg_s2_set_chr has not been called"):
+            call()
+
+    def launches(call):
+        n0 = capi.lib().rg_launch_count(st.h)
+        call()
+        return capi.lib().rg_launch_count(st.h) - n0
+
+    st.set_chr(rng.standard_normal((N, P)), np.ones(P))
+    assert launches(lambda: st.block_bed(packed)) == 4
+    assert launches(lambda: st.block_bgen8(probs)) == 6
+    p = rng.uniform(0.2, 0.8, (N, P))
+    gs = np.sqrt(p * (1 - p))
+    y = (rng.random((N, P)) < p).astype(float)
+    st.set_chr_bt(gs, gs, (y - p) / gs, [X * gs[:, [j]] for j in range(P)], y)
+    assert launches(lambda: st.block_bgen8_bt(probs)) == 5
+    assert launches(lambda: st.block_bed_bt(packed)) == 7
+    st.close()
