@@ -1,5 +1,5 @@
-// Genotype-block layout kernels: PLINK 2-bit rows -> internal padded 2-bit rows -> fp8 operand
-// planes for the tensor-core Gram.  Replaces the decode half of readChunkFromBedFileToG
+// Genotype-block layout kernel: PLINK 2-bit rows -> internal padded 2-bit rows (the tensor-core Gram and prediction
+// kernels build their int8 operand bytes from these on chip).  Replaces the decode half of readChunkFromBedFileToG
 // (reference src/Geno.cpp:1702-1768, LUT src/Geno.cpp:2833-2857); mean imputation is NOT
 // materialised: missing calls stay a separate indicator plane and the mean enters as an exact
 // rank-structured correction (see DESIGN.md "missing data").
@@ -61,36 +61,6 @@ __global__ void bed_relayout_kernel(const uint8_t* __restrict__ packed, int64_t 
   gp[(int64_t)row * words_per_row + w] = out;
 }
 
-// 2-bit codes -> two int8 operand planes:
-//   dosage 0 / 1 / 2 -> 0x00 / 0x08 / 0x10  =  8 * (0, 1, 2),   missing indicator -> 0x08.
-// The INT8 Gram therefore accumulates 64 x the integer Gram - exact in int32, a power-of-two scale the epilogue removes
-// (kZScaleGram) - and the INT8 prediction kernel reads the same bytes.
-// Byte-permute does the 4-way table lookup: selector nibble k = code of sample k.
-__device__ __forceinline__ uint32_t spread_sel(uint32_t b) {
-  return (b & 0x3u) | ((b & 0xCu) << 2) | ((b & 0x30u) << 4) | ((b & 0xC0u) << 6);
-}
-
-__global__ void bed_expand_fp8_kernel(const uint32_t* __restrict__ gp, int64_t words_per_row,
-                                      int rows_p, uint8_t* __restrict__ z, int64_t npad) {
-  const int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int row = blockIdx.y;
-  if (w >= words_per_row) return;
-  const uint32_t word = __ldg(gp + (int64_t)row * words_per_row + w);
-  const uint32_t kLutG = 0x00100800u;  // idx0 -> 0, idx1 -> 0x08, idx2 -> 0x10, idx3(missing) -> 0
-  const uint32_t kLutM = 0x08000000u;  // idx3 -> 0x08
-  uint4 g, m;
-  uint32_t* gv = reinterpret_cast<uint32_t*>(&g);
-  uint32_t* mv = reinterpret_cast<uint32_t*>(&m);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const uint32_t sel = spread_sel((word >> (8 * k)) & 0xFFu);
-    gv[k] = __byte_perm(kLutG, 0, sel);
-    mv[k] = __byte_perm(kLutM, 0, sel);
-  }
-  *reinterpret_cast<uint4*>(z + (int64_t)row * npad + w * 16) = g;
-  *reinterpret_cast<uint4*>(z + (int64_t)(rows_p + row) * npad + w * 16) = m;
-}
-
 void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int rows_p,
                          const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep, int ref_first,
                          uint32_t* gp, int64_t npad,
@@ -98,12 +68,6 @@ void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int 
   const int64_t wpr = npad / 16;
   dim3 grid((unsigned)ceil_div(wpr, 256), rows_p);
   bed_relayout_kernel<<<grid, 256, 0, s>>>(packed, row_stride, bs, file_idx_pad, word_base, word_keep, ref_first, gp, wpr);
-}
-
-void launch_bed_expand_fp8(const uint32_t* gp, int rows_p, uint8_t* z, int64_t npad, cudaStream_t s) {
-  const int64_t wpr = npad / 16;
-  dim3 grid((unsigned)ceil_div(wpr, 256), rows_p);
-  bed_expand_fp8_kernel<<<grid, 256, 0, s>>>(gp, wpr, rows_p, z, npad);
 }
 
 }  // namespace rg

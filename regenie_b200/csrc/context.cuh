@@ -63,7 +63,6 @@ struct rg_ctx {
     int packed_flip = 0;
     rg::DevBuf<uint8_t> pgen_in;      // rg_pgen_decode: metadata blob + record bytes of the block this lane runs next
     rg::DevBuf<uint32_t> gp;          // [rows_p][Npad/16]
-    rg::DevBuf<uint8_t> z;            // [2 rows_p][Npad] int8
     rg::DevBuf<float> zz;             // [K][2 rows_p][2 rows_p]
     // sparse Miss rows of zz (miss_gram.cu): missing-call total of the block (> miss_cap = dense tiles), list segments
     // [K][rows_p] (offset, count), sample lists, the block as sample-major 2-bit rows [Npad][rows_p / 16]
@@ -78,13 +77,13 @@ struct rg_ctx {
     rg::DevBuf<double> cm;            // [nmat][n_aug][nC]
     rg::DevBuf<double> inv;           // [nmat][nC/64][64x64]  L_kk^-T blocks
     rg::DevBuf<double> gam, gmu, cvec, part, mean_invsd;
-    std::map<int, CUtensorMap> tmaps; // keyed by rows_p (z base differs per lane)
     rg::DevBuf<uint8_t> dig;          // radix-254 digit rows of gamma for the tensor-core prediction
     rg::DevBuf<double> wraw;          // [P][R][Npad] raw (unstandardised) predictions of the block, local to this GPU
     rg::DevBuf<double*> wraw_tab;     // [P] per-phenotype base pointers into wraw (same addressing as W_tab with col0 = 0)
     rg::DevBuf<double> dscale;        // [K][Qp] column scales
     std::map<int, CUtensorMap> dmaps; // digit-matrix tensor maps keyed by rows_p
-    std::map<int, CUtensorMap> gmaps; // 2-bit row (gp) tensor maps of the INT8 prediction, keyed by rows_p
+    std::map<int, CUtensorMap> gmaps; // 2-bit row (gp) tensor maps of the Gram, statistics and INT8 prediction tiles,
+                                      // keyed by rows_p
     // dense FP64 route for real-valued genotypes (l0_dense.cu)
     rg::DevBuf<uint8_t> dense_in;                 // staged host input (probability / ploidy bytes or FP64 rows)
     rg::DevBuf<double> gd, dpart, dpart_y;        // [bs][Npad] G~; chunk partials of G G^T and G Y

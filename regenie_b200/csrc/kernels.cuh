@@ -17,7 +17,6 @@ void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int 
                          const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep, int ref_first,
                          uint32_t* gp, int64_t npad,
                          cudaStream_t s);
-void launch_bed_expand_fp8(const uint32_t* gp, int rows_p, uint8_t* z, int64_t npad, cudaStream_t s);
 
 // ---- l0_stats.cu
 struct SnpFinalizeArgs {
@@ -60,7 +59,6 @@ void launch_l0_assemble(const AssembleArgs& a, const double* rhs, int P, int Ppa
 
 // ---- gram_wgmma.cu
 void make_gram_tensor_map(CUtensorMap* tm, const uint8_t* z, int64_t npad, int rows2);
-size_t gram_smem_bytes(int bn = 256);
 // ---- l0_stats_tc.cu: the statistics as extra Gram column tiles
 constexpr int kStatQ = 14;          // xy columns per 128-row digit group (14 x 9 limbs = 126 rows)
 constexpr int kStatOnesRow = 126;   // row of the all-ones column (group 0)
@@ -70,11 +68,18 @@ void launch_l0_stats_finish(const float* T, int ldt, int64_t t_fold_stride, cons
                             int64_t zz_fold_stride, int rows_p, int cpp, int ncol, int K, const double* scale,
                             int32_t* cnt_fold, double* sum_fold, cudaStream_t s);
 void gram_tile_list(int rows2, std::vector<int2>& tiles);
-// miss_total != null: tiles of m tile >= miss_tile0 return at once when *miss_total <= miss_cap (miss_gram.cu)
+// int8 plane rows (make_gram_tensor_map) against int8 rows: Step 2's statistics tiles
 void launch_gram_wgmma(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
-                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256,
-                         const unsigned long long* miss_total = nullptr, int64_t miss_cap = 0, int miss_tile0 = 0);
-// operand-plane bytes of the Step-1 block (bed_expand_fp8_kernel): dosage d -> 8 d as int8
+                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256);
+// Step 1: Z = [G0; Miss] of a level-0 block from its 2-bit rows (tmG: make_gp_tensor_map over rows_p rows), against
+// itself (tmD == nullptr: the Z Z^T tiles of gram_tile_list) or against int8 digit rows (tmD, bn 256 or 128).
+// miss_total != null: tiles of m tile >= miss_tile0 return at once when *miss_total <= miss_cap (miss_gram.cu)
+void launch_gram_gp(const CUtensorMap& tmG, const CUtensorMap* tmD, int rows_p, const int2* tiles, int ntiles,
+                    const int2* fold_k, int K, float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s,
+                    int bn = 256, const unsigned long long* miss_total = nullptr, int64_t miss_cap = 0,
+                    int miss_tile0 = 0);
+// operand-plane bytes of the Step-1 block (built from the 2-bit rows inside the Gram and prediction kernels): dosage d
+// -> 8 d as int8
 constexpr float kZScaleGram = 1.f / 64;   // Z Z^T tiles: both operands carry 8
 constexpr float kZScaleStat = 1.f / 8;    // Z [X|Y]-digit tiles: the digit rows are plain int8 integers
 // ---- miss_gram.cu: the Miss rows of the Z Z^T Gram from per-(SNP, fold) lists of the missing calls
@@ -87,7 +92,8 @@ void launch_miss_transpose(const uint32_t* gp, int64_t npad, int rows_p, const u
                            uint32_t* gt, cudaStream_t s);
 void launch_miss_sparse(const uint32_t* gt, int rows_p, const int2* seg, const int32_t* list, int K,
                         const unsigned long long* total, int64_t cap, float* zz, int64_t fold_stride, cudaStream_t s);
-void launch_gram_reference(const uint8_t* z, int64_t npad, int rows2, int k0, int k1, float* out, int ldo,
+// CUDA-core reference of the Z Z^T Gram of samples k0 .. k1 - 1, from the 2-bit rows (integer sums, not x 64)
+void launch_gram_reference(const uint32_t* gp, int64_t npad, int rows_p, int k0, int k1, float* out, int ldo,
                            cudaStream_t s);
 
 // ---- chol.cu

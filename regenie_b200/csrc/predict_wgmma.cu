@@ -2,9 +2,9 @@
 //
 //   pred[t, q] = sum_i gamma[i,q] g0(i,t) + sum_i (gamma mu)[i,q] miss(i,t) - x_t . cvec_q
 // (reference: `beta.transpose() * Gmat.block(...)`, src/Step1_Models.cpp:503 - 2 P R bs N flops/block).
-// The genotype operand is the plane pair [G0; Miss] the Gram kernel consumes (8 x dosage and 8 x missing as int8, the
-// bytes bed_expand_fp8_kernel writes), but the kernel builds it in registers from the block's padded 2-bit rows: one
-// 32-bit word holds both planes of 16 samples, an eighth of the bytes of the int8 planes.  The real-valued coefficients
+// The genotype operand is the plane pair [G0; Miss] of the Gram kernel (8 x dosage and 8 x missing as int8), built in
+// registers from the block's padded 2-bit rows: one 32-bit word holds both planes of 16 samples, an eighth of the bytes
+// of the int8 planes.  The real-valued coefficients
 // are split into FIVE balanced radix-254 digits
 //   gamma[i,q] = (s_q / 127) * sum_l d_l[i,q] 254^-l,   d_l in {-127..127}  (int8),
 // so the s8 x s8 -> s32 MMAs accumulate exact integer sums (|sum| <= K2 * 16 * 127 < 2^24 for K2 <= 4096) and the FP64
@@ -194,7 +194,7 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_const
   const uint8_t* gA = gen_base + PI_STAGES * PI_B_BYTES;   // generic view of the A stages
 
   // A fragment of MMA kk of stage s: {sample 2 r, 2 r + 1} x {k 4 t4 .. +3, k 16 + 4 t4 .. +3} of the stage's 32-k slice
-  // kk, as the plane bytes of bed_expand_fp8_kernel: G0 = 8 x code (0 for code 3), Miss = 8 x (code == 3).
+  // kk, as the Gram kernel's plane bytes: G0 = 8 x code (0 for code 3), Miss = 8 x (code == 3).
   auto build = [&](int s, int kk, bool miss, uint32_t (&af)[4]) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {

@@ -402,6 +402,17 @@ static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, 
   }
 }
 
+// Tensor map of the lane's 2-bit rows (the operand of the Gram, statistics and INT8 prediction tiles), made once per rows_p.
+static const CUtensorMap& gp_map(const rg_ctx* h, rg_ctx::Lane& L, int rows_p) {
+  auto it = L.gmaps.find(rows_p);
+  if (it == L.gmaps.end()) {
+    CUtensorMap tm;
+    make_gp_tensor_map(&tm, L.gp.p, h->Npad / 16, rows_p);
+    it = L.gmaps.emplace(rows_p, tm).first;
+  }
+  return it->second;
+}
+
 // Out-of-fold predictions from the coefficients x[m][p][i] at xsrc + m * xstride + (xrow0 + p) * xld + i.
 static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, const double* xsrc, int64_t xstride, int xld,
                             int xrow0, cudaStream_t s) {
@@ -448,18 +459,13 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
       make_byte_tensor_map(&tm, L.dig.p, 2 * d.rows_p, (int64_t)K * ngroups * drows_per_group);
       L.dmaps[d.rows_p] = tm;
     }
-    if (!L.gmaps.count(d.rows_p)) {
-      CUtensorMap tm;
-      make_gp_tensor_map(&tm, L.gp.p, Npad / 16, d.rows_p);
-      L.gmaps[d.rows_p] = tm;
-    }
     launch_l0_coef_i8(xsrc, xstride, xld, xrow0, R, P, d.Q, d.Qp, d.bs, d.rows_p, K, L.mu.p, L.inv_sd.p, L.Bv.p, C,
                       L.gam.p, L.gmu.p, L.cvec.p, L.dscale.p, L.dig.p, ngroups, s);
     PredictTcArgs ta;
     ta.rows_p = d.rows_p; ta.C = C; ta.P = P; ta.Q = d.Q; ta.Qp = d.Qp; ta.cpp = h->cpp; ta.col0 = 0; ta.ngroups = ngroups;
     ta.npad = Npad; ta.tile_fold = h->tile_fold.p; ta.scale = L.dscale.p; ta.cvec = L.cvec.p;
     ta.xy = h->xy.p; ta.mask = h->mask.p; ta.W = L.wraw_tab.p; ta.part = L.part.p;
-    launch_l0_predict_i8(L.gmaps[d.rows_p], L.dmaps[d.rows_p], ta, d.ntiles_s, s);
+    launch_l0_predict_i8(gp_map(h, L, d.rows_p), L.dmaps[d.rows_p], ta, d.ntiles_s, s);
     h->launches += 2;
   }
   launch_l0_standardize(L.part.p, d.ntiles_s, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, h->W_tab.p, Npad, d.col0,
@@ -567,7 +573,6 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
 
   // --- scratch
   L.gp.alloc((size_t)h->rows_p_max * (Npad / 16));
-  L.z.alloc((size_t)2 * h->rows_p_max * Npad);
   L.zz.alloc((size_t)K * 4 * h->rows_p_max * h->rows_p_max);
   L.cnt_part.alloc((size_t)h->nchunks * h->rows_p_max * 4);
   L.sum_part.alloc((size_t)h->nchunks * h->rows_p_max * 2 * h->cpp);
@@ -587,7 +592,7 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   L.part.alloc((size_t)d.ntiles_s * Qp * 2);
   L.mean_invsd.alloc((size_t)2 * Qp);
 
-  // --- 1. decode: PLINK rows -> padded 2-bit rows -> int8 planes
+  // --- 1. decode: PLINK rows -> padded 2-bit rows (the tensor-core tiles build their int8 operands from them)
   {
     ScopedTimer t(h, "bed_relayout", s);
     launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, L.gp.p, Npad, s);
@@ -597,11 +602,7 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
       L.relayout_recorded[staged] = true;
     }
   }
-  {
-    ScopedTimer t(h, "bed_expand", s);
-    launch_bed_expand_fp8(L.gp.p, rows_p, L.z.p, Npad, s);
-  }
-  h->launches += 2;
+  h->launches += 1;
 
   // --- 2. sufficient statistics: FP64 CUDA-core path (fallback) or, after the Gram, as extra tensor-core tiles
   auto snp_finalize = [&]() {
@@ -627,18 +628,13 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
 
   // --- 3. exact integer Grams on the tensor cores
   {
-    if (!L.tmaps.count(rows_p)) {
-      CUtensorMap tm;
-      make_gram_tensor_map(&tm, L.z.p, Npad, 2 * rows_p);
-      L.tmaps[rows_p] = tm;
-    }
     const rg_ctx::TileList& tl =
         cached_tiles(h->tile_lists, rows_p, [&](std::vector<int2>& tiles) { gram_tile_list(2 * rows_p, tiles); });
     const int64_t zz_stride = (int64_t)4 * rows_p * rows_p;
     ScopedTimer t(h, "gram_wgmma", s);
     if (h->gram_dense) {
-      launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], tl.buf.p, tl.count, h->fold_k.p, K,
-                        L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s);
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, tl.buf.p, tl.count, h->fold_k.p, K,
+                     L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s);
       h->launches += 1;
     } else {
       // the Miss rows: the device picks the sparse sums or the dense tiles from the block's missing-call count
@@ -648,8 +644,8 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
       L.gt.alloc((size_t)Npad * (h->rows_p_max / 16));
       launch_miss_list(L.gp.p, Npad, rows_p, h->fold_k.p, K, L.miss_total.p, h->miss_cap, L.miss_seg.p, L.miss_list.p, s);
       launch_miss_transpose(L.gp.p, Npad, rows_p, L.miss_total.p, h->miss_cap, L.gt.p, s);
-      launch_gram_wgmma(L.tmaps[rows_p], L.tmaps[rows_p], tl.buf.p, tl.count, h->fold_k.p, K,
-                        L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, tl.buf.p, tl.count, h->fold_k.p, K,
+                     L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
       launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, L.miss_list.p, K, L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
       h->launches += 5;
     }
@@ -665,8 +661,8 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     });
     L.tstat.alloc((size_t)K * 2 * h->rows_p_max * h->stat_drows);
     const int64_t tfs = (int64_t)2 * rows_p * h->stat_drows;
-    launch_gram_wgmma(L.tmaps[rows_p], h->tmD, tl.buf.p, tl.count, h->fold_k.p,
-                      K, L.tstat.p, h->stat_drows, tfs, kZScaleStat, s, stat_bn);
+    launch_gram_gp(gp_map(h, L, rows_p), &h->tmD, rows_p, tl.buf.p, tl.count, h->fold_k.p,
+                   K, L.tstat.p, h->stat_drows, tfs, kZScaleStat, s, stat_bn);
     launch_l0_stats_finish(L.tstat.p, h->stat_drows, tfs, L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, rows_p,
                            h->cpp, C + P, K, h->xy_scale.p, L.cnt_fold.p, L.sum_fold.p, s);
     snp_finalize();
@@ -818,8 +814,9 @@ static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
   rg_ctx::Lane& L = *h->lanes[h->last_lane];
   const int rp = h->last_rows_p;
   if (n == "gp") return dev_view(L.gp.p, (size_t)rp * (h->Npad / 16) * 4);
-  if (n == "z") return dev_view(L.z.p, (size_t)2 * rp * h->Npad);
   if (n == "zz") return dev_view(L.zz.p, (size_t)h->K * 4 * rp * rp * 4);
+  if (n == "tstat" && h->stats_tc) return dev_view(L.tstat.p, (size_t)h->K * 2 * rp * h->stat_drows * 4);  // [K][2 rp][drows]
+  if (n == "xyD" && h->stats_tc) return dev_view(h->xyD.p, (size_t)h->stat_drows * h->Npad);                // [drows][Npad]
   if (n == "mu") return dev_view(L.mu.p, (size_t)rp * 8);
   if (n == "inv_sd") return dev_view(L.inv_sd.p, (size_t)rp * 8);
   if (n == "Bv") return dev_view(L.Bv.p, (size_t)rp * h->C * 8);
@@ -860,14 +857,14 @@ static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
   }
   if (n == "pad_of") return host_view(h->pad_of.data(), h->N);
   if (n == "zz_ref") {
-    // the integer Grams recomputed on the CUDA cores from the int8 planes
-    RG_CHECK(L.z.p, "debug buffer not filled yet: z");
+    // the integer Grams recomputed on the CUDA cores from the 2-bit rows
+    RG_CHECK(L.gp.p, "debug buffer not filled yet: gp");
     const size_t per = (size_t)4 * rp * rp;
     DevBuf<float> ref;
     ref.alloc(per * h->K);
     RG_CUDA(cudaMemsetAsync(ref.p, 0, per * h->K * 4, h->stream));
     for (int f = 0; f < h->K; ++f)
-      launch_gram_reference(L.z.p, h->Npad, 2 * rp, (int)h->fold_pad_start[f], (int)(h->fold_pad_start[f] + h->fold_pad_len[f]),
+      launch_gram_reference(L.gp.p, h->Npad, rp, (int)h->fold_pad_start[f], (int)(h->fold_pad_start[f] + h->fold_pad_len[f]),
                             ref.p + per * f, 2 * rp, h->stream);
     std::vector<float> v(per * h->K);
     RG_CUDA(cudaMemcpyAsync(v.data(), ref.p, v.size() * 4, cudaMemcpyDeviceToHost, h->stream));

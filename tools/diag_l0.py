@@ -62,7 +62,7 @@ def main():
         for ph in range(pr.Y.shape[1]):
             W = st.fetch_W(b, ph)
             print("  W ph", ph, "rel", rel(W, W_o[ph]))
-    for k in ["h2d", "bed_relayout", "bed_expand", "l0_stats", "gram_wgmma", "l0_assemble", "chol_factor",
+    for k in ["h2d", "bed_relayout", "l0_stats", "gram_wgmma", "l0_assemble", "chol_factor",
               "chol_backsolve", "l0_predict"]:
         ms, n = st.timing(k)
         print("  time %-16s %8.3f ms over %d" % (k, ms, n))
