@@ -321,6 +321,7 @@ void read_pheno_and_cov(const SampleSet& g, const std::string& pheno_file, const
   }
   ph.in_analysis.assign(N, 0);
   for (int64_t s = 0; s < N; ++s) ph.in_analysis[s] = in_ph[s] && in_cov[s];
+  ph.in_cov = in_cov;
 }
 
 // cyclic Jacobi eigen-decomposition of a small symmetric matrix (a: n x n row-major, destroyed);

@@ -66,6 +66,7 @@ struct Pheno {
   std::vector<uint8_t> mask;      // N x P column-major
   std::vector<double> X;          // N x C column-major, orthonormal basis
   std::vector<uint8_t> in_analysis;
+  std::vector<uint8_t> in_cov;    // samples with complete covariates (ind_in_cov_and_geno, src/Pheno.cpp:53)
   std::vector<double> neff, scale_Y;
   int64_t n_analyzed = 0;
   bool strict = false;

@@ -21,6 +21,7 @@
 
 #include "bgen.hpp"
 #include "bt_null.hpp"
+#include "condition.hpp"
 #include "data.hpp"
 #include "output.hpp"
 #include "pgen.hpp"
@@ -72,6 +73,8 @@ struct Params {
   int gpus = 1;                                // --gpus N (step 1): level-0 blocks sharded over N GPUs of this node, level 1 by phenotype
   bool gpu_inflate = false;                    // --gpu-inflate: zlib payloads of the .bgen are inflated on the device (rg_bgen_inflate)
   uint32_t par1_max = 2781479, par2_min = 155701383;   // hg38 (check_build_code, src/Regenie.cpp:1643-1660)
+  std::string cond_list, cond_fmt, cond_file, cond_sample;   // --condition-list / --condition-file FORMAT,FILE / --condition-file-sample
+  uint32_t max_cond = 10000;                   // --max-condition-vars
 };
 
 void rg_check(int rc) {
@@ -247,6 +250,20 @@ Params parse_cli(int argc, char** argv) {
       p.range_max = std::max(p0, p1);
       p.set_range = true;
     }
+    else if (a == "--condition-list") p.cond_list = need(i);
+    else if (a == "--condition-file") {                         // src/Regenie.cpp:714-723
+      const std::string v = need(i);
+      std::vector<std::string> t;                               // string_split: a trailing empty field is dropped
+      size_t at = 0;
+      for (size_t k; (k = v.find(',', at)) != std::string::npos; at = k + 1) t.push_back(v.substr(at, k - at));
+      if (at < v.size()) t.push_back(v.substr(at));
+      if (t.size() < 2) throw Fail("invalid option input for --condition-file");
+      if (t[0] != "bgen" && t[0] != "bed" && t[0] != "pgen") throw Fail("invalid file format for --condition-file (either bed/bge/pgen)");
+      p.cond_fmt = t[0];
+      p.cond_file = t[1];
+    }
+    else if (a == "--condition-file-sample") p.cond_sample = need(i);
+    else if (a == "--max-condition-vars") p.max_cond = (uint32_t)strtoul(need(i).c_str(), nullptr, 10);
     else if (a == "--bt") p.bt = true;
     else if (a == "--force-step1") p.force_step1 = true;
     else if (a == "--use-relative-path") p.rel_path = true;
@@ -261,7 +278,9 @@ Params parse_cli(int argc, char** argv) {
                    "  [--gz] [--print-prs | --use-prs] [--write-samples [--print-pheno]]  (.gz inputs are read by file name)\n"
                    "  [--test additive|dominant|recessive] [--no-split] [--af-cc] [--minCaseCount n] [--write-null-firth | --use-null-firth F]\n"
                    "  [--gpus N]  step 1: shard the level-0 blocks over N GPUs of this node (level 1 by phenotype), same output files\n"
-                   "  [--gpu-inflate]  step 2 on zlib-compressed .bgen: inflate the genotype blocks on the GPU instead of the host\n";
+                   "  [--gpu-inflate]  step 2 on zlib-compressed .bgen: inflate the genotype blocks on the GPU instead of the host\n"
+                   "  [--condition-list F [--condition-file bed|pgen|bgen,FILE [--condition-file-sample F]] [--max-condition-vars n]]\n"
+                   "      conditional analysis (steps 1 and 2): the listed variants become covariates and are not tested\n";
       exit(0);
     } else {
       throw Fail("option '" + a + "' is outside the hot path covered by rgb200 (see DESIGN.md, out of scope)");
@@ -284,6 +303,7 @@ Params parse_cli(int argc, char** argv) {
   if (p.write_samples && !p.bgen.empty() && p.sample.empty())                     // src/Regenie.cpp:903-904
     throw Fail("must specify sample file (using --sample) if writing sample IDs to file.");
   if (p.step == 2 && p.pred.empty() && !p.ignore_pred) throw Fail("must specify --pred if using --step 2 (otherwise use --ignore-pred).");
+  if (!p.cond_fmt.empty() && p.cond_list.empty()) throw Fail("must use --condition-list if using --condition-file.");   // src/Regenie.cpp:1159-1160
   if (p.htp) {
     if (p.step != 2) throw Fail("option --htp only works in step 2.");
     if (p.no_split) p.no_split = false;                       // src/Regenie.cpp:1068-1071: --no-split is ignored with --htp
@@ -355,6 +375,27 @@ void open_rows(const Params& p, BedFile& g, const std::set<std::string>& excl, c
   }
 }
 
+// --condition-list [--condition-file]: reads the list (get_conditional_vars, src/Geno.cpp:4151-4179, which runs before the
+// genotype file is set up); the IDs join the exclusion set `excl` of the main reader, on top of --exclude / --extract
+void init_conditioning(const Params& p, Conditioning& c, std::set<std::string>& excl, Log& log) {
+  if (p.cond_list.empty()) return;
+  c.list_file = p.cond_list;
+  c.fmt = p.cond_fmt; c.file = p.cond_file; c.sample_file = p.cond_sample;
+  c.max_vars = p.max_cond;
+  c.ref_first = p.ref_first;
+  c.read_list();
+  excl.insert(c.ids.begin(), c.ids.end());
+  if (!p.extract.empty()) log << "WARNING: only variants which satisfy both extract/exclude options will be kept.\n";   // src/Regenie.cpp:1081-1082
+}
+
+// same-file conditioning: the listed IDs among the variants of the main genotype file after --chr / --range
+void locate_conditioning(const Params& p, Conditioning& c) {
+  if (!c.on() || c.external()) return;
+  const std::string fmt = !p.bgen.empty() ? "bgen" : !p.pgen.empty() ? "pgen" : "bed";
+  c.locate_in_main(fmt, !p.bgen.empty() ? p.bgen : !p.pgen.empty() ? p.pgen : p.bed, p.sample, p.bgi, p.chrs, p.set_range,
+                   p.range_chr, p.range_min, p.range_max);
+}
+
 // ---- --split-l0 / --run-l0 / --run-l1 (src/Data.cpp:232-309, 818-908): level 0 as independent jobs that exchange
 // the N x R slabs of write_l0_file through <prefix>_job<j>_l0_Y<k>; files are interchangeable with the reference's.
 struct MasterJob { std::string prefix; int nblocks; long nsnps; };
@@ -421,14 +462,18 @@ void run_step1(const Params& p_in, Log& log) {
   const bool use_bgen = !p.bgen.empty();
   BedFile gbed;
   BgenFile gg;
+  Conditioning cond;
+  std::set<std::string> excl = read_id_list(p.exclude, 1);
+  init_conditioning(p, cond, excl, log);
   if (use_bgen) {
-    gg.open(p.bgen, p.sample, p.ref_first, read_id_list(p.exclude, 1), read_id_list(p.extract, 1), read_id_list(p.remove, 2),
+    gg.open(p.bgen, p.sample, p.ref_first, excl, read_id_list(p.extract, 1), read_id_list(p.remove, 2),
             read_id_list(p.keep, 2), p.chrs, p.bgi);
     if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
     log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
   } else {
-    open_rows(p, gbed, read_id_list(p.exclude, 1), read_id_list(p.extract, 1), read_id_list(p.remove, 2), read_id_list(p.keep, 2), log);
+    open_rows(p, gbed, excl, read_id_list(p.extract, 1), read_id_list(p.remove, 2), read_id_list(p.keep, 2), log);
   }
+  locate_conditioning(p, cond);
   // the fields of either reader the rest of Step 1 needs
   struct GenoView {
     const std::vector<Snp>& snps;
@@ -447,6 +492,7 @@ void run_step1(const Params& p_in, Log& log) {
   ph.pheno_cols = p.pheno_cols; ph.covar_cols = p.covar_cols; ph.rint = p.rint && !p.bt; ph.cat_cols = p.cat_cols; ph.max_cat_levels = p.max_cat_levels;
   ph.pheno_excl = p.pheno_excl; ph.covar_excl = p.covar_excl; ph.min_case_count = p.min_case_count;
   read_pheno_and_cov(SampleSet{g.keys, g.key_to_ind}, p.pheno, p.covar, false, p.strict, p.bt, ph, log);
+  if (cond.on()) cond.append(SampleSet{g.keys, g.key_to_ind}, ph, log);
   prep_run(ph, nullptr, log);
   if (p.bt && !p.loocv) {
     if (ph.n_analyzed < 5000) {                       // src/Data.cpp:353-356
@@ -1090,10 +1136,11 @@ void apply_range(const Params& p, std::vector<Snp>& snps) {
 
 // phenotypes + covariates + LOCO files for Step 2 (read_pheno_and_cov, blup_read, prep_run)
 void load_step2_inputs(const Params& p, const SampleSet& g, const std::vector<std::pair<std::string, std::string>>& ids_file,
-                       const std::vector<int32_t>& sample_idx, Pheno& ph, std::vector<Loco>& locos, Log& log) {
+                       const std::vector<int32_t>& sample_idx, Conditioning& cond, Pheno& ph, std::vector<Loco>& locos, Log& log) {
   ph.pheno_cols = p.pheno_cols; ph.covar_cols = p.covar_cols; ph.rint = p.rint && !p.bt; ph.cat_cols = p.cat_cols; ph.max_cat_levels = p.max_cat_levels;
   ph.pheno_excl = p.pheno_excl; ph.covar_excl = p.covar_excl; ph.min_case_count = p.min_case_count;
   read_pheno_and_cov(g, p.pheno, p.covar, true, p.strict, p.bt, ph, log);
+  if (cond.on()) cond.append(g, ph, log);
   const int64_t N = ph.N;
   const int P = ph.P;
   // write_ids (src/Pheno.cpp:1538-1576) runs right after blup_read, before setMasks: the samples with a phenotype
@@ -1194,6 +1241,7 @@ struct S2Input {
   const SampleSet ss;
   size_t n_file = 0;
   bool subset = false;                                       // the file holds samples that are not analysed
+  Conditioning cond;                                         // --condition-list
   Pheno ph;
   std::vector<Loco> locos;
   std::vector<Block> blocks;
@@ -1214,8 +1262,9 @@ struct S2Input {
       : p(p_), binary(binary_), use_bgen(!p_.bgen.empty()), snps(use_bgen ? gg.snps : g.snps),
         sample_idx(use_bgen ? gg.sample_idx : g.sample_idx),
         ss{use_bgen ? gg.keys : g.keys, use_bgen ? gg.key_to_ind : g.key_to_ind} {
-    const auto excl = read_id_list(p.exclude, 1), extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2),
-               keep = read_id_list(p.keep, 2);
+    const auto extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2), keep = read_id_list(p.keep, 2);
+    std::set<std::string> excl = read_id_list(p.exclude, 1);
+    init_conditioning(p, cond, excl, log);
     if (use_bgen) {
       gg.sex_specific = p.sex_specific;
       gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keep, p.chrs, p.bgi);
@@ -1228,9 +1277,10 @@ struct S2Input {
     apply_range(p, g.snps);
     if (g.pg) apply_range(p, g.pg->snps);
     if (p.set_range && snps.empty()) throw Fail("no variant left to include in analysis.");
+    locate_conditioning(p, cond);
     n_file = use_bgen ? gg.n_file : g.keys_file.size();
     subset = ss.keys.size() != n_file;
-    load_step2_inputs(p, ss, use_bgen ? gg.ids_file : g.ids_file, sample_idx, ph, locos, log);
+    load_step2_inputs(p, ss, use_bgen ? gg.ids_file : g.ids_file, sample_idx, cond, ph, locos, log);
     blocks = set_blocks(snps, p.bsize);
     log << " * # blocks            : [" << blocks.size() << "]\n";
     male = male_vector(use_bgen ? gg.sex_file : g.sex_file, sample_idx);
