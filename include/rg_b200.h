@@ -344,6 +344,49 @@ int rg_s2_block_bed_bt(rg_handle h, const uint8_t* packed, int64_t row_stride, i
 int rg_s2_firth(rg_handle h, int32_t n_sel, const int32_t* variant_idx, const int32_t* trait_idx, double* beta,
                 double* se, double* lrt, int32_t* status);
 
+/* ------------------------------------------------------------------ Step 2 (QT): GxE interaction tests */
+/*
+ * Per-chromosome state of the interaction tests with a quantitative variable E (--interaction VAR, E kept as a
+ * covariate: regenie's default gwas_condtl).  Takes effect for the blocks run after it on a handle that has had
+ * rg_s2_set_chr; the robust route reads the residuals and the covariate basis of rg_s2_set_chr.
+ *   E          [N]        pheno_data.interaction_cov (raw values, 0 outside the analysis)
+ *   n_px       K          columns of the HLM projection Px (0 = no HLM state: every variant takes the robust route)
+ *   dinv_sqrt  [P][N]     HLM Dinv_sqrt = exp(-V beta / 2) o mask                         (src/HLM.cpp:224)
+ *   px         [P][K][N]  orthonormal basis of Dinv_sqrt o X_hlm                         (src/HLM.cpp:225-229)
+ *   yres       [P][N]     Dinv_sqrt o y - Px Px^T (Dinv_sqrt o y)                        (src/HLM.cpp:232, :236-243)
+ */
+typedef struct rg_s2_int_chr {
+  const double* E;
+  int32_t n_px;
+  const double* dinv_sqrt;
+  const double* px;
+  const double* yres;
+} rg_s2_int_chr;
+int rg_s2_set_interaction(rg_handle h, const rg_s2_int_chr* st);
+
+/* options of rg_s2_interaction (src/Regenie.cpp: --rare-mac, --force-robust, --force-hc4, --no-robust, --minMAC) */
+typedef struct rg_s2_int_opts {
+  double rare_mac;       /* params.rareMAC_inter (default 1000)                                   */
+  double min_mac;        /* params.min_MAC: a trait with MAC below it is ignored (no rows)         */
+  int32_t force_robust;  /* params.force_robust                                                   */
+  int32_t force_hc4;     /* params.force_hc4 (HC4 for traits with MAC <= rare_mac)                */
+  int32_t no_robust;     /* params.no_robust (model-based SE)                                     */
+} rg_s2_int_opts;
+
+/*
+ * rg_s2_interaction -- the interaction model of every (variant, trait) pair of the block left resident by the last
+ * rg_s2_block_bed / rg_s2_block_bgen8 call (get_interaction_terms + apply_interaction_tests_qt / _HLM,
+ * src/Interaction.cpp:44-92, :109-437).  That call must be the last block call on the handle and must have run after
+ * rg_s2_set_interaction on the current chromosome (rg_s2_block_bed writes the per-sample genotype words this call reads
+ * only then); otherwise the call fails.  Per variant the route is HLM when any trait has MAC < rare_mac and the HLM
+ * state is set (unless force_robust or no_robust), the robust sandwich otherwise.  Outputs are host arrays, variant-major:
+ *   status [bs][P]     0 = no interaction rows (variant or trait ignored, or resid(E o G) has sd < numtol),
+ *                      1 = robust route, 2 = HLM route, -1 = H^T H (robust) or Xres^T Xres (HLM) is near-singular
+ *   coef   [bs][P][2]  (beta_G, beta_GxE), on the phenotype scale of the printed rows
+ *   vcov   [bs][P][4]  their 2 x 2 covariance (row-major), on the same scale
+ */
+int rg_s2_interaction(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, double* coef, double* vcov);
+
 /* ------------------------------------------------------------------ PGEN records (SURVEY 8 (f)3) */
 /*
  * rg_pgen_decode -- the variant records of one block of a PLINK 2 .pgen (hard calls), decoded ON THE DEVICE into

@@ -77,7 +77,7 @@ EXPORTS = [
     "rg_last_error", "rg_version", "rg_device_count", "rg_step1_create", "rg_destroy", "rg_sync",
     "rg_l0_block_bed", "rg_l0_status", "rg_l0_fetch_W", "rg_l1_fit", "rg_loco", "rg_step2_create",
     "rg_s2_set_chr", "rg_s2_block_bed", "rg_W_info", "rg_debug_fetch", "rg_launch_count", "rg_stream",
-    "rg_set_timing", "rg_get_timing", "rg_fence", "rg_s2_set_chr_bt", "rg_s2_block_bgen8_bt", "rg_s2_block_bgen8", "rg_s2_firth", "rg_l1_fit_bt", "rg_W_set_owned", "rg_W_export", "rg_W_attach_peer", "rg_l1_select", "rg_s2_set_sex", "rg_s2_set_non_par", "rg_l0_load_W", "rg_s2_spa", "rg_s2_block_bed_bt", "rg_prs", "rg_bgen_inflate",
+    "rg_set_timing", "rg_get_timing", "rg_fence", "rg_s2_set_chr_bt", "rg_s2_block_bgen8_bt", "rg_s2_block_bgen8", "rg_s2_firth", "rg_l1_fit_bt", "rg_W_set_owned", "rg_W_export", "rg_W_attach_peer", "rg_l1_select", "rg_s2_set_sex", "rg_s2_set_non_par", "rg_l0_load_W", "rg_s2_spa", "rg_s2_block_bed_bt", "rg_prs", "rg_bgen_inflate", "rg_s2_set_interaction", "rg_s2_interaction",
     "rg_l0_solver_stats", "rg_dbg_mixed_solve", "rg_l0_wait_input", "rg_l0_block_dosage_u8", "rg_l0_block_f64", "rg_W_attach_local",
     "rg_s2_stage", "rg_host_alloc", "rg_host_free", "rg_pgen_decode", "rg_warmup", "rg_l0_poll_status",
 ]
@@ -299,6 +299,15 @@ class Step1:
         return ms.value, n.value
 
 
+class S2IntChr(C.Structure):
+    _fields_ = [("E", C.c_void_p), ("n_px", C.c_int32), ("dinv_sqrt", C.c_void_p), ("px", C.c_void_p), ("yres", C.c_void_p)]
+
+
+class S2IntOpts(C.Structure):
+    _fields_ = [("rare_mac", C.c_double), ("min_mac", C.c_double), ("force_robust", C.c_int32),
+                ("force_hc4", C.c_int32), ("no_robust", C.c_int32)]
+
+
 class Step2:
     """Host-side mirror of the Step-2 QT call sequence of Data::test_snps_fast (src/Data.cpp:2230-2383)."""
 
@@ -471,6 +480,30 @@ class Step2:
         pv, status = np.empty(len(vi)), np.empty(len(vi), dtype=np.int32)
         check(L.rg_s2_spa(self.h, len(vi), _ptr(vi), _ptr(ti), _ptr(pv), _ptr(status)))
         return pv, status
+
+    # ---- GxE interaction tests (quantitative traits)
+    def set_interaction(self, E, dinv_sqrt=None, px=None, yres=None):
+        """rg_s2_set_interaction after set_chr.  E [N]; HLM state (or None): dinv_sqrt, yres [N x P], px list of P [N x K]."""
+        L = lib()
+        L.rg_s2_set_interaction.argtypes = [C.c_void_p, C.c_void_p]
+        E = np.ascontiguousarray(E, dtype=np.float64)
+        K = 0 if px is None else px[0].shape[1]
+        keep = [E]
+        if K:
+            keep += [_f64(dinv_sqrt), np.ascontiguousarray(np.stack([_f64(x) for x in px]).transpose(0, 2, 1)), _f64(yres)]
+        st = S2IntChr(E.ctypes.data, K, *[keep[k].ctypes.data if K else None for k in (1, 2, 3)])
+        check(L.rg_s2_set_interaction(self.h, C.byref(st)))
+
+    def interaction(self, bs, rare_mac=1000.0, min_mac=5.0, force_robust=False, force_hc4=False, no_robust=False):
+        """rg_s2_interaction on the resident block: (status [bs, P], coef [bs, P, 2], vcov [bs, P, 2, 2])."""
+        L = lib()
+        L.rg_s2_interaction.argtypes = [C.c_void_p] * 5
+        P = self.P
+        status = np.empty((bs, P), dtype=np.int32)
+        coef, vcov = np.empty((bs, P, 2)), np.empty((bs, P, 2, 2))
+        o = S2IntOpts(float(rare_mac), float(min_mac), int(force_robust), int(force_hc4), int(no_robust))
+        check(L.rg_s2_interaction(self.h, C.byref(o), _ptr(status), _ptr(coef), _ptr(vcov)))
+        return status, coef, vcov
 
     def debug(self, name, dtype, count):
         """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block."""

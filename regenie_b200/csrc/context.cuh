@@ -193,6 +193,14 @@ struct rg_ctx {
   rg::DevBuf<uint8_t> pgen_in, pgen_rows;             // rg_pgen_decode on a Step-2 handle: records in, 2-bit rows out
   rg::DevBuf<unsigned long long> pgen_err;            // first malformed record: (block + 1) << 32 | variant << 4 | code
   rg::DevBuf<uint32_t> dz;           // [rows_p][Npad] d | e << 10 | missing << 31
+  // GxE interaction tests (rg_s2_set_interaction / rg_s2_interaction, csrc/s2_interaction.cu)
+  bool int_set = false;
+  bool s2_dz_qt = false;             // dz holds the words of the resident quantitative-trait block of this chromosome
+  rg::DevBuf<int8_t> int_route;
+  int int_K = 0, int_nr = 0, int_nf = 0;
+  rg::DevBuf<double> int_F, int_E, int_part, int_sums, int_var, int_meat, int_out;
+  rg::DevBuf<uint8_t> int_pow2;
+  rg::DevBuf<int32_t> int_status;
   rg::DevBuf<double> bt_F, bt_w, bt_gs, bt_xw, bt_off, bt_coltot, bt_xwy, bt_part, bt_sums, bt_nnz, bt_n510;
   rg::DevBuf<double> bt_xtwg, bt_mu, bt_info, firth_gvec, firth_out, bt_den, bt_phat;
   rg::DevBuf<int8_t> bt_ym, firth_cflag;

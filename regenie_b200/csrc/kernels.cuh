@@ -362,4 +362,27 @@ struct SpaArgs {
 };
 void launch_s2_spa(const SpaArgs& a, cudaStream_t s);
 
+// ---- s2_interaction.cu
+struct S2IntArgs {
+  int bs, C, P, dp, K, nf, nr, nchunks, var_stride;
+  int force_robust, force_hc4, no_robust;
+  long long n_analyzed, n_samples;
+  double rare_mac, min_mac, numtol;
+  int64_t npad;
+  const uint32_t* dz;                // [rows_p][Npad] genotype words of the resident block
+  const double* Fint;                // [Npad][nf] interaction features (robust nr columns, then HLM P x (2K + 5))
+  const double* F;                   // [Npad][dp] the QT feature rows of rg_s2_set_chr (X, res, mask)
+  const double* E;                   // [Npad]
+  const int4* chunks;
+  const double *af_all, *mac, *YtX, *scf_sv, *mask_count;
+  const int32_t* flags;
+  double* sums;                      // [bs][nf]
+  double* var;                       // [bs][var_stride] per-variant robust state
+  double* meat_part;                 // [bs][P][nchunks][4]
+  int32_t* status;                   // [bs][P]
+  double *coef, *vcov;               // [bs][P][2], [bs][P][4]
+  int8_t* route;                     // [bs] 0 none, 1 robust, 2 HLM (written by the first kernel)
+};
+void launch_s2_interaction(const S2IntArgs& a, const uint8_t* pow2, double* part, cudaStream_t s);
+
 }  // namespace rg

@@ -158,6 +158,8 @@ static void s2_set_chr(rg_ctx* h, const double* res, const double* scf_sv) {
   s2_build_digits(h, h->F.p, dp, base + (with_sex ? 1 + P : 0));
   RG_CUDA(cudaStreamSynchronize(h->stream));
   h->s2_chr_set = true;
+  h->int_set = false;                                                // rg_s2_set_interaction follows, per chromosome
+  h->s2_dz_qt = false;
 }
 
 // per-variant non-PAR flags set by rg_s2_set_non_par apply to exactly one block call
@@ -231,6 +233,7 @@ static void s2_block_begin(rg_ctx* h, bool bt, int bs, const int32_t* sample_idx
   RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
   if (bt) RG_CHECK(h->bt_chr_set, "rg_s2_set_chr_bt has not been called");
   else RG_CHECK(h->s2_chr_set, "rg_s2_set_chr has not been called");
+  h->s2_dz_qt = false;                                               // set again by a QT route that writes dz
   RG_CUDA(cudaSetDevice(h->device));
   s2_wait_stage(h, in, h->stream);
   s2_wait_stage(h, in2, h->stream);
@@ -296,6 +299,13 @@ static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   a.male_tot = h->s2_male_tot.p;
   launch_s2_finalize(a, s);
   h->launches += 4;
+  if (h->int_set) {                                                  // what rg_s2_interaction reads
+    h->dz.alloc((size_t)h->rows_p_max * Npad);
+    launch_gp_to_dz(h->gp.p, rows_p, h->dz.p, Npad, s);
+    h->launches += 1;
+    h->s2_dz_qt = true;
+  }
+  h->s2_last_bs = bs;
   h->s2_sums_rows = rows_p;
   s2_copy_out(h, bs, out, nullptr, nullptr, s);
 }
@@ -419,6 +429,8 @@ static void s2_block_bgen8_qt(rg_ctx* h, const uint8_t* probs, const uint8_t* mi
   a.male_tot = h->s2_male_tot.p; a.nz_count = h->bt_nnz.p; a.info_sums = h->bt_xtwg.p; a.info = h->bt_info.p;
   launch_s2_finalize(a, s);
   h->launches += 6;
+  h->s2_last_bs = bs;
+  h->s2_dz_qt = true;
   h->s2_sums_rows = rows_p;
   h->bt_sums_rows = rows_p; h->bt_sums_dp = dp;
   s2_copy_out(h, bs, out, info_out, a.info, s);
@@ -515,7 +527,115 @@ static void s2_spa(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* 
   });
 }
 
+// ---------------------------------------------------------------- GxE interaction tests (quantitative traits)
+// Feature rows [Npad][nf] of s2_int_sums_kernel: robust columns X_c, E X_c, res_p, E res_p (times g), 1, E, E^2 (times
+// g^2); then per trait d Px_k, d E Px_k, d yres, d E yres (times g), d^2, d^2 E, d^2 E^2 (times g^2).  Built on the host
+// from the state of rg_s2_set_chr (X, res, in_analysis) and the HLM state, like the feature rows of s2_set_chr.
+static void s2_set_interaction(rg_ctx* h, const rg_s2_int_chr* st) {
+  RG_CHECK(h->kind == 2 && h->s2_chr_set, "rg_s2_set_interaction needs a Step-2 handle after rg_s2_set_chr");
+  RG_CHECK(st->n_px >= 0 && (st->n_px == 0 || (st->dinv_sqrt && st->px && st->yres)), "HLM state incomplete");
+  RG_CUDA(cudaSetDevice(h->device));
+  const int64_t N = h->N, Npad = h->Npad;
+  const int C = h->C, P = h->P, K = st->n_px, dp = h->dp;
+  const int nr = 2 * C + 2 * P + 3, nh = K > 0 ? P * (2 * K + 5) : 0, nf = nr + nh;
+  std::vector<double> E(Npad, 0.0);
+  std::vector<uint8_t> pow2(nf, 0);
+  for (int k = 0; k < 3; ++k) pow2[2 * C + 2 * P + k] = 1;
+  for (int p = 0; p < P && K > 0; ++p)
+    for (int k = 0; k < 3; ++k) pow2[nr + p * (2 * K + 5) + 2 * K + 2 + k] = 1;
+  for (int64_t s = 0; s < N; ++s) E[s] = h->in_analysis[s] ? st->E[s] : 0.0;
+  h->int_F.alloc((size_t)Npad * nf); h->int_E.alloc(Npad); h->int_pow2.alloc(nf);
+  RG_CUDA(cudaMemcpyAsync(h->int_E.p, E.data(), Npad * 8, cudaMemcpyHostToDevice, h->stream));
+  RG_CUDA(cudaMemcpyAsync(h->int_pow2.p, pow2.data(), nf, cudaMemcpyHostToDevice, h->stream));
+  // the rows go up in slabs of kSlab samples, so the host holds one slab of them (and of F) at a time
+  constexpr int64_t kSlab = 16384;
+  std::vector<double> Fh((size_t)kSlab * dp), F((size_t)kSlab * nf);
+  for (int64_t s0 = 0; s0 < Npad; s0 += kSlab) {
+    const int64_t ns = std::min(kSlab, Npad - s0);
+    RG_CUDA(cudaMemcpyAsync(Fh.data(), h->F.p + (size_t)s0 * dp, (size_t)ns * dp * 8, cudaMemcpyDeviceToHost, h->stream));
+    RG_CUDA(cudaStreamSynchronize(h->stream));                       // also: the previous slab's upload has finished
+    std::fill(F.begin(), F.end(), 0.0);
+    for (int64_t s = s0; s < std::min(s0 + ns, N); ++s) {
+      if (!h->in_analysis[s]) continue;
+      const double e = E[s];
+      const double* fr = &Fh[(size_t)(s - s0) * dp];
+      double* r = &F[(size_t)(s - s0) * nf];
+      for (int c = 0; c < C; ++c) { r[c] = fr[1 + c]; r[C + c] = e * fr[1 + c]; }
+      for (int p = 0; p < P; ++p) { r[2 * C + p] = fr[1 + C + p]; r[2 * C + P + p] = e * fr[1 + C + p]; }
+      r[2 * C + 2 * P] = 1.0; r[2 * C + 2 * P + 1] = e; r[2 * C + 2 * P + 2] = e * e;
+      for (int p = 0; p < P && K > 0; ++p) {
+        double* t = r + nr + p * (2 * K + 5);
+        const double d = st->dinv_sqrt[(size_t)p * N + s], y = st->yres[(size_t)p * N + s];
+        for (int k = 0; k < K; ++k) {
+          const double x = d * st->px[((size_t)p * K + k) * N + s];
+          t[k] = x; t[K + k] = e * x;
+        }
+        t[2 * K] = d * y; t[2 * K + 1] = d * e * y;
+        t[2 * K + 2] = d * d; t[2 * K + 3] = d * d * e; t[2 * K + 4] = d * d * e * e;
+      }
+    }
+    RG_CUDA(cudaMemcpyAsync(h->int_F.p + (size_t)s0 * nf, F.data(), (size_t)ns * nf * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  RG_CUDA(cudaStreamSynchronize(h->stream));
+  h->int_K = K; h->int_nr = nr; h->int_nf = nf;
+  h->int_set = true;
+}
+
+static void s2_interaction(rg_ctx* h, const rg_s2_int_opts* o, int32_t* status, double* coef, double* vcov) {
+  RG_CHECK(h->kind == 2 && h->int_set, "rg_s2_interaction needs rg_s2_set_interaction");
+  // the genotype words of the last block: written by rg_s2_block_bgen8, and by rg_s2_block_bed only when the interaction
+  // state was set before the block ran; any other block call or rg_s2_set_chr since then leaves none for this chromosome
+  RG_CHECK(h->s2_dz_qt && h->s2_last_bs > 0,
+           "rg_s2_interaction needs the block of the last rg_s2_block_bed / rg_s2_block_bgen8 call, run after "
+           "rg_s2_set_interaction on the current chromosome");
+  RG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  const int bs = h->s2_last_bs, P = h->P, C = h->C, nf = h->int_nf;
+  const int bs_pad = (int)round_up(bs, 16);
+  const rg_s2_out d = s2_out_at(h, h->s2_out_d.p, h->s2_out_i.p);
+  S2IntArgs a;
+  a.bs = bs; a.C = C; a.P = P; a.dp = h->dp; a.K = h->int_K; a.nf = nf; a.nr = h->int_nr; a.nchunks = h->nchunks;
+  a.var_stride = 8 + 2 * C + 2 * P;
+  a.force_robust = o->force_robust; a.force_hc4 = o->force_hc4; a.no_robust = o->no_robust;
+  a.n_analyzed = h->n_analyzed; a.n_samples = h->N;
+  a.rare_mac = o->rare_mac; a.min_mac = o->min_mac; a.numtol = 1e-6;
+  a.npad = h->Npad; a.dz = h->dz.p; a.Fint = h->int_F.p; a.F = h->F.p; a.E = h->int_E.p; a.chunks = h->chunks.p;
+  a.af_all = d.af_all; a.mac = d.mac; a.YtX = h->s2_YtX.p; a.scf_sv = h->s2_scf.p; a.mask_count = h->s2_maskcount.p;
+  a.flags = d.flags;
+  h->int_part.alloc((size_t)h->nchunks * bs_pad * nf);
+  h->int_sums.alloc((size_t)bs * nf);
+  h->int_var.alloc((size_t)bs * a.var_stride);
+  h->int_meat.alloc((size_t)bs * P * h->nchunks * 4);
+  h->int_out.alloc((size_t)bs * P * 6);
+  h->int_status.alloc((size_t)bs * P);
+  h->int_route.alloc(bs);
+  a.route = h->int_route.p;
+  a.sums = h->int_sums.p; a.var = h->int_var.p; a.meat_part = h->int_meat.p; a.status = h->int_status.p;
+  a.coef = h->int_out.p; a.vcov = h->int_out.p + (size_t)bs * P * 2;
+  launch_s2_interaction(a, h->int_pow2.p, h->int_part.p, s);
+  h->launches += 5;
+  RG_CUDA(cudaMemcpyAsync(status, a.status, (size_t)bs * P * 4, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaMemcpyAsync(coef, a.coef, (size_t)bs * P * 2 * 8, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaMemcpyAsync(vcov, a.vcov, (size_t)bs * P * 4 * 8, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaStreamSynchronize(s));
+}
+
 extern "C" {
+
+int rg_s2_set_interaction(rg_handle h, const rg_s2_int_chr* st) {
+  RG_API_BEGIN
+  RG_CHECK(h && st && st->E, "null argument");
+  s2_set_interaction(h, st);
+  RG_API_END
+}
+
+int rg_s2_interaction(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, double* coef, double* vcov) {
+  RG_API_BEGIN
+  RG_CHECK(h && opts && status && coef && vcov, "null argument");
+  s2_interaction(h, opts, status, coef, vcov);
+  RG_CUDA(cudaGetLastError());
+  RG_API_END
+}
 
 int rg_s2_spa(rg_handle h, int32_t n_sel, const int32_t* variant_idx, const int32_t* trait_idx, double* pval,
               int32_t* status) {
