@@ -344,7 +344,7 @@ static void require_device() {
   if (g_ndev.valid() && g_ndev.get() < 1) throw Fail("no CUDA device available: rgb200 has no CPU fallback");
 }
 
-// ------------------------------------------------------------------------------------ step 1
+// ------------------------------------------------------------------------------------ genotype input
 // .pgen input: the records of a block go to the GPU as they are and are expanded there (rg_pgen_decode, SURVEY 8 (f)3).
 // RG_B200_PGEN=host selects the host decoder (host/pgen.cpp), which also serves the options that edit rows on the host
 // (--no-split genotype counts, --test dominant / recessive, --af-cc).
@@ -359,43 +359,106 @@ static void pgen_rows_device(rg_handle h, const PgenBatch& pb, int bs, int64_t n
   rg_check(rg_pgen_decode(h, &blk, rows, stride));
 }
 
-// .bed/.bim/.fam or .pgen/.pvar/.psam behind the same row interface
-void open_rows(const Params& p, BedFile& g, const std::set<std::string>& excl, const std::set<std::string>& extr,
-               const std::set<std::string>& rem, const std::set<std::string>& keep, Log& log) {
-  g.sex_specific = p.sex_specific;
-  if (p.sex_specific) log << "   -keeping only " << (p.sex_specific == 1 ? "male" : "female") << " individuals in the analysis\n";
-  if (!p.pgen.empty()) {
-    g.open_pgen(p.pgen, excl, extr, rem, keep, p.chrs);
-    log << " * pvar                : [" << p.pgen << ".pvar] n_snps = " << g.snps.size() << "\n";
-    log << " * psam                : [" << p.pgen << ".psam] n_samples = " << g.keys.size() << "\n";
-  } else {
-    g.open(p.bed, p.ref_first, excl, extr, rem, keep, p.chrs);
-    log << " * bim                 : [" << p.bed << ".bim] n_snps = " << g.snps.size() << "\n";
-    log << " * fam                 : [" << p.bed << ".fam] n_samples = " << g.keys.size() << "\n";
+// --range (in_range, src/Geno.cpp:2790-2800): keep the variants of one chromosome window
+void apply_range(const Params& p, std::vector<Snp>& snps) {
+  if (!p.set_range) return;
+  snps.erase(std::remove_if(snps.begin(), snps.end(), [&](const Snp& s) {
+               return s.chrom != p.range_chr || (double)s.pos < p.range_min || (double)s.pos > p.range_max;
+             }), snps.end());
+}
+
+// The genotype file of either step: 8-bit dosages of a .bgen (BgenFile), or 2-bit rows of a .bed or a .pgen (BedFile),
+// after --extract / --exclude / --chr, the --condition-list variants (which leave the tested set), --remove / --keep /
+// --sex-specific and --range (Step 1 switches --range off before it opens the file).  The sample view is that of
+// whichever reader is open.
+struct GenoInput {
+  const Params& p;
+  const bool use_bgen;
+  BedFile g;
+  BgenFile gg;
+  Conditioning cond;                                         // --condition-list
+  const std::vector<Snp>& snps;
+  const SampleSet ss;                                        // keys and key_to_ind of the kept samples
+  const std::vector<int32_t>& sample_idx;                    // file index of each kept sample
+  const std::vector<std::pair<std::string, std::string>>& ids_file;
+  const std::vector<int>& sex_file;
+  size_t n_file = 0;
+  bool subset = false;                                       // the file holds samples that are not analysed
+  int threads = 1;                                           // host threads (BGEN inflate, --htp counts)
+
+  GenoInput(const Params& p_, Log& log)
+      : p(p_), use_bgen(!p_.bgen.empty()), snps(use_bgen ? gg.snps : g.snps),
+        ss{use_bgen ? gg.keys : g.keys, use_bgen ? gg.key_to_ind : g.key_to_ind},
+        sample_idx(use_bgen ? gg.sample_idx : g.sample_idx), ids_file(use_bgen ? gg.ids_file : g.ids_file),
+        sex_file(use_bgen ? gg.sex_file : g.sex_file) {
+    const auto extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2), keep = read_id_list(p.keep, 2);
+    std::set<std::string> excl = read_id_list(p.exclude, 1);
+    if (!p.cond_list.empty()) {
+      // --condition-list [--condition-file]: the list is read before the genotype file is set up (get_conditional_vars,
+      // src/Geno.cpp:4151-4179); its IDs join the exclusion set, on top of --exclude / --extract
+      cond.list_file = p.cond_list;
+      cond.fmt = p.cond_fmt; cond.file = p.cond_file; cond.sample_file = p.cond_sample;
+      cond.max_vars = p.max_cond;
+      cond.ref_first = p.ref_first;
+      cond.read_list();
+      excl.insert(cond.ids.begin(), cond.ids.end());
+      if (!p.extract.empty()) log << "WARNING: only variants which satisfy both extract/exclude options will be kept.\n";   // src/Regenie.cpp:1081-1082
+    }
+    // check_samples_include_exclude (src/Geno.cpp:1286-1293)
+    if (p.sex_specific) log << "   -keeping only " << (p.sex_specific == 1 ? "male" : "female") << " individuals in the analysis\n";
+    gg.sex_specific = g.sex_specific = p.sex_specific;
+    if (use_bgen) {
+      gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keep, p.chrs, p.bgi);
+      if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
+      log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
+    } else if (!p.pgen.empty()) {
+      g.open_pgen(p.pgen, excl, extr, rem, keep, p.chrs);
+      log << " * pvar                : [" << p.pgen << ".pvar] n_snps = " << g.snps.size() << "\n";
+      log << " * psam                : [" << p.pgen << ".psam] n_samples = " << g.keys.size() << "\n";
+    } else {
+      g.open(p.bed, p.ref_first, excl, extr, rem, keep, p.chrs);
+      log << " * bim                 : [" << p.bed << ".bim] n_snps = " << g.snps.size() << "\n";
+      log << " * fam                 : [" << p.bed << ".fam] n_samples = " << g.keys.size() << "\n";
+    }
+    apply_range(p, gg.snps);
+    apply_range(p, g.snps);
+    if (g.pg) apply_range(p, g.pg->snps);
+    if (p.set_range && snps.empty()) throw Fail("no variant left to include in analysis.");
+    if (cond.on() && !cond.external())             // same-file conditioning: the listed IDs among the variants after --chr / --range
+      cond.locate_in_main(use_bgen ? "bgen" : !p.pgen.empty() ? "pgen" : "bed", use_bgen ? p.bgen : !p.pgen.empty() ? p.pgen : p.bed,
+                          p.sample, p.bgi, p.chrs, p.set_range, p.range_chr, p.range_min, p.range_max);
+    n_file = use_bgen ? gg.n_file : g.keys_file.size();
+    subset = ss.keys.size() != n_file;
+    threads = p.threads > 0 ? p.threads : (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
   }
+
+  const int32_t* sidx() const { return subset ? sample_idx.data() : nullptr; }
+};
+
+// phenotypes and covariates of the kept samples (read_pheno_and_cov), then the --condition-list columns
+void read_pheno(const Params& p, GenoInput& in, bool step2, Pheno& ph, Log& log) {
+  ph.pheno_cols = p.pheno_cols; ph.covar_cols = p.covar_cols; ph.rint = p.rint && !p.bt; ph.cat_cols = p.cat_cols; ph.max_cat_levels = p.max_cat_levels;
+  ph.pheno_excl = p.pheno_excl; ph.covar_excl = p.covar_excl; ph.min_case_count = p.min_case_count;
+  read_pheno_and_cov(in.ss, p.pheno, p.covar, step2, p.strict, p.bt, ph, log);
+  if (in.cond.on()) in.cond.append(in.ss, ph, log);
 }
 
-// --condition-list [--condition-file]: reads the list (get_conditional_vars, src/Geno.cpp:4151-4179, which runs before the
-// genotype file is set up); the IDs join the exclusion set `excl` of the main reader, on top of --exclude / --extract
-void init_conditioning(const Params& p, Conditioning& c, std::set<std::string>& excl, Log& log) {
-  if (p.cond_list.empty()) return;
-  c.list_file = p.cond_list;
-  c.fmt = p.cond_fmt; c.file = p.cond_file; c.sample_file = p.cond_sample;
-  c.max_vars = p.max_cond;
-  c.ref_first = p.ref_first;
-  c.read_list();
-  excl.insert(c.ids.begin(), c.ids.end());
-  if (!p.extract.empty()) log << "WARNING: only variants which satisfy both extract/exclude options will be kept.\n";   // src/Regenie.cpp:1081-1082
+// Runs f(d) for the devices d < G: inline for one device, else on one host thread per device; once all have finished, the
+// first error in device order is rethrown.
+template <typename F>
+void on_devices(int G, F&& f) {
+  if (G == 1) { f(0); return; }
+  std::vector<std::string> errs(G);
+  std::vector<std::thread> workers;
+  for (int d = 0; d < G; ++d)
+    workers.emplace_back([&, d] {
+      try { f(d); } catch (const std::exception& e) { errs[d] = e.what(); }
+    });
+  for (auto& w : workers) w.join();
+  for (const auto& e : errs) if (!e.empty()) throw Fail(e);
 }
 
-// same-file conditioning: the listed IDs among the variants of the main genotype file after --chr / --range
-void locate_conditioning(const Params& p, Conditioning& c) {
-  if (!c.on() || c.external()) return;
-  const std::string fmt = !p.bgen.empty() ? "bgen" : !p.pgen.empty() ? "pgen" : "bed";
-  c.locate_in_main(fmt, !p.bgen.empty() ? p.bgen : !p.pgen.empty() ? p.pgen : p.bed, p.sample, p.bgi, p.chrs, p.set_range,
-                   p.range_chr, p.range_min, p.range_max);
-}
-
+// ------------------------------------------------------------------------------------ step 1
 // ---- --split-l0 / --run-l0 / --run-l1 (src/Data.cpp:232-309, 818-908): level 0 as independent jobs that exchange
 // the N x R slabs of write_l0_file through <prefix>_job<j>_l0_Y<k>; files are interchangeable with the reference's.
 struct MasterJob { std::string prefix; int nblocks; long nsnps; };
@@ -445,8 +508,9 @@ void write_master(const Params& p, const std::vector<Snp>& snps, const std::vect
   }
 }
 
-void run_step1(const Params& p_in, Log& log) {
-  Params p = p_in;
+// the options Step 1 switches off, and the master file of a --run-l0 / --run-l1 job (a --run-l0 job reads the variants of
+// its own blocks and writes its slabs under the job prefix)
+Master setup_jobs(Params& p, Log& log) {
   if (p.af_cc) log << "WARNING: disabling option --af-cc (only for BTs in step 2 in native output format split by trait).\n";
   if (p.set_range) { log << "WARNING: option --range only works for step 2.\n"; p.set_range = false; }
   Master master;
@@ -458,134 +522,221 @@ void run_step1(const Params& p_in, Log& log) {
     p.exclude.clear();
     p.lowmem_prefix = master.jobs[p.run_l0_job - 1].prefix;
   }
-  // genotype input: 2-bit rows (.bed / decoded .pgen) or 8-bit dosages (.bgen, readChunkFromBGENFileToG_fast src/Geno.cpp:1574)
-  const bool use_bgen = !p.bgen.empty();
-  BedFile gbed;
-  BgenFile gg;
-  Conditioning cond;
-  std::set<std::string> excl = read_id_list(p.exclude, 1);
-  init_conditioning(p, cond, excl, log);
-  if (use_bgen) {
-    gg.open(p.bgen, p.sample, p.ref_first, excl, read_id_list(p.extract, 1), read_id_list(p.remove, 2),
-            read_id_list(p.keep, 2), p.chrs, p.bgi);
-    if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
-    log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
-  } else {
-    open_rows(p, gbed, excl, read_id_list(p.extract, 1), read_id_list(p.remove, 2), read_id_list(p.keep, 2), log);
-  }
-  locate_conditioning(p, cond);
-  // the fields of either reader the rest of Step 1 needs
-  struct GenoView {
-    const std::vector<Snp>& snps;
-    const std::vector<std::string>& keys;
-    const std::map<std::string, uint32_t>& key_to_ind;
-    const std::vector<int32_t>& sample_idx;
-    size_t n_file;
-    size_t row_stride;
-  };
-  const GenoView g = use_bgen ? GenoView{gg.snps, gg.keys, gg.key_to_ind, gg.sample_idx, (size_t)gg.n_file, 0}
-                              : GenoView{gbed.snps, gbed.keys, gbed.key_to_ind, gbed.sample_idx, gbed.keys_file.size(), (size_t)gbed.row_stride};
-  if (g.snps.empty()) throw Fail("no variant left to include in analysis.");
-  if (g.snps.size() > 1000000 && !p.force_step1)
-    throw Fail("it is not recommened to use more than 1000000 variants in step 1 (otherwise use '--force-step1').");
+  return master;
+}
+
+// Step 1 (Data::run_step1, src/Data.cpp:95-133) as a sequence of phases over one state; run_step1 lists them.
+// --gpus G: one handle per device, all describing the same problem.  Level-0 blocks are partitioned contiguously by the
+// reference's --split-l0 rule (write_l0_master, src/Data.cpp:268-301), level 1 by phenotype (p mod G); every GPU stores the
+// predictor tiles of a phenotype straight into the HBM of the GPU that owns it (peer access over NVLink), so there is no
+// exchange step and no file protocol.  Results do not depend on G (fixed-order reductions); one GPU is G = 1, where device 0
+// feeds every block and owns every phenotype.
+struct Step1 {
+  Params p;
+  Log& log;
+  const Master master;
+  GenoInput in;
   Pheno ph;
-  ph.pheno_cols = p.pheno_cols; ph.covar_cols = p.covar_cols; ph.rint = p.rint && !p.bt; ph.cat_cols = p.cat_cols; ph.max_cat_levels = p.max_cat_levels;
-  ph.pheno_excl = p.pheno_excl; ph.covar_excl = p.covar_excl; ph.min_case_count = p.min_case_count;
-  read_pheno_and_cov(SampleSet{g.keys, g.key_to_ind}, p.pheno, p.covar, false, p.strict, p.bt, ph, log);
-  if (cond.on()) cond.append(SampleSet{g.keys, g.key_to_ind}, ph, log);
-  prep_run(ph, nullptr, log);
-  if (p.bt && !p.loocv) {
-    if (ph.n_analyzed < 5000) {                       // src/Data.cpp:353-356
+  std::vector<Block> blocks;
+  int nb = 0, P = 0, G = 1;
+  int64_t N = 0;
+  std::vector<double> h1;                                    // level-1 ridge grid
+  std::vector<rg_handle> hs;                                 // one handle per device
+  std::vector<uint8_t> l1_sel;
+  double B = 0;                                              // level-1 predictors: blocks x level-0 ridge values
+  std::vector<double> tau, cs, loco, prs;
+  std::vector<int32_t> best;
+
+  Step1(const Params& p_in, Log& log_) : p(p_in), log(log_), master(setup_jobs(p, log_)), in(p, log_) {}
+  ~Step1() {                                                 // errors unwind through here
+    for (auto& h : hs) if (h && !g_fast_exit) rg_destroy(h);
+  }
+  rg_handle owner_of(int ph_i) const { return hs[ph_i % G]; }
+
+  // phenotypes, covariates (and conditioning columns), blocks
+  void read_inputs() {
+    if (in.snps.empty()) throw Fail("no variant left to include in analysis.");
+    if (in.snps.size() > 1000000 && !p.force_step1)
+      throw Fail("it is not recommened to use more than 1000000 variants in step 1 (otherwise use '--force-step1').");
+    read_pheno(p, in, false, ph, log);
+    prep_run(ph, nullptr, log);
+    if (p.bt && !p.loocv && ph.n_analyzed < 5000) {            // src/Data.cpp:353-356
       log << "   -WARNING: Sample size is less than 5,000 so using LOOCV instead of " << p.cv << "-fold CV.\n";
       p.loocv = true;
     }
-  }
-  const auto blocks = set_blocks(g.snps, p.bsize);
-  const int nb = (int)blocks.size();
-  if (p.split_jobs) { write_master(p, g.snps, blocks, log); return; }
-  if (p.run_l0_job) {
-    const MasterJob& mj = master.jobs[p.run_l0_job - 1];
-    if (mj.nblocks != nb || mj.nsnps != (long)g.snps.size())
-      throw Fail("number of variants/blocks in file (=" + std::to_string(g.snps.size()) + "/" + std::to_string(nb) +
-                 ") don't match with that in master file (=" + std::to_string(mj.nsnps) + "/" + std::to_string(mj.nblocks) + ").");
-  }
-  if (p.run_l1) {
-    long tb = 0, ts = 0;
-    for (auto& j : master.jobs) { tb += j.nblocks; ts += j.nsnps; }
-    if (tb != nb || ts != (long)g.snps.size())
-      throw Fail("number of blocks/variants in master file '" + p.master + "' doesn't match that in the analysis.");
-    log << " * using results from running " << master.jobs.size() << " parallel jobs at level 0\n";
-  }
-  const int64_t N = ph.N;
-  const int P = ph.P;
-  std::vector<int64_t> folds;
-  if (!p.loocv) folds = set_folds(ph.in_analysis, p.cv);
-  if ((p.setl0.empty() && p.l0 < 2) || (p.setl1.empty() && p.l1 < 2))                 // set_ridge_params, src/Regenie.cpp:1499-1500
-    throw Fail("number of ridge parameters must be at least 2 (=" + std::to_string(p.setl0.empty() && p.l0 < 2 ? p.l0 : p.l1) + ")");
-  const auto h0 = p.setl0.empty() ? ridge_grid(p.l0) : p.setl0, h1 = p.setl1.empty() ? ridge_grid(p.l1) : p.setl1;
-  std::vector<double> lambda(p.l0);
-  const double M = p.run_l0_job ? (double)master.n_geno : (double)g.snps.size();     // src/Data.cpp:607
-  for (int j = 0; j < p.l0; ++j) lambda[j] = M * (1 - h0[j]) / h0[j];           // src/Data.cpp:607
-  log << " * # blocks            : [" << nb << "] for " << g.snps.size() << " variants\n";
-  log << " * # CV folds          : [" << (p.loocv ? ph.n_analyzed : p.cv) << "]\n";
-
-  rg_step1_config cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.device = p.gpu; cfg.n_samples = N; cfg.n_cov = ph.C; cfg.n_pheno = P; cfg.n_folds = p.cv;
-  cfg.n_ridge_l0 = p.l0; cfg.n_ridge_l1 = p.l1; cfg.loocv = p.loocv; cfg.max_block_size = p.bsize;
-  cfg.total_blocks = nb; cfg.n_analyzed = ph.n_analyzed;
-  // --gpus G: one handle per device, all describing the same problem.  Level-0 blocks are partitioned contiguously by the
-  // reference's --split-l0 rule (write_l0_master, src/Data.cpp:268-301), level 1 by phenotype (p mod G); every GPU stores the
-  // predictor tiles of a phenotype straight into the HBM of the GPU that owns it (peer access over NVLink), so there is no
-  // exchange step and no file protocol.  Results do not depend on G (fixed-order reductions).
-  const int G = std::max(1, p.gpus);
-  if (G > 1) {
-    if (G > rg_device_count()) throw Fail("--gpus " + std::to_string(G) + " but only " + std::to_string(rg_device_count()) + " CUDA device(s) visible.");
-    if (G > nb) throw Fail("number of GPUs cannot be greater than number of blocks.");
-    if (p.run_l0_job || p.run_l1 || p.split_jobs) throw Fail("--gpus N shards one run; it cannot be combined with --split-l0 / --run-l0 / --run-l1.");
-    log << " * sharding level 0 over " << G << " GPUs (blocks), level 1 by phenotype\n";
-  }
-  phase("inputs parsed");
-  require_device();
-  phase("cuda context");
-  std::vector<rg_handle> hs(G, nullptr);
-  struct HandlesGuard {
-    std::vector<rg_handle>& v;
-    ~HandlesGuard() { for (auto& x : v) { if (x && !g_fast_exit) rg_destroy(x); x = nullptr; } }
-  } guards{hs};
-  for (int d = 0; d < G; ++d) {
-    cfg.device = (G > 1 ? d : p.gpu);
-    rg_check(rg_step1_create(&cfg, ph.X.data(), ph.Y.data(), ph.mask.data(), ph.in_analysis.data(),
-                             p.loocv ? nullptr : folds.data(), lambda.data(), ph.neff.data(), &hs[d]));
-  }
-  rg_handle h = hs[0];
-  phase("rg_step1_create");
-  std::vector<std::vector<uint8_t>> owned(G, std::vector<uint8_t>(P, 0));
-  if (G > 1) {
-    for (int i = 0; i < P; ++i) owned[i % G][i] = 1;
-    for (int d = 0; d < G; ++d) rg_check(rg_W_set_owned(hs[d], owned[d].data()));
-    for (int d = 0; d < G; ++d)
-      for (int e = 0; e < G; ++e)
-        if (e != d) rg_check(rg_W_attach_local(hs[d], hs[e], owned[e].data()));
-  }
-  auto owner_of = [&](int ph_i) { return hs[G > 1 ? ph_i % G : 0]; };
-
-  // --l1-phenoList (with --run-l1): level 1 only for the named phenotypes (select_pheno_l1, src/Regenie.cpp:862-868)
-  std::vector<uint8_t> l1_sel(P, 1);
-  if (p.run_l1 && !p.l1_phenos.empty()) {
-    bool any = false;
-    for (int i = 0; i < P; ++i) { l1_sel[i] = p.l1_phenos.count(ph.names[i]) ? 1 : 0; any |= l1_sel[i] != 0; }
-    if (!any) throw Fail("none of the phenotypes in --l1-phenoList is in the phenotype file.");
-    rg_check(rg_l1_select(h, l1_sel.data()));
+    blocks = set_blocks(in.snps, p.bsize);
+    nb = (int)blocks.size();
+    N = ph.N;
+    P = ph.P;
   }
 
-  // ---- level 0
-  std::vector<uint8_t> rows(use_bgen ? 0 : (size_t)p.bsize * g.row_stride);
-  const bool subset = g.keys.size() != g.n_file;
-  int last_chr = -1;
-  const double t0 = now_ms();
-  if (p.run_l1) {
-    // read_l0 / read_l0_chunk (src/Step1_Models.cpp:1921-1987): columns [bstart*R, (bstart+btot)*R) from every job file
+  // --split-l0 writes the master file (false: the run ends there); --run-l0 / --run-l1 check the blocks against it
+  bool check_jobs() {
+    if (p.split_jobs) { write_master(p, in.snps, blocks, log); return false; }
+    if (p.run_l0_job) {
+      const MasterJob& mj = master.jobs[p.run_l0_job - 1];
+      if (mj.nblocks != nb || mj.nsnps != (long)in.snps.size())
+        throw Fail("number of variants/blocks in file (=" + std::to_string(in.snps.size()) + "/" + std::to_string(nb) +
+                   ") don't match with that in master file (=" + std::to_string(mj.nsnps) + "/" + std::to_string(mj.nblocks) + ").");
+    }
+    if (p.run_l1) {
+      long tb = 0, ts = 0;
+      for (auto& j : master.jobs) { tb += j.nblocks; ts += j.nsnps; }
+      if (tb != nb || ts != (long)in.snps.size())
+        throw Fail("number of blocks/variants in master file '" + p.master + "' doesn't match that in the analysis.");
+      log << " * using results from running " << master.jobs.size() << " parallel jobs at level 0\n";
+    }
+    return true;
+  }
+
+  // folds and ridge grids, one handle per device, the owner of each phenotype's W, --l1-phenoList
+  void create_handles() {
+    std::vector<int64_t> folds;
+    if (!p.loocv) folds = set_folds(ph.in_analysis, p.cv);
+    if ((p.setl0.empty() && p.l0 < 2) || (p.setl1.empty() && p.l1 < 2))                 // set_ridge_params, src/Regenie.cpp:1499-1500
+      throw Fail("number of ridge parameters must be at least 2 (=" + std::to_string(p.setl0.empty() && p.l0 < 2 ? p.l0 : p.l1) + ")");
+    const auto h0 = p.setl0.empty() ? ridge_grid(p.l0) : p.setl0;
+    h1 = p.setl1.empty() ? ridge_grid(p.l1) : p.setl1;
+    std::vector<double> lambda(p.l0);
+    const double M = p.run_l0_job ? (double)master.n_geno : (double)in.snps.size();     // src/Data.cpp:607
+    for (int j = 0; j < p.l0; ++j) lambda[j] = M * (1 - h0[j]) / h0[j];           // src/Data.cpp:607
+    log << " * # blocks            : [" << nb << "] for " << in.snps.size() << " variants\n";
+    log << " * # CV folds          : [" << (p.loocv ? ph.n_analyzed : p.cv) << "]\n";
+
+    rg_step1_config cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.device = p.gpu; cfg.n_samples = N; cfg.n_cov = ph.C; cfg.n_pheno = P; cfg.n_folds = p.cv;
+    cfg.n_ridge_l0 = p.l0; cfg.n_ridge_l1 = p.l1; cfg.loocv = p.loocv; cfg.max_block_size = p.bsize;
+    cfg.total_blocks = nb; cfg.n_analyzed = ph.n_analyzed;
+    G = std::max(1, p.gpus);
+    if (G > 1) {
+      if (G > rg_device_count()) throw Fail("--gpus " + std::to_string(G) + " but only " + std::to_string(rg_device_count()) + " CUDA device(s) visible.");
+      if (G > nb) throw Fail("number of GPUs cannot be greater than number of blocks.");
+      if (p.run_l0_job || p.run_l1 || p.split_jobs) throw Fail("--gpus N shards one run; it cannot be combined with --split-l0 / --run-l0 / --run-l1.");
+      log << " * sharding level 0 over " << G << " GPUs (blocks), level 1 by phenotype\n";
+    }
+    phase("inputs parsed");
+    require_device();
+    phase("cuda context");
+    hs.assign(G, nullptr);
+    for (int d = 0; d < G; ++d) {
+      cfg.device = (G > 1 ? d : p.gpu);
+      rg_check(rg_step1_create(&cfg, ph.X.data(), ph.Y.data(), ph.mask.data(), ph.in_analysis.data(),
+                               p.loocv ? nullptr : folds.data(), lambda.data(), ph.neff.data(), &hs[d]));
+    }
+    phase("rg_step1_create");
+    if (G > 1) {
+      std::vector<std::vector<uint8_t>> owned(G, std::vector<uint8_t>(P, 0));
+      for (int i = 0; i < P; ++i) owned[i % G][i] = 1;
+      for (int d = 0; d < G; ++d) rg_check(rg_W_set_owned(hs[d], owned[d].data()));
+      for (int d = 0; d < G; ++d)
+        for (int e = 0; e < G; ++e)
+          if (e != d) rg_check(rg_W_attach_local(hs[d], hs[e], owned[e].data()));
+    }
+    // --l1-phenoList (with --run-l1, so one device): level 1 only for the named phenotypes (select_pheno_l1, src/Regenie.cpp:862-868)
+    l1_sel.assign(P, 1);
+    if (p.run_l1 && !p.l1_phenos.empty()) {
+      bool any = false;
+      for (int i = 0; i < P; ++i) { l1_sel[i] = p.l1_phenos.count(ph.names[i]) ? 1 : 0; any |= l1_sel[i] != 0; }
+      if (!any) throw Fail("none of the phenotypes in --l1-phenoList is in the phenotype file.");
+      rg_check(rg_l1_select(hs[0], l1_sel.data()));
+    }
+  }
+
+  // Blocks [first, last) into the handle of device d.  Reader threads fetch blocks b+1 and b+2 from the file while block b
+  // is handed to the GPU (three buffers in rotation).  .bed rows sit in PINNED buffers (rg_host_alloc), so a block crosses
+  // PCIe by DMA straight from the buffer the reader filled (a pageable buffer is first copied into the driver's staging
+  // area, ~5 ms per 25 MB block); rg_l0_wait_input after each call tells when the buffer may be refilled.  Pageable
+  // inputs (.bgen bytes, .pgen records) are staged before their call returns and can be refilled at once.
+  void feed_l0(int d, int first, int last, bool pgen_dev, std::mutex& io_mu, std::mutex& log_mu) {
+    constexpr int kBuf = 3, kAhead = 2;
+    const rg_handle h = hs[d];
+    const bool use_bgen = in.use_bgen;
+    // Two reads in flight where the reader is re-entrant: pread on the .bed, the records of the in-memory .pgen.  One
+    // where reads share state: the stream fallback of the .bed reader (a file cursor, which the feeds of the other devices
+    // share too, hence the lock) and the host .pgen decoder (the record it decoded last).  The .bgen reader maps the file
+    // and its read_block is const; it keeps one read in flight.
+    const bool shared = !use_bgen && !pgen_dev && (in.g.pg || in.g.bed_fd < 0);
+    const int ahead = (use_bgen || shared) ? 1 : kAhead;
+    const int bgen_threads = std::max(1, in.threads / G);
+    const size_t row_bytes = (use_bgen || pgen_dev) ? 0 : (size_t)p.bsize * in.g.row_stride;
+    struct PinnedSet {
+      void* p[kBuf] = {nullptr, nullptr, nullptr};
+      ~PinnedSet() { for (void* q : p) if (q && !g_fast_exit) rg_host_free(q); }
+    } pinned;
+    std::vector<uint8_t> pageable[kBuf];
+    uint8_t* bufs[kBuf];
+    bool pin = row_bytes > 0;
+    for (int k = 0; k < kBuf && pin; ++k) pin = rg_host_alloc(&pinned.p[k], (int64_t)row_bytes) == 0;
+    for (int k = 0; k < kBuf; ++k) {
+      if (!pin) pageable[k].resize(row_bytes);
+      bufs[k] = pin ? (uint8_t*)pinned.p[k] : pageable[k].data();
+    }
+    std::vector<uint8_t> probs[kBuf], pmiss[kBuf];               // .bgen: inflated probability pairs + ploidy bytes of a block
+    if (use_bgen)
+      for (int k = 0; k < kBuf; ++k) { probs[k].resize((size_t)p.bsize * in.n_file * 2); pmiss[k].resize((size_t)p.bsize * in.n_file); }
+    PgenBatch pbatch[kBuf];
+    std::future<void> pending[kBuf];                              // after the buffers: an error waits for the reads here
+    auto fetch = [&](int b) {
+      return std::async(std::launch::async, [&, b] {
+        const int k = b % kBuf;
+        if (use_bgen) in.gg.read_block(blocks[b].first, blocks[b].size, probs[k].data(), pmiss[k].data(), bgen_threads);
+        else if (pgen_dev) in.g.pg->gather(blocks[b].first, blocks[b].size, pbatch[k]);
+        else if (shared) { std::lock_guard<std::mutex> lk(io_mu); in.g.read_rows(blocks[b].first, blocks[b].size, bufs[k]); }
+        else in.g.read_rows(blocks[b].first, blocks[b].size, bufs[k]);
+      });
+    };
+    const std::string gpu_tag = G > 1 ? " (gpu " + std::to_string(d) + ")" : "";
+    int last_chr = -1;
+    for (int b = first; b < first + ahead && b < last; ++b) pending[b % kBuf] = fetch(b);
+    for (int b = first; b < last; ++b) {
+      const int k = b % kBuf, bs = blocks[b].size;
+      if (G == 1 && blocks[b].chrom != last_chr) { log << "Chromosome " << blocks[b].chrom << "\n"; last_chr = blocks[b].chrom; }
+      pending[k].get();
+      if (b + ahead < last) pending[(b + ahead) % kBuf] = fetch(b + ahead);      // its buffer was block b-1's (or b's own slot + 1): consumed
+      if (use_bgen) {
+        rg_check(rg_l0_block_dosage_u8(h, probs[k].data(), pmiss[k].data(), (int64_t)in.n_file, bs, in.sidx(), p.ref_first, b));
+      } else {
+        const uint8_t* rows = bufs[k];
+        int64_t stride = (int64_t)in.g.row_stride;
+        if (pgen_dev) pgen_rows_device(h, pbatch[k], bs, (int64_t)in.g.pg->n_file, b, &rows, &stride);
+        rg_check(rg_l0_block_bed(h, rows, stride, bs, in.sidx(), p.ref_first, b));
+        if (pin) rg_check(rg_l0_wait_input(h));
+      }
+      std::lock_guard<std::mutex> lk(log_mu);
+      log << " block [" << b + 1 << "] : " << bs << " snps" << gpu_tag << "\n";
+    }
+  }
+
+  // level 0 over the blocks of every device (with --run-l1: the slabs of the job files instead)
+  void level0() {
+    const double t0 = now_ms();
+    if (p.run_l1) read_l0_files();
+    const bool pgen_dev = !in.use_bgen && in.g.pg && pgen_on_device();
+    if (pgen_dev) log << " * pgen records are decoded on the GPU\n";
+    if (!p.run_l1) {
+      std::mutex io_mu, log_mu;
+      const int nall = nb / G, rem = nb - nall * G;             // write_l0_master's partition
+      on_devices(G, [&](int d) {
+        const int first = d * nall + std::min(d, rem);
+        feed_l0(d, first, first + nall + (d < rem ? 1 : 0), pgen_dev, io_mu, log_mu);
+      });
+    }
+    for (int d = 0; d < G; ++d) {
+      const int64_t st = rg_l0_status(hs[d]);
+      if (st != 0) {
+        if (st > 0 && st < (1ll << 40))
+          throw Fail("!! Uh-oh, SNP " + in.snps[blocks[(st - 1) / p.bsize].first + (st - 1) % p.bsize].id + " has low variance.");
+        throw Fail(std::string(rg_last_error()));
+      }
+    }
+    log << " Level 0 done (" << (long)(now_ms() - t0) << "ms)\n";
+    phase("level 0");
+  }
+
+  // ---- level-0 slab files
+  // --run-l1: read_l0 / read_l0_chunk (src/Step1_Models.cpp:1921-1987): columns [bstart*R, (bstart+btot)*R) from every job file
+  void read_l0_files() {
     log << " (skipping to level 1 models)\n";
     std::vector<double> slab((size_t)N * p.l0);
     for (int ph_i = 0; ph_i < P; ++ph_i) {
@@ -605,303 +756,196 @@ void run_step1(const Params& p_in, Log& log) {
       }
     }
   }
-  // reader threads fetch blocks b+1 and b+2 from the file while block b is handed to the GPU (three buffers in rotation).
-  // .bed rows sit in PINNED buffers (rg_host_alloc), so a block crosses PCIe by DMA straight from the buffer the reader
-  // filled (a pageable buffer is first copied into the driver's staging area, ~5 ms per 25 MB block); rg_l0_wait_input
-  // after each call tells when the buffer may be refilled.  Pageable inputs (.bgen bytes, .pgen records) are staged
-  // before their call returns and can be refilled at once.
-  constexpr int kBuf = 3, kAhead = 2;
-  struct PinnedSet {
-    void* p[kBuf] = {nullptr, nullptr, nullptr};
-    ~PinnedSet() { for (void* q : p) if (q && !g_fast_exit) rg_host_free(q); }
-  } pinned;
-  std::vector<uint8_t> rows_extra[kBuf];
-  uint8_t* bufs[kBuf] = {rows.data(), nullptr, nullptr};
-  bool pin_rows = !use_bgen && !p.run_l1 && G == 1 && !rows.empty() && !(gbed.pg && pgen_on_device());
-  for (int k = 0; k < kBuf && pin_rows; ++k) pin_rows = rg_host_alloc(&pinned.p[k], (int64_t)rows.size()) == 0;
-  for (int k = 0; k < kBuf; ++k) {
-    if (pin_rows) bufs[k] = (uint8_t*)pinned.p[k];
-    else if (k > 0) { rows_extra[k].resize(rows.size()); bufs[k] = rows_extra[k].data(); }
-  }
-  std::vector<uint8_t> probs[kBuf], pmiss[kBuf];               // .bgen: inflated probability pairs + ploidy bytes of a block
-  if (use_bgen && !p.run_l1)
-    for (int k = 0; k < kBuf; ++k) { probs[k].resize((size_t)p.bsize * g.n_file * 2); pmiss[k].resize((size_t)p.bsize * g.n_file); }
-  const int io_threads = std::max(1, std::min(32, (int)std::thread::hardware_concurrency()));
-  const bool pgen_dev = !use_bgen && gbed.pg && pgen_on_device();
-  if (pgen_dev) log << " * pgen records are decoded on the GPU\n";
-  PgenBatch pbatch[kBuf];
-  std::future<void> pending[kBuf];
-  auto fetch = [&](int b) {
-    return std::async(std::launch::async, [&, b] {
-      const int k = b % kBuf;
-      if (use_bgen) gg.read_block(blocks[b].first, blocks[b].size, probs[k].data(), pmiss[k].data(), io_threads);
-      else if (pgen_dev) gbed.pg->gather(blocks[b].first, blocks[b].size, pbatch[k]);
-      else gbed.read_rows(blocks[b].first, blocks[b].size, bufs[k]);
-    });
-  };
-  if (G == 1) {
-    // two reads in flight only where the reader is re-entrant (pread on the .bed, the in-memory .pgen); the .bgen reader
-    // and the stream fallback of the .bed reader share a file cursor
-    const int ahead = (use_bgen || (!gbed.pg && gbed.bed_fd < 0)) ? 1 : kAhead;
-    for (int b = 0; b < ahead && b < nb && !p.run_l1; ++b) pending[b % kBuf] = fetch(b);
-    for (int b = 0; b < nb && !p.run_l1; ++b) {
-      if (blocks[b].chrom != last_chr) { log << "Chromosome " << blocks[b].chrom << "\n"; last_chr = blocks[b].chrom; }
-      const int k = b % kBuf;
-      pending[k].get();
-      if (b + ahead < nb) pending[(b + ahead) % kBuf] = fetch(b + ahead);      // its buffer was block b-1's (or b's own slot + 1): consumed
-      if (use_bgen)
-        rg_check(rg_l0_block_dosage_u8(h, probs[k].data(), pmiss[k].data(), (int64_t)g.n_file, blocks[b].size,
-                                       subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-      else if (pgen_dev) {
-        const uint8_t* drows = nullptr;
-        int64_t dstride = 0;
-        pgen_rows_device(h, pbatch[k], blocks[b].size, (int64_t)gbed.pg->n_file, b, &drows, &dstride);
-        rg_check(rg_l0_block_bed(h, drows, dstride, blocks[b].size, subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-      } else {
-        rg_check(rg_l0_block_bed(h, bufs[k], (int64_t)g.row_stride, blocks[b].size,
-                                 subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-        if (pin_rows) rg_check(rg_l0_wait_input(h));
-      }
-      log << " block [" << b + 1 << "] : " << blocks[b].size << " snps\n";
-    }
-  } else {
-    // one host thread per GPU, each feeding its contiguous block range; the .bed stream is shared, so reads take a lock
-    std::mutex io_mu, log_mu;
-    std::vector<std::string> errs(G);
-    std::vector<std::thread> workers;
-    const int nall = nb / G, rem = nb - nall * G;
-    int b0 = 0;
-    for (int d = 0; d < G; ++d) {
-      const int cnt = nall + (d < rem ? 1 : 0), first = b0;
-      b0 += cnt;
-      workers.emplace_back([&, d, first, cnt] {
-        try {
-          std::vector<uint8_t> buf(use_bgen ? 0 : (size_t)p.bsize * g.row_stride), pr, pm;
-          if (use_bgen) { pr.resize((size_t)p.bsize * g.n_file * 2); pm.resize((size_t)p.bsize * g.n_file); }
-          for (int b = first; b < first + cnt; ++b) {
-            if (use_bgen) {
-              gg.read_block(blocks[b].first, blocks[b].size, pr.data(), pm.data(), std::max(1, io_threads / G));
-              rg_check(rg_l0_block_dosage_u8(hs[d], pr.data(), pm.data(), (int64_t)g.n_file, blocks[b].size,
-                                             subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-            } else if (pgen_dev) {
-              PgenBatch pb;                                  // gather only reads the mapped file: no lock
-              gbed.pg->gather(blocks[b].first, blocks[b].size, pb);
-              const uint8_t* drows = nullptr;
-              int64_t dstride = 0;
-              pgen_rows_device(hs[d], pb, blocks[b].size, (int64_t)gbed.pg->n_file, b, &drows, &dstride);
-              rg_check(rg_l0_block_bed(hs[d], drows, dstride, blocks[b].size, subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-            } else {
-              { std::lock_guard<std::mutex> lk(io_mu); gbed.read_rows(blocks[b].first, blocks[b].size, buf.data()); }
-              rg_check(rg_l0_block_bed(hs[d], buf.data(), (int64_t)g.row_stride, blocks[b].size,
-                                       subset ? g.sample_idx.data() : nullptr, p.ref_first, b));
-            }
-            std::lock_guard<std::mutex> lk(log_mu);
-            log << " block [" << b + 1 << "] : " << blocks[b].size << " snps (gpu " << d << ")\n";
-          }
-        } catch (const Fail& f) { errs[d] = f.what(); }
-        catch (const std::exception& e) { errs[d] = e.what(); }
-      });
-    }
-    for (auto& w : workers) w.join();
-    for (int d = 0; d < G; ++d) if (!errs[d].empty()) throw Fail(errs[d]);
-  }
-  for (int d = 0; d < G; ++d) {
-    const int64_t st = rg_l0_status(hs[d]);
-    if (st != 0) {
-      if (st > 0 && st < (1ll << 40))
-        throw Fail("!! Uh-oh, SNP " + g.snps[blocks[(st - 1) / p.bsize].first + (st - 1) % p.bsize].id + " has low variance.");
-      throw Fail(std::string(rg_last_error()));
-    }
-  }
-  log << " Level 0 done (" << (long)(now_ms() - t0) << "ms)\n";
-  phase("level 0");
-  if ((p.lowmem && p.keep_l0) || p.run_l0_job) {
-    // write_l0_file (src/Step1_Models.cpp:728-733): per phenotype, per block an N x R column-major f64 slab.
-    // The reference deletes these after level 1 unless --keep-l0 (src/Data.cpp:1011,1108,1131-1137); here W
-    // never leaves HBM for level 1, so the files are only materialised when they are kept.
-    const std::string pfx = p.lowmem_prefix.empty() ? p.out : p.lowmem_prefix;
-    log << "   -files will have prefix [" << pfx << "_l0_Y]\n";
-    std::vector<double> slab((size_t)N * p.l0);
-    for (int ph_i = 0; ph_i < P; ++ph_i) {
-      std::ofstream f(pfx + "_l0_Y" + std::to_string(ph_i + 1), std::ios::binary);
-      if (!f) throw Fail("cannot write temporary file " + pfx + "_l0_Y" + std::to_string(ph_i + 1));
-      for (int b = 0; b < nb; ++b) {
-        rg_check(rg_l0_fetch_W(owner_of(ph_i), b, ph_i, slab.data()));
-        f.write(reinterpret_cast<const char*>(slab.data()), (std::streamsize)(slab.size() * sizeof(double)));
-      }
-    }
-  }
-  if (p.run_l0_job) {
-    log << "\nDone writing level 0 predictions to file.\n";
-    return;
-  }
-  log << "\n Level 1 ridge...\n";
 
-  // ---- level 1 (tau = B(1-h)/h, src/Step1_Models.cpp:2115)
-  const double B = (double)nb * p.l0;
-  std::vector<double> tau((size_t)P * p.l1), cs((size_t)5 * P * p.l1);
-  const double tau_mult = p.bt ? 3.0 / (M_PI * M_PI) : 1.0;                     // src/Step1_Models.cpp:2115-2117
-  for (int ph_i = 0; ph_i < P; ++ph_i)
-    for (int j = 0; j < p.l1; ++j) tau[(size_t)ph_i * p.l1 + j] = B * (1 - h1[j]) / h1[j] * tau_mult;
-  std::vector<int32_t> best(P);
-  std::vector<double> bt_offs;
-  if (p.bt) {
-    // offset_nullreg: covariate-only logistic fit per trait (fit_null_logistic, src/Step1_Models.cpp:54-140)
-    std::vector<double> offs((size_t)N * P);
-    for (int ph_i = 0; ph_i < P; ++ph_i) {
-      const std::vector<double> eta = null_logistic_eta(ph.names[ph_i], &ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C,
-                                                        &ph.mask[(size_t)ph_i * N]);
-      std::copy(eta.begin(), eta.end(), offs.begin() + (size_t)ph_i * N);
+  // --lowmem --keep-l0 / --run-l0: write_l0_file (src/Step1_Models.cpp:728-733): per phenotype, per block an N x R
+  // column-major f64 slab.  The reference deletes these after level 1 unless --keep-l0 (src/Data.cpp:1011,1108,1131-1137);
+  // here W never leaves HBM for level 1, so the files are only materialised when they are kept.  False for a --run-l0
+  // job, which ends here.
+  bool write_l0_files() {
+    if ((p.lowmem && p.keep_l0) || p.run_l0_job) {
+      const std::string pfx = p.lowmem_prefix.empty() ? p.out : p.lowmem_prefix;
+      log << "   -files will have prefix [" << pfx << "_l0_Y]\n";
+      std::vector<double> slab((size_t)N * p.l0);
+      for (int ph_i = 0; ph_i < P; ++ph_i) {
+        std::ofstream f(pfx + "_l0_Y" + std::to_string(ph_i + 1), std::ios::binary);
+        if (!f) throw Fail("cannot write temporary file " + pfx + "_l0_Y" + std::to_string(ph_i + 1));
+        for (int b = 0; b < nb; ++b) {
+          rg_check(rg_l0_fetch_W(owner_of(ph_i), b, ph_i, slab.data()));
+          f.write(reinterpret_cast<const char*>(slab.data()), (std::streamsize)(slab.size() * sizeof(double)));
+        }
+      }
     }
-    cs.assign((size_t)6 * P * p.l1, 0.0);
-    if (G == 1) rg_check(rg_l1_fit_bt(h, ph.Y_raw.data(), offs.data(), tau.data(), cs.data(), best.data()));
-    else bt_offs = offs;
-  } else if (G == 1) {
-    rg_check(rg_l1_fit(h, tau.data(), cs.data(), best.data()));
+    if (p.run_l0_job) {
+      log << "\nDone writing level 0 predictions to file.\n";
+      return false;
+    }
+    return true;
   }
-  phase("level 1");
-  std::vector<int32_t> chr_of_block(nb);
-  for (int b = 0; b < nb; ++b) chr_of_block[b] = blocks[b].chrom;
-  std::vector<double> loco((size_t)P * 23 * N);
-  if (G == 1) {
-    rg_check(rg_loco(h, chr_of_block.data(), loco.data()));
-  } else {
-    // every GPU fits and assembles the phenotypes it owns, concurrently; the host merges disjoint supports
-    std::vector<std::string> errs(G);
-    std::vector<std::vector<double>> cs_d(G, std::vector<double>(cs.size(), 0.0)), loco_d(G);
+
+  // ---- level 1 (tau = B(1-h)/h, src/Step1_Models.cpp:2115), LOCO and PRS: every device fits and assembles the phenotypes
+  // it owns, concurrently; each phenotype's results are then taken from its owner
+  void level1() {
+    log << "\n Level 1 ridge...\n";
+    B = (double)nb * p.l0;
+    tau.resize((size_t)P * p.l1);
+    const double tau_mult = p.bt ? 3.0 / (M_PI * M_PI) : 1.0;                     // src/Step1_Models.cpp:2115-2117
+    for (int ph_i = 0; ph_i < P; ++ph_i)
+      for (int j = 0; j < p.l1; ++j) tau[(size_t)ph_i * p.l1 + j] = B * (1 - h1[j]) / h1[j] * tau_mult;
+    std::vector<double> offs;
+    if (p.bt) {
+      // offset_nullreg: covariate-only logistic fit per trait (fit_null_logistic, src/Step1_Models.cpp:54-140)
+      offs.resize((size_t)N * P);
+      for (int ph_i = 0; ph_i < P; ++ph_i) {
+        const std::vector<double> eta = null_logistic_eta(ph.names[ph_i], &ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C,
+                                                          &ph.mask[(size_t)ph_i * N]);
+        std::copy(eta.begin(), eta.end(), offs.begin() + (size_t)ph_i * N);
+      }
+    }
+    const int nsum = p.bt ? 6 : 5;                               // CV sums per (phenotype, ridge value)
+    std::vector<std::vector<double>> cs_d(G, std::vector<double>((size_t)nsum * P * p.l1, 0.0));
     std::vector<std::vector<int32_t>> best_d(G, std::vector<int32_t>(P, 0));
-    std::vector<std::thread> workers;
-    for (int d = 0; d < G; ++d)
-      workers.emplace_back([&, d] {
-        try {
-          if (p.bt) rg_check(rg_l1_fit_bt(hs[d], ph.Y_raw.data(), bt_offs.data(), tau.data(), cs_d[d].data(), best_d[d].data()));
-          else rg_check(rg_l1_fit(hs[d], tau.data(), cs_d[d].data(), best_d[d].data()));
-          loco_d[d].assign((size_t)P * 23 * N, 0.0);
-          rg_check(rg_loco(hs[d], chr_of_block.data(), loco_d[d].data()));
-        } catch (const Fail& f) { errs[d] = f.what(); }
-        catch (const std::exception& e) { errs[d] = e.what(); }
-      });
-    for (auto& w : workers) w.join();
-    for (int d = 0; d < G; ++d) if (!errs[d].empty()) throw Fail(errs[d]);
-    const int nsum = (int)(cs.size() / ((size_t)P * p.l1));
+    on_devices(G, [&](int d) {
+      if (p.bt) rg_check(rg_l1_fit_bt(hs[d], ph.Y_raw.data(), offs.data(), tau.data(), cs_d[d].data(), best_d[d].data()));
+      else rg_check(rg_l1_fit(hs[d], tau.data(), cs_d[d].data(), best_d[d].data()));
+    });
+    phase("level 1");
+    std::vector<int32_t> chr_of_block(nb);
+    for (int b = 0; b < nb; ++b) chr_of_block[b] = blocks[b].chrom;
+    std::vector<std::vector<double>> loco_d(G), prs_d(G);
+    on_devices(G, [&](int d) {
+      loco_d[d].resize((size_t)P * 23 * N);
+      rg_check(rg_loco(hs[d], chr_of_block.data(), loco_d[d].data()));
+      if (p.print_prs) {                                         // whole-genome PRS next to the LOCO files (src/Data.cpp:1906-1922)
+        prs_d[d].resize((size_t)P * N);
+        rg_check(rg_prs(hs[d], prs_d[d].data()));
+      }
+    });
+    // device 0 owns phenotypes 0, G, 2G, ...: its arrays are the result once the others' phenotypes are copied in
+    cs = std::move(cs_d[0]); best = std::move(best_d[0]); loco = std::move(loco_d[0]); prs = std::move(prs_d[0]);
     for (int ph_i = 0; ph_i < P; ++ph_i) {
       const int d = ph_i % G;
+      if (d == 0) continue;
       best[ph_i] = best_d[d][ph_i];
       for (int k = 0; k < nsum; ++k)
         for (int j = 0; j < p.l1; ++j) cs[((size_t)k * P + ph_i) * p.l1 + j] = cs_d[d][((size_t)k * P + ph_i) * p.l1 + j];
-      std::copy(loco_d[d].begin() + (size_t)ph_i * 23 * N, loco_d[d].begin() + (size_t)(ph_i + 1) * 23 * N,
-                loco.begin() + (size_t)ph_i * 23 * N);
+      auto copy_rows = [&](const std::vector<double>& src, std::vector<double>& dst, size_t n) {
+        std::copy(src.begin() + ph_i * n, src.begin() + (ph_i + 1) * n, dst.begin() + ph_i * n);
+      };
+      copy_rows(loco_d[d], loco, (size_t)23 * N);
+      if (p.print_prs) copy_rows(prs_d[d], prs, (size_t)N);
     }
+    phase("loco assembled");
   }
 
   // ---- output (Data::output src/Data.cpp:956-1120, write_predictions :1795-1982)
-  log << "Output\n------\n";
-  std::ofstream plist(p.out + "_pred.list"), prs_list;
-  if (!plist) throw Fail("cannot write to file : " + p.out + "_pred.list");
-  std::vector<double> prs;
-  if (p.print_prs) {                                         // whole-genome PRS next to the LOCO files (src/Data.cpp:1906-1922)
-    prs_list.open(p.out + "_prs.list");
-    if (!prs_list) throw Fail("cannot write to file : " + p.out + "_prs.list");
-    prs.resize((size_t)P * N);
-    if (G == 1) {
-      rg_check(rg_prs(h, prs.data()));
-    } else {
-      std::vector<double> tmp((size_t)P * N);
-      for (int d = 0; d < G; ++d) {
-        rg_check(rg_prs(hs[d], tmp.data()));
-        for (int ph_i = d; ph_i < P; ph_i += G) std::copy(tmp.begin() + (size_t)ph_i * N, tmp.begin() + (size_t)(ph_i + 1) * N, prs.begin() + (size_t)ph_i * N);
-      }
-    }
-  }
-  const std::string gz_ext = p.gz ? ".gz" : "";
-  std::vector<uint32_t> order;             // std::map key order of FID_IID, analysed samples only
-  for (auto& kv : g.key_to_ind) if (ph.in_analysis[kv.second]) order.push_back(kv.second);
-  std::vector<int> chr_labels(23);
-  for (int c = 0; c < 23; ++c) chr_labels[c] = c + 1;
-  phase("loco assembled");
-  for (int ph_i = 0; ph_i < P; ++ph_i) {
-    if (!l1_sel[ph_i]) continue;
-    log << "phenotype " << ph_i + 1 << " (" << ph.names[ph_i] << ") : \n";
-    auto CS = [&](int k, int j) { return cs[((size_t)k * P + ph_i) * p.l1 + j]; };
-    const double ne = ph.neff[ph_i];
-    for (int j = 0; j < p.l1; ++j) {
-      double num = CS(4, j) - CS(0, j) * CS(1, j) / ne;
-      const double rsq = num * num / ((CS(2, j) - CS(0, j) * CS(0, j) / ne) * (CS(3, j) - CS(1, j) * CS(1, j) / ne));
-      const double sse = CS(2, j) + CS(3, j) - 2 * CS(4, j);
-      std::ostringstream l;
-      const double tj = tau[(size_t)ph_i * p.l1 + j];
-      l << "  " << std::setw(5) << (p.bt ? B / (B + (M_PI * M_PI / 3.0) * tj) : B / (B + tj)) << " : Rsq = " << rsq
-        << ", MSE = " << sse / ne;
-      if (p.bt) l << ", -logLik/N = " << CS(5, j) / ne;
-      l << (j == best[ph_i] ? "<- min value" : "");
-      log << l.str() << "\n";
-    }
-    const uint8_t* mask_p = &ph.mask[(size_t)ph_i * N];
-    const std::string loco_file = p.out + "_" + std::to_string(ph_i + 1) + ".loco" + gz_ext;
-    {
-      TextWriter of;
-      of.open(loco_file);
-      const double* L = loco.data() + (size_t)ph_i * 23 * N;
-      std::vector<const double*> chr_rows(23);
-      for (int c = 0; c < 23; ++c) chr_rows[c] = L + (size_t)c * N;
-      write_pred_file(of, g.keys, order, mask_p, chr_labels, chr_rows);
-      of.close();
-    }
-    plist << ph.names[ph_i] << " " << full_path(loco_file, p.rel_path) << "\n";
-    log << "  * making predictions...writing LOCO predictions...";
+  void write_outputs() {
+    log << "Output\n------\n";
+    std::ofstream plist(p.out + "_pred.list"), prs_list;
+    if (!plist) throw Fail("cannot write to file : " + p.out + "_pred.list");
     if (p.print_prs) {
-      const std::string prs_file = p.out + "_" + std::to_string(ph_i + 1) + ".prs" + gz_ext;
-      TextWriter of;
-      of.open(prs_file);
-      write_pred_file(of, g.keys, order, mask_p, {0}, {prs.data() + (size_t)ph_i * N});
-      of.close();
-      prs_list << ph.names[ph_i] << " " << full_path(prs_file, p.rel_path) << "\n";
-      log << "writing whole genome PRS...";
+      prs_list.open(p.out + "_prs.list");
+      if (!prs_list) throw Fail("cannot write to file : " + p.out + "_prs.list");
     }
-    log << "done\n\n";
-  }
-  if (p.write_null_firth && p.bt) {
-    // null approximate-Firth estimates per chromosome, warm-started along the chromosomes (src/Data.cpp:1873-1903); they are
-    // starting values for Step 2 (--use-null-firth), not results
-    std::ofstream flist(p.out + "_firth.list");
-    if (!flist) throw Fail("cannot write to file : " + p.out + "_firth.list");
+    const std::string gz_ext = p.gz ? ".gz" : "";
+    std::vector<uint32_t> order;             // std::map key order of FID_IID, analysed samples only
+    for (auto& kv : in.ss.key_to_ind) if (ph.in_analysis[kv.second]) order.push_back(kv.second);
+    std::vector<int> chr_labels(23);
+    for (int c = 0; c < 23; ++c) chr_labels[c] = c + 1;
     for (int ph_i = 0; ph_i < P; ++ph_i) {
       if (!l1_sel[ph_i]) continue;
-      const std::string ffile = p.out + "_" + std::to_string(ph_i + 1) + ".firth" + gz_ext;
-      std::vector<double> bhat = null_logistic_beta(ph.names[ph_i], &ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C,
-                                                    &ph.mask[(size_t)ph_i * N]);
-      std::string text;
-      bool ok = true;
-      char num[40];
-      for (int c = 0; c < 23 && ok; ++c) {
-        ok = fit_null_firth(&ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C, loco.data() + ((size_t)ph_i * 23 + c) * N,
-                            &ph.mask[(size_t)ph_i * N], bhat);
-        text += std::to_string(c + 1);
-        for (double v : bhat) text.append(num, (size_t)snprintf(num, sizeof(num), " %g", v));
-        text += '\n';
+      log << "phenotype " << ph_i + 1 << " (" << ph.names[ph_i] << ") : \n";
+      auto CS = [&](int k, int j) { return cs[((size_t)k * P + ph_i) * p.l1 + j]; };
+      const double ne = ph.neff[ph_i];
+      for (int j = 0; j < p.l1; ++j) {
+        double num = CS(4, j) - CS(0, j) * CS(1, j) / ne;
+        const double rsq = num * num / ((CS(2, j) - CS(0, j) * CS(0, j) / ne) * (CS(3, j) - CS(1, j) * CS(1, j) / ne));
+        const double sse = CS(2, j) + CS(3, j) - 2 * CS(4, j);
+        std::ostringstream l;
+        const double tj = tau[(size_t)ph_i * p.l1 + j];
+        l << "  " << std::setw(5) << (p.bt ? B / (B + (M_PI * M_PI / 3.0) * tj) : B / (B + tj)) << " : Rsq = " << rsq
+          << ", MSE = " << sse / ne;
+        if (p.bt) l << ", -logLik/N = " << CS(5, j) / ne;
+        l << (j == best[ph_i] ? "<- min value" : "");
+        log << l.str() << "\n";
       }
-      if (!ok) { log << "WARNING: Firth failed to converge for phenotype '" << ph.names[ph_i] << "'\n"; continue; }
-      TextWriter of;
-      of.open(ffile);
-      of << text;
-      of.close();
-      flist << ph.names[ph_i] << " " << full_path(ffile, p.rel_path) << "\n";
+      const uint8_t* mask_p = &ph.mask[(size_t)ph_i * N];
+      const std::string loco_file = p.out + "_" + std::to_string(ph_i + 1) + ".loco" + gz_ext;
+      {
+        TextWriter of;
+        of.open(loco_file);
+        const double* L = loco.data() + (size_t)ph_i * 23 * N;
+        std::vector<const double*> chr_rows(23);
+        for (int c = 0; c < 23; ++c) chr_rows[c] = L + (size_t)c * N;
+        write_pred_file(of, in.ss.keys, order, mask_p, chr_labels, chr_rows);
+        of.close();
+      }
+      plist << ph.names[ph_i] << " " << full_path(loco_file, p.rel_path) << "\n";
+      log << "  * making predictions...writing LOCO predictions...";
+      if (p.print_prs) {
+        const std::string prs_file = p.out + "_" + std::to_string(ph_i + 1) + ".prs" + gz_ext;
+        TextWriter of;
+        of.open(prs_file);
+        write_pred_file(of, in.ss.keys, order, mask_p, {0}, {prs.data() + (size_t)ph_i * N});
+        of.close();
+        prs_list << ph.names[ph_i] << " " << full_path(prs_file, p.rel_path) << "\n";
+        log << "writing whole genome PRS...";
+      }
+      log << "done\n\n";
     }
-    flist.close();
-    log << "List of files with null Firth estimates written to: [" << p.out << "_firth.list]\n";
-  }
-  plist.close();
-  phase("prediction files");
-  if (p.run_l1 && !p.keep_l0)                        // rm_l0_files (src/Data.cpp:1131-1147)
-    for (const auto& mj : master.jobs) {
-      for (int ph_i = 0; ph_i < P; ++ph_i) remove((mj.prefix + "_l0_Y" + std::to_string(ph_i + 1)).c_str());
-      remove((mj.prefix + ".snplist").c_str());
+    if (p.write_null_firth && p.bt) {
+      // null approximate-Firth estimates per chromosome, warm-started along the chromosomes (src/Data.cpp:1873-1903); they are
+      // starting values for Step 2 (--use-null-firth), not results
+      std::ofstream flist(p.out + "_firth.list");
+      if (!flist) throw Fail("cannot write to file : " + p.out + "_firth.list");
+      for (int ph_i = 0; ph_i < P; ++ph_i) {
+        if (!l1_sel[ph_i]) continue;
+        const std::string ffile = p.out + "_" + std::to_string(ph_i + 1) + ".firth" + gz_ext;
+        std::vector<double> bhat = null_logistic_beta(ph.names[ph_i], &ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C,
+                                                      &ph.mask[(size_t)ph_i * N]);
+        std::string text;
+        bool ok = true;
+        char num[40];
+        for (int c = 0; c < 23 && ok; ++c) {
+          ok = fit_null_firth(&ph.Y_raw[(size_t)ph_i * N], ph.X.data(), N, ph.C, loco.data() + ((size_t)ph_i * 23 + c) * N,
+                              &ph.mask[(size_t)ph_i * N], bhat);
+          text += std::to_string(c + 1);
+          for (double v : bhat) text.append(num, (size_t)snprintf(num, sizeof(num), " %g", v));
+          text += '\n';
+        }
+        if (!ok) { log << "WARNING: Firth failed to converge for phenotype '" << ph.names[ph_i] << "'\n"; continue; }
+        TextWriter of;
+        of.open(ffile);
+        of << text;
+        of.close();
+        flist << ph.names[ph_i] << " " << full_path(ffile, p.rel_path) << "\n";
+      }
+      flist.close();
+      log << "List of files with null Firth estimates written to: [" << p.out << "_firth.list]\n";
     }
-  log << "List of blup files written to: [" << p.out << "_pred.list]\n";
-  if (p.print_prs) {
-    prs_list.close();
-    log << "List of files with whole genome PRS written to: [" << p.out << "_prs.list]\n";
+    plist.close();
+    phase("prediction files");
+    if (p.run_l1 && !p.keep_l0)                        // rm_l0_files (src/Data.cpp:1131-1147)
+      for (const auto& mj : master.jobs) {
+        for (int ph_i = 0; ph_i < P; ++ph_i) remove((mj.prefix + "_l0_Y" + std::to_string(ph_i + 1)).c_str());
+        remove((mj.prefix + ".snplist").c_str());
+      }
+    log << "List of blup files written to: [" << p.out << "_pred.list]\n";
+    if (p.print_prs) {
+      prs_list.close();
+      log << "List of files with whole genome PRS written to: [" << p.out << "_prs.list]\n";
+    }
   }
+};
+
+void run_step1(const Params& p, Log& log) {
+  Step1 s(p, log);                 // the options and jobs of Step 1, then the genotype file
+  s.read_inputs();
+  if (!s.check_jobs()) return;
+  s.create_handles();
+  s.level0();
+  if (!s.write_l0_files()) return;
+  s.level1();
+  s.write_outputs();
 }
 
 // ------------------------------------------------------------------------------------ step 2
@@ -1126,21 +1170,9 @@ struct BedTraitCounts {
   }
 };
 
-// --range (in_range, src/Geno.cpp:2790-2800): keep the variants of one chromosome window
-void apply_range(const Params& p, std::vector<Snp>& snps) {
-  if (!p.set_range) return;
-  snps.erase(std::remove_if(snps.begin(), snps.end(), [&](const Snp& s) {
-               return s.chrom != p.range_chr || (double)s.pos < p.range_min || (double)s.pos > p.range_max;
-             }), snps.end());
-}
-
 // phenotypes + covariates + LOCO files for Step 2 (read_pheno_and_cov, blup_read, prep_run)
-void load_step2_inputs(const Params& p, const SampleSet& g, const std::vector<std::pair<std::string, std::string>>& ids_file,
-                       const std::vector<int32_t>& sample_idx, Conditioning& cond, Pheno& ph, std::vector<Loco>& locos, Log& log) {
-  ph.pheno_cols = p.pheno_cols; ph.covar_cols = p.covar_cols; ph.rint = p.rint && !p.bt; ph.cat_cols = p.cat_cols; ph.max_cat_levels = p.max_cat_levels;
-  ph.pheno_excl = p.pheno_excl; ph.covar_excl = p.covar_excl; ph.min_case_count = p.min_case_count;
-  read_pheno_and_cov(g, p.pheno, p.covar, true, p.strict, p.bt, ph, log);
-  if (cond.on()) cond.append(g, ph, log);
+void load_step2_inputs(const Params& p, GenoInput& in, Pheno& ph, std::vector<Loco>& locos, Log& log) {
+  read_pheno(p, in, true, ph, log);
   const int64_t N = ph.N;
   const int P = ph.P;
   // write_ids (src/Pheno.cpp:1538-1576) runs right after blup_read, before setMasks: the samples with a phenotype
@@ -1149,7 +1181,7 @@ void load_step2_inputs(const Params& p, const SampleSet& g, const std::vector<st
     if (!p.write_samples) return;
     log << " * user specified to write sample IDs for each trait\n";
     std::vector<std::pair<std::string, std::string>> kept(N);
-    for (int64_t s = 0; s < N; ++s) kept[s] = ids_file.at((size_t)sample_idx[s]);
+    for (int64_t s = 0; s < N; ++s) kept[s] = in.ids_file.at((size_t)in.sample_idx[s]);
     std::vector<uint8_t> m(N);
     for (int i = 0; i < P; ++i) {
       for (int64_t s = 0; s < N; ++s) m[s] = ph.mask[(size_t)i * N + s] && (!extra || (*extra)[(size_t)i * N + s]);
@@ -1174,8 +1206,8 @@ void load_step2_inputs(const Params& p, const SampleSet& g, const std::vector<st
     log << "   -file [" << it->second << "] for phenotype '" << ph.names[i] << "'\n";
     const auto& first = locos[i].first;                      // blup_read checks the first data row
     for (size_t c = 0; c < locos[i].ids.size(); ++c) {
-      auto k = g.key_to_ind.find(locos[i].ids[c]);
-      if (k == g.key_to_ind.end() || first.empty()) continue;
+      auto k = in.ss.key_to_ind.find(locos[i].ids[c]);
+      if (k == in.ss.key_to_ind.end() || first.empty()) continue;
       extra[(size_t)i * N + k->second] = !std::isnan(first[c]);
     }
   }
@@ -1221,33 +1253,22 @@ std::vector<uint8_t> male_vector(const std::vector<int>& sex_file, const std::ve
   return m;
 }
 
-// The Step-2 input of either trait kind: the genotype file (BGEN, or .bed / .pgen rows) after --range, the samples,
-// phenotypes, covariates and LOCO predictions, the blocks, and their prefetch.  Blocks are fetched (file read / threaded
-// BGEN inflate) one block ahead of the GPU call into two slots, block b in slot b & 1: the rg_s2_block_* calls return
-// with the results on the host, so the slot of block b is free again when block b + 2 is fetched.  The fetch thread also
-// derives from each block what its rows print:
+// The Step-2 input of either trait kind: the genotype file (GenoInput), the phenotypes, covariates and LOCO predictions,
+// the blocks, and their prefetch.  Blocks are fetched (file read / threaded BGEN inflate) one block ahead of the GPU call
+// into two slots, block b in slot b & 1: the rg_s2_block_* calls return with the results on the host, so the slot of
+// block b is free again when block b + 2 is fetched.  The fetch thread also derives from each block what its rows print:
 // - the INFO over all analysed samples (--minINFO drops a variant whose INFO is too low, src/Geno.cpp:2074) and the
 //   dosage genotype counts of --no-split, from the inflated bytes;
 // - the --htp genotype counts per trait (update_genocounts, src/Geno.cpp:2986-3018): thresholded from the inflated bytes
 //   (BgenFile::trait_counts) or popcounts over the 2-bit rows (BedTraitCounts).  A binary trait counts its cases and
 //   controls apart, a quantitative trait all its samples as one class.
-struct S2Input {
-  const Params& p;
-  const bool binary, use_bgen;
-  BedFile g;
-  BgenFile gg;
-  const std::vector<Snp>& snps;
-  const std::vector<int32_t>& sample_idx;
-  const SampleSet ss;
-  size_t n_file = 0;
-  bool subset = false;                                       // the file holds samples that are not analysed
-  Conditioning cond;                                         // --condition-list
+struct S2Input : GenoInput {
+  const bool binary;
   Pheno ph;
   std::vector<Loco> locos;
   std::vector<Block> blocks;
   size_t b_first = 0;                                        // --starting-block
   std::vector<uint8_t> male;                                 // params.sex == 1 of the kept samples
-  int threads = 1;
   bool use_info1 = false, htp_bgen = false, dev_inflate = false, pgen_dev = false;
   std::vector<uint8_t> rows[2], probs[2], pmiss[2], comp[2];
   std::vector<uint64_t> comp_offs[2];
@@ -1258,32 +1279,11 @@ struct S2Input {
   BedTraitCounts btc;
   std::future<void> pending;
 
-  S2Input(const Params& p_, bool binary_, Log& log)
-      : p(p_), binary(binary_), use_bgen(!p_.bgen.empty()), snps(use_bgen ? gg.snps : g.snps),
-        sample_idx(use_bgen ? gg.sample_idx : g.sample_idx),
-        ss{use_bgen ? gg.keys : g.keys, use_bgen ? gg.key_to_ind : g.key_to_ind} {
-    const auto extr = read_id_list(p.extract, 1), rem = read_id_list(p.remove, 2), keep = read_id_list(p.keep, 2);
-    std::set<std::string> excl = read_id_list(p.exclude, 1);
-    init_conditioning(p, cond, excl, log);
-    if (use_bgen) {
-      gg.sex_specific = p.sex_specific;
-      gg.open(p.bgen, p.sample, p.ref_first, excl, extr, rem, keep, p.chrs, p.bgi);
-      if (gg.used_bgi) log << "   -index bgi file [" << (p.bgi.empty() ? p.bgen + ".bgi" : p.bgi) << "]\n";
-      log << " * bgen                : [" << p.bgen << "] n_snps = " << gg.snps.size() << ", n_samples = " << gg.keys.size() << "\n";
-    } else {
-      open_rows(p, g, excl, extr, rem, keep, log);
-    }
-    apply_range(p, gg.snps);
-    apply_range(p, g.snps);
-    if (g.pg) apply_range(p, g.pg->snps);
-    if (p.set_range && snps.empty()) throw Fail("no variant left to include in analysis.");
-    locate_conditioning(p, cond);
-    n_file = use_bgen ? gg.n_file : g.keys_file.size();
-    subset = ss.keys.size() != n_file;
-    load_step2_inputs(p, ss, use_bgen ? gg.ids_file : g.ids_file, sample_idx, cond, ph, locos, log);
+  S2Input(const Params& p_, bool binary_, Log& log) : GenoInput(p_, log), binary(binary_) {
+    load_step2_inputs(p, *this, ph, locos, log);
     blocks = set_blocks(snps, p.bsize);
     log << " * # blocks            : [" << blocks.size() << "]\n";
-    male = male_vector(use_bgen ? gg.sex_file : g.sex_file, sample_idx);
+    male = male_vector(sex_file, sample_idx);
   }
 
   // a Step-2 handle over the analysed samples with the per-trait sample masks `mask` [P][N]
@@ -1298,7 +1298,6 @@ struct S2Input {
   // buffers, the decode choices and the fetch of the first block; runs once the handles exist
   void start(Log& log) {
     const int bsz = p.bsize, P = ph.P;
-    threads = p.threads > 0 ? p.threads : (int)std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
     for (int k = 0; k < 2; ++k) {
       if (use_bgen) { probs[k].resize((size_t)bsz * n_file * 2); pmiss[k].resize((size_t)bsz * n_file); }
       else rows[k].resize((size_t)bsz * g.row_stride);

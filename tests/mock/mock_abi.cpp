@@ -11,8 +11,10 @@
 #include <zlib.h>
 
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -25,7 +27,8 @@ struct rg_ctx {
   int P = 0, C = 0, K = 0, R = 0, R1 = 0, nb = 0, bs_max = 0;
   std::vector<double> Y, res, scf;
   std::vector<uint8_t> mask, in_analysis, l1_sel, male, nonpar;
-  std::map<std::pair<int, int>, std::vector<double>> W;        // (block, pheno) -> N x R slab
+  std::map<std::pair<int, int>, std::vector<double>> W;        // (block, pheno) -> N x R slab of the phenotypes owned here
+  std::vector<rg_ctx*> W_owner;                                // per pheno: the handle whose W holds it (rg_W_attach_local)
   std::vector<double> prs;
   std::vector<double> last_stat;                               // [bs x P] of the last block (Firth / SPA)
   std::vector<uint8_t> inflate_probs, inflate_miss;
@@ -36,7 +39,8 @@ struct rg_ctx {
 };
 
 namespace {
-std::string g_err;
+thread_local std::string g_err;                               // one driver thread per device: errors stay with their thread
+std::mutex g_W_mu;                                            // level-0 slabs of a phenotype land in its owner's W
 int fail(const std::string& m) { g_err = m; return 1; }
 
 // PLINK 1 code -> ALT-allele count as the driver's kernels see it (ref-last): 00 -> 2, 01 -> missing, 10 -> 1, 11 -> 0
@@ -111,7 +115,10 @@ extern "C" {
 
 const char* rg_last_error(void) { return g_err.c_str(); }
 const char* rg_version(void) { return "mock ABI for host-plumbing tests"; }
-int rg_device_count(void) { return 1; }
+int rg_device_count(void) {
+  const char* e = getenv("RG_MOCK_DEVICES");
+  return e ? atoi(e) : 1;
+}
 int rg_warmup(int32_t) { return 0; }
 int rg_l0_wait_input(rg_handle) { return 0; }
 void rg_destroy(rg_handle h) { delete h; }
@@ -127,26 +134,33 @@ int rg_step1_create(const rg_step1_config* cfg, const double*, const double* Y, 
   h->mask.assign(mask, mask + (size_t)h->N * h->P);
   h->in_analysis.assign(in_analysis, in_analysis + h->N);
   h->l1_sel.assign(h->P, 1);
+  h->W_owner.assign(h->P, h);
   *out = h;
   return 0;
+}
+
+// the slab of (block, pheno): column r, sample s = mean genotype-weighted phenotype, a function of every input byte; it is
+// stored in the W of the phenotype's owner, like the library's peer stores
+static void store_W(rg_handle h, int block_id, int bs, const std::vector<double>& colsum) {
+  for (int p = 0; p < h->P; ++p) {
+    std::vector<double> w((size_t)h->N * h->R, 0.0);
+    for (int r = 0; r < h->R; ++r)
+      for (int64_t s = 0; s < h->N; ++s)
+        w[(size_t)r * h->N + s] = h->mask[(size_t)p * h->N + s] ? (colsum[s] / bs - 1.0) * (r + 1) * 0.1 + 0.01 * h->Y[(size_t)p * h->N + s] : 0.0;
+    std::lock_guard<std::mutex> lk(g_W_mu);
+    h->W_owner[p]->W[{block_id, p}] = std::move(w);
+  }
 }
 
 int rg_l0_block_bed(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
                     int32_t block_id) {
   if (block_id < 0 || block_id >= h->nb || bs > h->bs_max) return fail("mock: bad block");
-  // the slab of (block, pheno): column r, sample s = mean genotype-weighted phenotype, a function of every input byte
   std::vector<double> colsum(h->N, 0.0);
   for (int v = 0; v < bs; ++v) {
     const Geno x = from_bed(h, packed + (size_t)v * row_stride, sample_idx, ref_first);
     for (int64_t s = 0; s < h->N; ++s) colsum[s] += (x.g[s] + 0.25 * x.miss[s]) * (1.0 + 0.001 * (v % 17));
   }
-  for (int p = 0; p < h->P; ++p) {
-    std::vector<double>& w = h->W[{block_id, p}];
-    w.assign((size_t)h->N * h->R, 0.0);
-    for (int r = 0; r < h->R; ++r)
-      for (int64_t s = 0; s < h->N; ++s)
-        w[(size_t)r * h->N + s] = h->mask[(size_t)p * h->N + s] ? (colsum[s] / bs - 1.0) * (r + 1) * 0.1 + 0.01 * h->Y[(size_t)p * h->N + s] : 0.0;
-  }
+  store_W(h, block_id, bs, colsum);
   return 0;
 }
 int rg_l0_block_dosage_u8(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
@@ -162,13 +176,7 @@ int rg_l0_block_dosage_u8(rg_handle h, const uint8_t* probs, const uint8_t* pm, 
       const double g = miss ? 0.25 : (ref_first ? 2.0 - (2.0 * pr[0] + pr[1]) / 255.0 : (2.0 * pr[0] + pr[1]) / 255.0);
       colsum[s] += g * (1.0 + 0.001 * (v % 17));
     }
-  for (int p = 0; p < h->P; ++p) {
-    std::vector<double>& w = h->W[{block_id, p}];
-    w.assign((size_t)h->N * h->R, 0.0);
-    for (int r = 0; r < h->R; ++r)
-      for (int64_t s = 0; s < h->N; ++s)
-        w[(size_t)r * h->N + s] = h->mask[(size_t)p * h->N + s] ? (colsum[s] / bs - 1.0) * (r + 1) * 0.1 + 0.01 * h->Y[(size_t)p * h->N + s] : 0.0;
-  }
+  store_W(h, block_id, bs, colsum);
   return 0;
 }
 int64_t rg_l0_status(rg_handle) { return 0; }
@@ -183,10 +191,18 @@ int rg_l0_load_W(rg_handle h, int32_t b, int32_t ph, const double* in) {
   h->W[{b, ph}].assign(in, in + (size_t)h->N * h->R);
   return 0;
 }
-// multi-GPU plumbing: the mock keeps one W map per handle, so "attaching" a peer shares nothing - the driver's
-// --gpus path is exercised on hardware only (tests/test_multigpu_gpu.py)
-int rg_W_set_owned(rg_handle, const uint8_t*) { return fail("mock: --gpus is not modelled"); }
-int rg_W_attach_local(rg_handle, rg_handle, const uint8_t*) { return fail("mock: --gpus is not modelled"); }
+// --gpus N (RG_MOCK_DEVICES handles): level 1 runs on the owned phenotypes (rg_api.cu rg_W_set_owned), and the level-0
+// slabs of a phenotype owned by a peer go to the peer's W map
+int rg_W_set_owned(rg_handle h, const uint8_t* owned) {
+  if (!h || !owned || !h->W.empty()) return fail("mock: rg_W_set_owned must come before the first block");
+  for (int p = 0; p < h->P; ++p) h->l1_sel[p] = owned[p] ? 1 : 0;
+  return 0;
+}
+int rg_W_attach_local(rg_handle h, rg_handle peer, const uint8_t* owned_by_peer) {
+  if (!h || !peer || peer == h || !owned_by_peer) return fail("mock: bad rg_W_attach_local arguments");
+  for (int p = 0; p < h->P; ++p) if (owned_by_peer[p]) h->W_owner[p] = peer;
+  return 0;
+}
 int rg_l1_select(rg_handle h, const uint8_t* sel) { h->l1_sel.assign(sel, sel + h->P); return 0; }
 
 static int l1_common(rg_handle h, const double* tau, double* cs, int32_t* best, int nsums) {

@@ -339,25 +339,79 @@ def test_no_split_output_on_dosages(tmp_path, golden_dir):
     helpers.check_no_split_bgen(run, read, tmp_path, golden_dir)
 
 
-def test_sex_specific_and_starting_block(tmp_path, golden_dir):
-    """--sex-specific keeps one sex like --keep would (src/Geno.cpp:1287-1293); --starting-block resumes a Step-2 run at a
-    block (src/Data.cpp:2168, :2275): its rows are the tail of the full run."""
+GENO = {"bed": lambda d: ["--bed", d + "/example_3chr"], "pgen": lambda d: ["--pgen", d + "/example"],
+        "bgen": lambda d: ["--bgen", d + "/example_3chr.bgen", "--sample", d + "/example_3chr.sample"]}
+
+
+@pytest.mark.parametrize("geno,extra", [(g, t + c) for g in GENO for t in ([], ["--bt"]) for c in ([], ["--loocv"])] +
+                         [("bed", ["--print-prs", "--lowmem", "--keep-l0"])])
+def test_step1_gpus_n_writes_the_single_gpu_files(tmp_path, golden_dir, monkeypatch, geno, extra):
+    """--gpus N: each device feeds its range of level-0 blocks and fits the phenotypes it owns.  The mock stores every
+    slab in the W of the phenotype's owner like the library's peer stores, so the files must be those of one device
+    (on GPUs: tests/test_multigpu_gpu.py)."""
     d = golden_dir
-    # the fixtures carry no sex information: write a .fam with alternating sexes
-    for ext in (".bed", ".bim"):
-        shutil.copy(d + "/example_3chr" + ext, tmp_path / ("sx" + ext))
+    monkeypatch.setenv("RG_MOCK_DEVICES", "3")
+    pheno = d + ("/phenotype_bin.txt" if "--bt" in extra else "/phenotype.txt")
+    files = {}
+    for g in (1, 2, 3):
+        o = str(tmp_path / ("g%d" % g))
+        log = run(["--step", "1"] + GENO[geno](d) + ["--phenoFile", pheno, "--covarFile", d + "/covariates.txt", "--bsize", "100",
+                                                      "--gpus", g] + extra + ["--out", o])
+        assert ("(gpu 2)" in log) == (g == 3)
+        out = sorted(f for f in glob.glob(o + "_*") if not f.endswith(".list"))
+        files[g] = {os.path.basename(f)[2:]: open(f, "rb").read() for f in out}
+        files[g]["pred.list"] = [l.split()[0] for l in open(o + "_pred.list")]
+    assert len(files[1]) == (7 if "--print-prs" in extra else 3)         # .loco (+ .prs, _l0_Y) per phenotype, pred.list
+    assert files[2] == files[1] and files[3] == files[1]
+
+
+def sexed_copies(t, d):
+    """The fixtures carry no sex information: copies of the .bed, .pgen and .bgen filesets with alternating sexes (male
+    first), each with the genotype arguments that select it and a --keep file of its males."""
     fam = [l.split() for l in open(d + "/example_3chr.fam")]
-    with open(tmp_path / "sx.fam", "w") as fh:
-        for k, t in enumerate(fam):
-            t[4] = "1" if k % 2 == 0 else "2"
-            fh.write(" ".join(t) + "\n")
-    with open(tmp_path / "males.txt", "w") as fh:
-        fh.write("".join("%s %s\n" % (t[0], t[1]) for k, t in enumerate(fam) if k % 2 == 0))
-    base = ["--step", "2", "--bed", tmp_path / "sx", "--phenoFile", d + "/phenotype.txt", "--covarFile", d + "/covariates.txt", "--bsize", "100",
-            "--ignore-pred"]
-    log = run(base + ["--sex-specific", "male", "--out", str(tmp_path / "m1")])
-    run(base + ["--keep", tmp_path / "males.txt", "--out", str(tmp_path / "m2")])
-    assert "-keeping only male individuals in the analysis" in log
+    for ext in (".bed", ".bim"):
+        shutil.copy(d + "/example_3chr" + ext, t / ("sx" + ext))
+    with open(t / "sx.fam", "w") as fh:
+        fh.write("".join(" ".join(r[:4] + ["1" if k % 2 == 0 else "2"] + r[5:]) + "\n" for k, r in enumerate(fam)))
+    for ext in (".pgen", ".pvar"):
+        shutil.copy(d + "/example" + ext, t / ("sxp" + ext))
+    psam = [l.split() for l in open(d + "/example.psam")]
+    with open(t / "sxp.psam", "w") as fh:
+        fh.write("\t".join(psam[0]) + "\n" + "".join("\t".join([r[0], r[1], "1" if k % 2 == 0 else "2"] + r[3:]) + "\n"
+                                                  for k, r in enumerate(psam[1:])))
+    shutil.copy(d + "/example_3chr.bgen", t / "sxg.bgen")
+    sample = [l.split() for l in open(d + "/example_3chr.sample")]
+    with open(t / "sxg.sample", "w") as fh:
+        fh.write("".join(" ".join(r) + "\n" for r in sample[:2]) +
+                 "".join(" ".join(r[:3] + ["1" if k % 2 == 0 else "2"] + r[4:]) + "\n" for k, r in enumerate(sample[2:])))
+    out = {}
+    for fmt, args, ids in (("bed", ["--bed", t / "sx"], fam), ("pgen", ["--pgen", t / "sxp"], psam[1:]),
+                           ("bgen", ["--bgen", t / "sxg.bgen", "--sample", t / "sxg.sample"], sample[2:])):
+        keep = t / ("males_%s.txt" % fmt)
+        keep.write_text("".join("%s %s\n" % (r[0], r[1]) for r in ids[::2]))
+        out[fmt] = (args, keep)
+    return out
+
+
+def test_sex_specific_and_starting_block(tmp_path, golden_dir):
+    """--sex-specific keeps one sex like --keep would (src/Geno.cpp:1286-1293), in both steps and on every genotype format;
+    --starting-block resumes a Step-2 run at a block (src/Data.cpp:2168, :2275): its rows are the tail of the full run."""
+    d = golden_dir
+    covs = ["--phenoFile", d + "/phenotype.txt", "--covarFile", d + "/covariates.txt", "--bsize", "100"]
+    for fmt, (geno, males) in sexed_copies(tmp_path, d).items():
+        s1 = ["--step", "1"] + geno + covs
+        log = run(s1 + ["--sex-specific", "male", "--out", str(tmp_path / ("s1m_" + fmt))])
+        run(s1 + ["--keep", males, "--out", str(tmp_path / ("s1k_" + fmt))])
+        assert "-keeping only male individuals in the analysis" in log, fmt
+        loco = read(str(tmp_path / ("s1m_" + fmt)) + "_1.loco")
+        assert loco == read(str(tmp_path / ("s1k_" + fmt)) + "_1.loco") and len(loco.splitlines()[0].split()) == 251, fmt
+        log = run(["--step", "2"] + geno + covs + ["--ignore-pred", "--sex-specific", "male", "--out", str(tmp_path / ("s2m_" + fmt))])
+        assert "-keeping only male individuals in the analysis" in log, fmt
+        rows = [l.split() for l in read(str(tmp_path / ("s2m_" + fmt)) + "_Y1.regenie").splitlines()]
+        assert {r[rows[0].index("N")] for r in rows[1:]} == {"250"}, fmt
+    base = ["--step", "2", "--bed", tmp_path / "sx"] + covs + ["--ignore-pred"]
+    run(base + ["--sex-specific", "male", "--out", str(tmp_path / "m1")])
+    run(base + ["--keep", tmp_path / "males_bed.txt", "--out", str(tmp_path / "m2")])
     m1 = read(str(tmp_path / "m1") + "_Y1.regenie")
     assert m1 == read(str(tmp_path / "m2") + "_Y1.regenie") and {l.split()[6] for l in m1.splitlines()[1:]} == {"250"}
     run(base + ["--out", str(tmp_path / "full")])
