@@ -64,8 +64,9 @@ struct rg_ctx {
     rg::DevBuf<uint8_t> pgen_in;      // rg_pgen_decode: metadata blob + record bytes of the block this lane runs next
     rg::DevBuf<uint32_t> gp;          // [rows_p][Npad/16]
     rg::DevBuf<float> zz;             // [K][2 rows_p][2 rows_p]
-    // sparse Miss rows of zz (miss_gram.cu): missing-call total of the block (> miss_cap = dense tiles), list segments
-    // [K][rows_p] (offset, count), sample lists, the block as sample-major 2-bit rows [Npad][rows_p / 16]
+    // sparse Miss rows of zz (miss_gram.cu), written by the relayout: missing-call total of the block (> miss_cap =
+    // dense tiles), list segments [rows_p][miss_nct] (offset, count), sample lists, the block as sample-major 2-bit rows
+    // [Npad][rows_p / 16]
     rg::DevBuf<unsigned long long> miss_total;
     rg::DevBuf<int2> miss_seg;
     rg::DevBuf<int32_t> miss_list;
@@ -211,6 +212,11 @@ struct rg_ctx {
   //      (RG_B200_GRAM=dense)
   bool gram_dense = false;
   int64_t miss_cap = 0;
+  // column tiles of the relayout's missing lists (BedMissOut): (first word, words, fold) and each fold's tile range
+  int miss_nct = 0;
+  std::vector<int4> miss_ctile_host;
+  rg::DevBuf<int4> miss_ctile;
+  rg::DevBuf<int2> miss_fold_ct;
 
   // ---- level-0 solver selection (RG_B200_SOLVER = mixed | f64) and its counters
   int solver_mixed = 1;

@@ -13,10 +13,29 @@ constexpr int kLimbsI8 = 5;        // radix-254 int8 digits per coefficient of t
 constexpr int kLimbQI8 = 50;       // outputs per INT8 prediction pass (5 x 50 = 250 <= 256 digit rows)   // phenotypes per register pass of the LOOCV prediction kernel
 
 // ---- bed_kernels.cu
+// bit 2k set where the 2-bit code k of w is 3 (missing)
+__device__ __forceinline__ uint32_t miss_bits(uint32_t w) { return w & (w >> 1) & 0x55555555u; }
+// What the Step-1 relayout writes for the sparse Miss rows of the Gram (miss_gram.cu).  Column tile ct covers words
+// ctile[ct].x .. + ctile[ct].y - 1 (at most 32) of fold ctile[ct].z; fold f owns tiles fold_ct[f].x .. fold_ct[f].y - 1.
+struct BedMissOut {
+  const int4* ctile = nullptr;
+  int nct = 0;
+  int rows_p = 0;
+  unsigned long long* total = nullptr;   // missing calls of the block; > cap: the dense Miss tiles run
+  unsigned long long cap = 0;
+  int2* seg = nullptr;                   // [rows_p][nct] (offset, count) into list
+  int32_t* list = nullptr;               // missing samples, cap entries
+  uint32_t* gt = nullptr;                // [Npad][rows_p / 16] sample-major 2-bit rows
+};
+// PLINK rows -> padded 2-bit rows gp [rows_p][npad / 16] (rows_p a multiple of 128)
 void launch_bed_relayout(const uint8_t* packed, int64_t row_stride, int bs, int rows_p,
                          const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep, int ref_first,
                          uint32_t* gp, int64_t npad,
                          cudaStream_t s);
+// the same, and the missing lists and Gt of the sparse Miss rows from the same pass (zeroes *mo.total first)
+void launch_bed_relayout_miss(const uint8_t* packed, int64_t row_stride, int bs, int rows_p,
+                              const int32_t* file_idx_pad, const int32_t* word_base, const uint32_t* word_keep,
+                              int ref_first, uint32_t* gp, int64_t npad, const BedMissOut& mo, cudaStream_t s);
 
 // ---- l0_stats.cu
 struct SnpFinalizeArgs {
@@ -86,12 +105,10 @@ constexpr float kZScaleStat = 1.f / 8;    // Z [X|Y]-digit tiles: the digit rows
 // missing calls per block (as a fraction of bs_max x analysed samples) up to which the sparse sums run: the crossover
 // of tools/miss_rate_sweep.py (DESIGN.md section 3)
 constexpr double kMissSparseRate = 0.015;
-void launch_miss_list(const uint32_t* gp, int64_t npad, int rows_p, const int2* fold_k, int K, unsigned long long* total,
-                      int64_t cap, int2* seg, int32_t* list, cudaStream_t s);
-void launch_miss_transpose(const uint32_t* gp, int64_t npad, int rows_p, const unsigned long long* total, int64_t cap,
-                           uint32_t* gt, cudaStream_t s);
-void launch_miss_sparse(const uint32_t* gt, int rows_p, const int2* seg, const int32_t* list, int K,
-                        const unsigned long long* total, int64_t cap, float* zz, int64_t fold_stride, cudaStream_t s);
+// one warp per (SNP row, fold): the fold's column tiles of seg (launch_bed_relayout_miss) -> Miss rows of zz
+void launch_miss_sparse(const uint32_t* gt, int rows_p, const int2* seg, int nct, const int2* fold_ct,
+                        const int32_t* list, int K, const unsigned long long* total, int64_t cap, float* zz,
+                        int64_t fold_stride, cudaStream_t s);
 // CUDA-core reference of the Z Z^T Gram of samples k0 .. k1 - 1, from the 2-bit rows (integer sums, not x 64)
 void launch_gram_reference(const uint32_t* gp, int64_t npad, int rows_p, int k0, int k1, float* out, int ldo,
                            cudaStream_t s);

@@ -217,6 +217,23 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
     h->gram_dense = mode == "dense";
     const double rate = mode == "sparse" ? 1.0 : kMissSparseRate;
     h->miss_cap = std::min<int64_t>((int64_t)(rate * h->bs_max * h->n_analyzed), INT32_MAX);
+    // the relayout's column tiles: 512 samples (32 words) each, cut at the fold ends so that a tile's calls belong to
+    // one fold
+    std::vector<int2> fold_ct(K);
+    h->miss_ctile_host.clear();
+    for (int f = 0; f < K; ++f) {
+      fold_ct[f].x = (int)h->miss_ctile_host.size();
+      const int64_t w1 = (h->fold_pad_start[f] + h->fold_pad_len[f]) / 16;
+      for (int64_t w = h->fold_pad_start[f] / 16; w < w1; w += 32)
+        h->miss_ctile_host.push_back(make_int4((int)w, (int)std::min<int64_t>(32, w1 - w), f, 0));
+      fold_ct[f].y = (int)h->miss_ctile_host.size();
+    }
+    h->miss_nct = (int)h->miss_ctile_host.size();
+    h->miss_ctile.alloc(h->miss_nct);
+    h->miss_fold_ct.alloc(K);
+    RG_CUDA(cudaMemcpyAsync(h->miss_ctile.p, h->miss_ctile_host.data(), h->miss_nct * sizeof(int4),
+                            cudaMemcpyHostToDevice, s));
+    RG_CUDA(cudaMemcpyAsync(h->miss_fold_ct.p, fold_ct.data(), K * sizeof(int2), cudaMemcpyHostToDevice, s));
   }
   RG_CUDA(cudaStreamSynchronize(s));   // host vectors go out of scope
 }
@@ -592,10 +609,26 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   L.part.alloc((size_t)d.ntiles_s * Qp * 2);
   L.mean_invsd.alloc((size_t)2 * Qp);
 
-  // --- 1. decode: PLINK rows -> padded 2-bit rows (the tensor-core tiles build their int8 operands from them)
+  // --- 1. decode: PLINK rows -> padded 2-bit rows (the tensor-core tiles build their int8 operands from them); on the
+  //        sparse Miss path the same pass writes the missing lists and the sample-major rows Gt (miss_gram.cu)
   {
     ScopedTimer t(h, "bed_relayout", s);
-    launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, L.gp.p, Npad, s);
+    if (h->gram_dense) {
+      launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p,
+                          ref_first, L.gp.p, Npad, s);
+    } else {
+      L.miss_total.alloc(1);
+      L.miss_seg.alloc((size_t)h->rows_p_max * h->miss_nct);
+      L.miss_list.alloc((size_t)std::max<int64_t>(h->miss_cap, 1));
+      L.gt.alloc((size_t)Npad * (h->rows_p_max / 16));
+      BedMissOut mo;
+      mo.ctile = h->miss_ctile.p; mo.nct = h->miss_nct; mo.rows_p = rows_p;
+      mo.total = L.miss_total.p; mo.cap = (unsigned long long)h->miss_cap;
+      mo.seg = L.miss_seg.p; mo.list = L.miss_list.p; mo.gt = L.gt.p;
+      launch_bed_relayout_miss(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p,
+                               ref_first, L.gp.p, Npad, mo, s);
+      h->launches += 1;                    // the memset of the total
+    }
     if (staged >= 0) {
       if (!L.relayout_done[staged]) RG_CUDA(cudaEventCreateWithFlags(&L.relayout_done[staged], cudaEventDisableTiming));
       RG_CUDA(cudaEventRecord(L.relayout_done[staged], s));
@@ -638,16 +671,11 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
       h->launches += 1;
     } else {
       // the Miss rows: the device picks the sparse sums or the dense tiles from the block's missing-call count
-      L.miss_total.alloc(1);
-      L.miss_seg.alloc((size_t)K * h->rows_p_max);
-      L.miss_list.alloc((size_t)std::max<int64_t>(h->miss_cap, 1));
-      L.gt.alloc((size_t)Npad * (h->rows_p_max / 16));
-      launch_miss_list(L.gp.p, Npad, rows_p, h->fold_k.p, K, L.miss_total.p, h->miss_cap, L.miss_seg.p, L.miss_list.p, s);
-      launch_miss_transpose(L.gp.p, Npad, rows_p, L.miss_total.p, h->miss_cap, L.gt.p, s);
       launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, tl.buf.p, tl.count, h->fold_k.p, K,
                      L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
-      launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, L.miss_list.p, K, L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
-      h->launches += 5;
+      launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, h->miss_nct, h->miss_fold_ct.p, L.miss_list.p, K,
+                         L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
+      h->launches += 2;
     }
     L.last_gram_dense = h->gram_dense;
   }
@@ -854,6 +882,14 @@ static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
       v[1] = (int64_t)tot;
     }
     return host_view(v, 3);
+  }
+  if (n == "miss_ctile") return host_view(h->miss_ctile_host.data(), h->miss_ctile_host.size());  // (word, words, fold, 0)
+  if (n == "miss_seg" || n == "miss_list") {
+    // the relayout's missing lists of the last block (sparse path only): seg [rows_p][miss_nct] (offset, count) into
+    // list; a view holds them once the block's total is within the capacity
+    RG_CHECK(!L.last_gram_dense && L.miss_seg.p, "no missing lists for the last block: " + n);
+    if (n == "miss_seg") return dev_view(L.miss_seg.p, (size_t)rp * h->miss_nct * sizeof(int2));
+    return dev_view(L.miss_list.p, (size_t)std::max<int64_t>(h->miss_cap, 1) * 4);
   }
   if (n == "pad_of") return host_view(h->pad_of.data(), h->N);
   if (n == "zz_ref") {

@@ -17,7 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 os.environ["RG_B200_LANES"] = "1"
 
-GRAM = ("miss_list", "miss_transpose", "gram_s8_wgmma", "miss_sparse", "Memset")
+GRAM = ("bed_relayout", "miss_list", "miss_transpose", "gram_s8_wgmma", "miss_sparse", "Memset")
 
 
 def main():
@@ -78,8 +78,9 @@ def main():
         print("%-28s %9.1f us" % ("all other kernels", other))
         st.set_timing(True)
         one_pass()
-        ms, n = st.timing("gram_wgmma")
-        print("%-28s %9.1f us per block (CUDA events, %d blocks)" % ("gram_wgmma timer", 1e3 * ms / max(n, 1), n))
+        for timer in ("bed_relayout", "gram_wgmma"):
+            ms, n = st.timing(timer)
+            print("%-28s %9.1f us per block (CUDA events, %d blocks)" % (timer + " timer", 1e3 * ms / max(n, 1), n))
         st.set_timing(False)
         st.close()
 
