@@ -506,7 +506,9 @@ class Step2:
         return status, coef, vcov
 
     def debug(self, name, dtype, count):
-        """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block."""
+        """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block; "s2_gp"
+        (uint32 [rows_p][Npad/16]), "s2_T" (float32 [chunk][3 rows_p][drows]) and "s2_FD" (int8 [drows][Npad]): the 2-bit
+        rows, tensor sums and digit rows of F of the last 2-bit block."""
         return debug_fetch(self, name, dtype, count)
 
     def firth(self, variant_idx, trait_idx):

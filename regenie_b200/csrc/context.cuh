@@ -105,7 +105,9 @@ struct rg_ctx {
   int next_lane = 0, last_lane = 0;
   rg::DevBuf<uint8_t> packed_dev;    // step 2 (single lane)
   rg::DevBuf<uint32_t> gp;           // step 2
-  // Gram tile lists on the device, keyed by rows_p: the Z Z^T tiles, and the statistics tiles Z [X | Y]-digits
+  std::map<int, CUtensorMap> gmaps;  // step 2: tensor maps of gp, keyed by rows_p
+  // Gram tile lists on the device (cached_tiles): the Z Z^T tiles keyed by rows_p, and the statistics tiles Z against
+  // digit rows, keyed by rows_p (Step 1: Z [X | Y]-digits) or by rows_p * 4096 + drows / 256 (Step 2: Z F-digits)
   struct TileList {
     rg::DevBuf<int2> buf;
     int count = 0;
@@ -159,15 +161,12 @@ struct rg_ctx {
   bool s2_tc = false;
   int s2_drows = 0, s2_nchunk = 0, s2_ncol = 0;
   int64_t s2_chunk_len = 0;                   // samples per tensor-core chunk (the last one may be shorter)
-  rg::DevBuf<uint8_t> s2_z3, s2_FD;           // [3 rows_p][Npad] planes; digit rows of F
+  rg::DevBuf<uint8_t> s2_FD;                  // [drows][Npad] digit rows of F
   rg::DevBuf<double> s2_Fscale;
   rg::DevBuf<float> s2_T;                     // [chunk][3 rows_p][drows]
   rg::DevBuf<int2> s2_fold_k;
-  std::map<int, std::unique_ptr<rg::DevBuf<int2>>> s2_tile_lists;
   rg::DevBuf<uint8_t> s2_ones;
   CUtensorMap s2_tmD;
-  std::map<int, CUtensorMap> s2_tmZ;          // keyed by rows_p
-  std::map<int, int> s2_ntiles;
   // chrX: male indicator of every sample (empty = none), F column of it, per-block non-PAR flags
   std::vector<uint8_t> s2_male;
   int s2_col_male = -1, bt_col_male = -1;
@@ -241,6 +240,32 @@ void flush_timers(rg_ctx* h);
 void sync_lanes(rg_ctx* h);
 // throws when a kernel of rg_pgen_decode flagged a malformed record (pgen_decode.cu)
 void pgen_check_errors(rg_ctx* h);
+
+// Tensor map of the 2-bit rows gp [rows_p][npad / 16] (the operand of the Gram, statistics and INT8 prediction tiles),
+// made once per rows_p: gp is allocated once, for rows_p_max rows, so its address does not change.
+inline const CUtensorMap& gp_tensor_map(std::map<int, CUtensorMap>& cache, const uint32_t* gp, int64_t npad, int rows_p) {
+  auto it = cache.find(rows_p);
+  if (it == cache.end()) {
+    CUtensorMap tm;
+    make_gp_tensor_map(&tm, gp, npad / 16, rows_p);
+    it = cache.emplace(rows_p, tm).first;
+  }
+  return it->second;
+}
+
+// Device copy of a tile list, built by fill and uploaded on first use of each key.
+template <class Fill>
+const rg_ctx::TileList& cached_tiles(std::map<int, rg_ctx::TileList>& cache, int key, Fill fill) {
+  rg_ctx::TileList& e = cache[key];
+  if (e.count == 0) {
+    std::vector<int2> tiles;
+    fill(tiles);
+    e.buf.alloc(tiles.size());
+    RG_CUDA(cudaMemcpy(e.buf.p, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice));
+    e.count = (int)tiles.size();
+  }
+  return e;
+}
 }
 
 // body of every C ABI entry point: an exception becomes return code 1 and the message of rg_last_error

@@ -87,20 +87,30 @@ void launch_l0_stats_finish(const float* T, int ldt, int64_t t_fold_stride, cons
                             int64_t zz_fold_stride, int rows_p, int cpp, int ncol, int K, const double* scale,
                             int32_t* cnt_fold, double* sum_fold, cudaStream_t s);
 void gram_tile_list(int rows2, std::vector<int2>& tiles);
-// int8 plane rows (make_gram_tensor_map) against int8 rows: Step 2's statistics tiles
-void launch_gram_wgmma(const CUtensorMap& tm, const CUtensorMap& tmB, const int2* tiles, int ntiles, const int2* fold_k, int K,
-                         float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s, int bn = 256);
-// Step 1: Z = [G0; Miss] of a level-0 block from its 2-bit rows (tmG: make_gp_tensor_map over rows_p rows), against
-// itself (tmD == nullptr: the Z Z^T tiles of gram_tile_list) or against int8 digit rows (tmD, bn 256 or 128).
+void stat_tile_list(int zrows, int drows, int bn, std::vector<int2>& tiles);
+// The int8 planes of Z, built from the 2-bit rows inside the Gram kernel: Z row r is plane r / rows_p of 2-bit row
+// r % rows_p, and lut[plane] is a PRMT table whose byte c is the plane's value for code c (3 = missing).  Every table
+// carries a factor 8, which out_scale takes back out.
+struct ZPlanes {
+  uint32_t lut[3];
+};
+constexpr uint32_t kPlaneG = 0x00100800u;      // 8 g, 0 for a missing call
+constexpr uint32_t kPlaneG2 = 0x00200800u;     // 8 g^2
+constexpr uint32_t kPlaneMiss = 0x08000000u;   // 8 for a missing call
+constexpr ZPlanes kZLevel0 = {{kPlaneG, kPlaneMiss, 0u}};         // Z = [G0; Miss] of a level-0 block
+constexpr ZPlanes kZStep2 = {{kPlaneG, kPlaneG2, kPlaneMiss}};    // Z = [G; G^2; Miss]: Step 2's S1, S2, Sm
+// Z of the 2-bit rows (tmG: make_gp_tensor_map over rows_p rows) against itself (tmD == nullptr: the Z Z^T tiles of
+// gram_tile_list, bn 256) or against int8 digit rows (tmD: the statistics tiles of stat_tile_list, bn 256 or 128).
 // miss_total != null: tiles of m tile >= miss_tile0 return at once when *miss_total <= miss_cap (miss_gram.cu)
-void launch_gram_gp(const CUtensorMap& tmG, const CUtensorMap* tmD, int rows_p, const int2* tiles, int ntiles,
-                    const int2* fold_k, int K, float* out, int ldo, int64_t fold_stride, float out_scale, cudaStream_t s,
-                    int bn = 256, const unsigned long long* miss_total = nullptr, int64_t miss_cap = 0,
-                    int miss_tile0 = 0);
-// operand-plane bytes of the Step-1 block (built from the 2-bit rows inside the Gram and prediction kernels): dosage d
-// -> 8 d as int8
+void launch_gram_gp(const CUtensorMap& tmG, const CUtensorMap* tmD, int rows_p, const ZPlanes& planes,
+                    const int2* tiles, int ntiles, const int2* fold_k, int K, float* out, int ldo, int64_t fold_stride,
+                    float out_scale, cudaStream_t s, int bn = 256, const unsigned long long* miss_total = nullptr,
+                    int64_t miss_cap = 0, int miss_tile0 = 0);
 constexpr float kZScaleGram = 1.f / 64;   // Z Z^T tiles: both operands carry 8
-constexpr float kZScaleStat = 1.f / 8;    // Z [X|Y]-digit tiles: the digit rows are plain int8 integers
+// Z digit-row tiles: the digit rows are plain int8 integers.  Each accumulator is 8 x an integer sum, and a multiple of
+// 8 below 2^27 converts to FP32 exactly, so the power-of-two scale leaves that sum exact.  Step 2's sample chunks (at
+// most 2^18 samples, s2_build_digits) keep |acc| <= 8 * 60 * 2^18 < 2^27 (digits |d| <= 15, planes <= 4).
+constexpr float kZScaleStat = 1.f / 8;
 // ---- miss_gram.cu: the Miss rows of the Z Z^T Gram from per-(SNP, fold) lists of the missing calls
 // missing calls per block (as a fraction of bs_max x analysed samples) up to which the sparse sums run: the crossover
 // of tools/miss_rate_sweep.py (DESIGN.md section 3)
@@ -304,13 +314,11 @@ struct S2FinalizeArgs {
 void launch_s2_stats(const uint32_t* gp, int64_t npad, const double* F, int dp, const int4* chunks, int nchunks,
                      int rows_p, double* part, double* sums, cudaStream_t s);
 void launch_s2_finalize(const S2FinalizeArgs& a, cudaStream_t s);
-void launch_bed_expand3_fp8(const uint32_t* gp, int rows_p, uint8_t* z, int64_t npad, cudaStream_t s);
-// hard calls for the binary-trait path: tensor sums -> [rows][4][dp] (S1, S2, Sm, 0) + non-zero / hom-alt counts + dz words
-void launch_s2_bt_bed_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                             const double* scale, double* sums4, double* nnz, double* n2, cudaStream_t s);
+// tensor sums T [chunk][3 rows_p][ldt] -> S1, S2, Sm: sums [rows][3][dp] for s2_finalize_kernel (nnz == nullptr), or
+// for the binary-trait finish on hard calls [rows][4][dp] (S1, S2, Sm, 0) + non-zero / hom-alt counts nnz / n2
+void launch_s2_tensor_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
+                             const double* scale, double* sums, double* nnz, double* n2, cudaStream_t s);
 void launch_gp_to_dz(const uint32_t* gp, int rows_p, uint32_t* dz, int64_t npad, cudaStream_t s);
-void launch_s2_stats_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                            const double* scale, double* sums, cudaStream_t s);
 
 // ---- s2_dosage_kernels.cu
 struct S2BtFinalizeArgs {

@@ -419,15 +419,9 @@ static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, 
   }
 }
 
-// Tensor map of the lane's 2-bit rows (the operand of the Gram, statistics and INT8 prediction tiles), made once per rows_p.
+// Tensor map of the lane's 2-bit rows.
 static const CUtensorMap& gp_map(const rg_ctx* h, rg_ctx::Lane& L, int rows_p) {
-  auto it = L.gmaps.find(rows_p);
-  if (it == L.gmaps.end()) {
-    CUtensorMap tm;
-    make_gp_tensor_map(&tm, L.gp.p, h->Npad / 16, rows_p);
-    it = L.gmaps.emplace(rows_p, tm).first;
-  }
-  return it->second;
+  return gp_tensor_map(L.gmaps, L.gp.p, h->Npad, rows_p);
 }
 
 // Out-of-fold predictions from the coefficients x[m][p][i] at xsrc + m * xstride + (xrow0 + p) * xld + i.
@@ -541,20 +535,6 @@ static rg_ctx::Lane& l0_begin_block(rg_ctx* h, int bs, int block_id, const int32
   return L;
 }
 
-// Device copy of a tile list, built and uploaded on first use for each rows_p.
-template <class Fill>
-static const rg_ctx::TileList& cached_tiles(std::map<int, rg_ctx::TileList>& cache, int rows_p, Fill fill) {
-  rg_ctx::TileList& e = cache[rows_p];
-  if (e.count == 0) {
-    std::vector<int2> tiles;
-    fill(tiles);
-    e.buf.alloc(tiles.size());
-    RG_CUDA(cudaMemcpy(e.buf.p, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice));
-    e.count = (int)tiles.size();
-  }
-  return e;
-}
-
 static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, int bs,
                          const int32_t* sample_idx, int ref_first, int block_id) {
   BlockDims d;
@@ -666,12 +646,12 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     const int64_t zz_stride = (int64_t)4 * rows_p * rows_p;
     ScopedTimer t(h, "gram_wgmma", s);
     if (h->gram_dense) {
-      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, tl.buf.p, tl.count, h->fold_k.p, K,
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p, K,
                      L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s);
       h->launches += 1;
     } else {
       // the Miss rows: the device picks the sparse sums or the dense tiles from the block's missing-call count
-      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, tl.buf.p, tl.count, h->fold_k.p, K,
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p, K,
                      L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
       launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, h->miss_nct, h->miss_fold_ct.p, L.miss_list.p, K,
                          L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
@@ -684,12 +664,11 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     ScopedTimer t(h, "l0_stats", s);
     const int stat_bn = (h->stat_drows % 256 == 0) ? 256 : 128;
     const rg_ctx::TileList& tl = cached_tiles(h->stat_tile_lists, rows_p, [&](std::vector<int2>& tiles) {
-      for (int nj = 0; nj < h->stat_drows / stat_bn; ++nj)
-        for (int mi = 0; mi < 2 * rows_p / 128; ++mi) tiles.push_back(make_int2(mi, nj));
+      stat_tile_list(2 * rows_p, h->stat_drows, stat_bn, tiles);
     });
     L.tstat.alloc((size_t)K * 2 * h->rows_p_max * h->stat_drows);
     const int64_t tfs = (int64_t)2 * rows_p * h->stat_drows;
-    launch_gram_gp(gp_map(h, L, rows_p), &h->tmD, rows_p, tl.buf.p, tl.count, h->fold_k.p,
+    launch_gram_gp(gp_map(h, L, rows_p), &h->tmD, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p,
                    K, L.tstat.p, h->stat_drows, tfs, kZScaleStat, s, stat_bn);
     launch_l0_stats_finish(L.tstat.p, h->stat_drows, tfs, L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, rows_p,
                            h->cpp, C + P, K, h->xy_scale.p, L.cnt_fold.p, L.sum_fold.p, s);
@@ -817,6 +796,12 @@ static DebugView s2_debug_view(const rg_ctx* h, const std::string& n) {
   if (n == "bt_sums") return dev_view(h->bt_sums.p, (size_t)h->bt_sums_rows * 4 * h->bt_sums_dp * 8);   // [rows_p][4][dp]
   if (n == "bt_nnz") return dev_view(h->bt_nnz.p, (size_t)h->bt_sums_rows * 8);
   if (n == "bt_n510") return dev_view(h->bt_n510.p, (size_t)h->bt_sums_rows * 8);
+  // the tensor sums, when the last block was a 2-bit one: its rows [rows_p][Npad/16], the digit sums
+  // [s2_nchunk][3 rows_p][drows] of the planes [G; G^2; Miss], and the digit rows of F [drows][Npad] they were taken against
+  const size_t rp = (size_t)round_up(h->s2_last_bs, kRowPad);
+  if (n == "s2_gp") return dev_view(h->gp.p, rp * (h->Npad / 16) * 4);
+  if (n == "s2_T" && h->s2_tc) return dev_view(h->s2_T.p, (size_t)h->s2_nchunk * 3 * rp * h->s2_drows * 4);
+  if (n == "s2_FD" && h->s2_tc) return dev_view(h->s2_FD.p, (size_t)h->s2_drows * h->Npad);
   throw Error{"unknown Step-2 debug buffer: " + n};
 }
 

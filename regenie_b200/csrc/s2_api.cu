@@ -90,31 +90,16 @@ static void s2_build_digits(rg_ctx* h, const double* Fdev, int dp, int D) {
   RG_CUDA(cudaMemcpyAsync(h->s2_fold_k.p, fk.data(), fk.size() * sizeof(int2), cudaMemcpyHostToDevice, s));
 }
 
-// 2-bit rows in h->gp -> S1 / S2 / Sm digit sums in h->s2_T (three int8 planes x digit rows, INT8 Gram kernel)
+// 2-bit rows in h->gp -> S1 / S2 / Sm digit sums in h->s2_T: the planes [G; G^2; Miss] against the digit rows, INT8 Gram
+// kernel
 static void s2_tensor_sums(rg_ctx* h, int rows_p, cudaStream_t s) {
   const int drows = h->s2_drows;
-  const int64_t Npad = h->Npad;
-  h->s2_z3.alloc((size_t)3 * h->rows_p_max * Npad);
   h->s2_T.alloc((size_t)h->s2_nchunk * 3 * h->rows_p_max * drows);
-  launch_bed_expand3_fp8(h->gp.p, rows_p, h->s2_z3.p, Npad, s);
-  if (!h->s2_tmZ.count(rows_p)) {
-    CUtensorMap tm;
-    make_gram_tensor_map(&tm, h->s2_z3.p, Npad, 3 * rows_p);
-    h->s2_tmZ[rows_p] = tm;
-  }
-  const int key = rows_p * 4096 + drows / 256;
-  if (!h->s2_tile_lists.count(key)) {
-    std::vector<int2> tiles;
-    for (int nj = 0; nj < drows / 256; ++nj)
-      for (int mi = 0; mi < 3 * rows_p / 128; ++mi) tiles.push_back(make_int2(mi, nj));
-    auto buf = std::make_unique<DevBuf<int2>>();
-    buf->alloc(tiles.size());
-    RG_CUDA(cudaMemcpy(buf->p, tiles.data(), tiles.size() * sizeof(int2), cudaMemcpyHostToDevice));
-    h->s2_ntiles[key] = (int)tiles.size();
-    h->s2_tile_lists[key] = std::move(buf);
-  }
-  launch_gram_wgmma(h->s2_tmZ[rows_p], h->s2_tmD, h->s2_tile_lists[key]->p, h->s2_ntiles[key], h->s2_fold_k.p,
-                      h->s2_nchunk, h->s2_T.p, drows, (int64_t)3 * rows_p * drows, 1.f, s);
+  const rg_ctx::TileList& tl = cached_tiles(h->stat_tile_lists, rows_p * 4096 + drows / 256, [&](std::vector<int2>& tiles) {
+    stat_tile_list(3 * rows_p, drows, 256, tiles);
+  });
+  launch_gram_gp(gp_tensor_map(h->gmaps, h->gp.p, h->Npad, rows_p), &h->s2_tmD, rows_p, kZStep2, tl.buf.p, tl.count,
+                 h->s2_fold_k.p, h->s2_nchunk, h->s2_T.p, drows, (int64_t)3 * rows_p * drows, kZScaleStat, s);
 }
 
 static void s2_set_chr(rg_ctx* h, const double* res, const double* scf_sv) {
@@ -288,8 +273,8 @@ static void s2_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, h->gp.p, Npad, s);
   if (h->s2_tc) {
     s2_tensor_sums(h, rows_p, s);
-    launch_s2_stats_finish(h->s2_T.p, h->s2_drows, (int64_t)3 * rows_p * h->s2_drows, h->s2_nchunk, rows_p, h->dp, h->s2_ncol,
-                           h->s2_Fscale.p, h->s2_sums.p, s);
+    launch_s2_tensor_finish(h->s2_T.p, h->s2_drows, (int64_t)3 * rows_p * h->s2_drows, h->s2_nchunk, rows_p, h->dp,
+                            h->s2_ncol, h->s2_Fscale.p, h->s2_sums.p, nullptr, nullptr, s);
   } else {
     launch_s2_stats(h->gp.p, Npad, h->F.p, h->dp, h->chunks.p, h->nchunks, rows_p, h->s2_part.p, h->s2_sums.p, s);
   }
@@ -452,7 +437,7 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   h->bt_nnz.alloc(h->rows_p_max); h->bt_n510.alloc(h->rows_p_max);
   launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p, ref_first, h->gp.p, Npad, s);
   s2_tensor_sums(h, rows_p, s);
-  launch_s2_bt_bed_finish(h->s2_T.p, h->s2_drows, (int64_t)3 * rows_p * h->s2_drows, h->s2_nchunk, rows_p, dp, h->s2_ncol,
+  launch_s2_tensor_finish(h->s2_T.p, h->s2_drows, (int64_t)3 * rows_p * h->s2_drows, h->s2_nchunk, rows_p, dp, h->s2_ncol,
                           h->s2_Fscale.p, h->bt_sums.p, h->bt_nnz.p, h->bt_n510.p, s);
   launch_gp_to_dz(h->gp.p, rows_p, h->dz.p, Npad, s);               // what rg_s2_firth / rg_s2_spa read
   S2BtFinalizeArgs a;
@@ -460,7 +445,7 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   s2_finalize_args(h, a, bs, dp, min_mac, h->bt_sums.p, h->bt_col_male);
   a.unit = 1.0;
   launch_s2_bt_finalize(a, s);
-  h->launches += 7;
+  h->launches += 5;
   h->s2_last_bs = bs;
   h->bt_sums_rows = rows_p; h->bt_sums_dp = dp;
   s2_copy_out(h, bs, out, nullptr, nullptr, s);

@@ -177,41 +177,20 @@ __global__ void s2_finalize_kernel(S2FinalizeArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The same sums on the tensor cores, exactly: three int8 planes of a variant row (g0, g0^2, missing) against the
-// radix-30 digit rows of the feature matrix F (built once per chromosome by l0_xy_digits_kernel), as column tiles of
-// the INT8 Gram kernel.  Products are integers <= 60, sample chunks are kept below 2^18 so every sum is an exact
-// integer < 2^24; the chunk sums are added and reassembled in FP64 here.  Counts (N, A1FREQ numerators) come from the
-// 0/1 columns of F, whose digits are exact, so they stay bit-exact.
-__global__ void bed_expand3_fp8_kernel(const uint32_t* __restrict__ gp, int64_t words_per_row, int rows_p,
-                                       uint8_t* __restrict__ z, int64_t npad) {
-  const int64_t w = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  const int row = blockIdx.y;
-  if (w >= words_per_row) return;
-  const uint32_t word = __ldg(gp + (int64_t)row * words_per_row + w);
-  const uint32_t kLutG = 0x00020100u;   // code 0 -> 0, 1 -> 1, 2 -> 2, 3 (missing) -> 0
-  const uint32_t kLutQ = 0x00040100u;   // g^2: 0, 1, 4, 0
-  const uint32_t kLutM = 0x01000000u;   // missing -> 1
-  uint4 g, q, m;
-  uint32_t* gv = reinterpret_cast<uint32_t*>(&g);
-  uint32_t* qv = reinterpret_cast<uint32_t*>(&q);
-  uint32_t* mv = reinterpret_cast<uint32_t*>(&m);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const uint32_t b = (word >> (8 * k)) & 0xFFu;
-    const uint32_t sel = (b & 0x3u) | ((b & 0xCu) << 2) | ((b & 0x30u) << 4) | ((b & 0xC0u) << 6);
-    gv[k] = __byte_perm(kLutG, 0, sel);
-    qv[k] = __byte_perm(kLutQ, 0, sel);
-    mv[k] = __byte_perm(kLutM, 0, sel);
-  }
-  *reinterpret_cast<uint4*>(z + (int64_t)row * npad + w * 16) = g;
-  *reinterpret_cast<uint4*>(z + (int64_t)(rows_p + row) * npad + w * 16) = q;
-  *reinterpret_cast<uint4*>(z + (int64_t)(2 * rows_p + row) * npad + w * 16) = m;
-}
-
-// T [chunk][3 rows_p][ldt] exact digit sums -> sums [row][3][dp] (S1, S2, Sm).  grid: (ceil(D/128), rows_p), block 128.
+// The same sums on the tensor cores, exactly: the planes G, G^2 and Miss of a variant row, built in registers from the
+// 2-bit rows, against the radix-30 digit rows of the feature matrix F (built once per chromosome by
+// l0_xy_digits_kernel), as column tiles of the INT8 Gram kernel (gram_wgmma.cu, kZStep2).  Products are integers <= 60,
+// sample chunks are kept below 2^18 so every sum is an exact integer < 2^24; the chunk sums are added and reassembled
+// in FP64 here.  Counts (N, A1FREQ numerators) come from the 0/1 columns of F, whose digits are exact, so they stay
+// bit-exact.
+// T [chunk][3 rows_p][ldt] exact digit sums -> S1, S2, Sm of row i: sums [row][3][dp], or with nnz [row][4][dp] (Se = 0,
+// the layout of s2_bt_finalize_kernel) plus the counts check_sparse_G needs: non-zero calls n1 + n2 and hom-alt calls
+// n2 from the column of F that flags the analysed samples (n1 = 2 S1 - S2, n2 = (S2 - S1) / 2).
+// grid: (ceil(dp/128), rows_p), block 128.
 __global__ void __launch_bounds__(128)
-s2_stats_finish_kernel(const float* __restrict__ T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                       const double* __restrict__ scale, double* __restrict__ sums) {
+s2_tensor_finish_kernel(const float* __restrict__ T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
+                        const double* __restrict__ scale, double* __restrict__ sums, double* __restrict__ nnz,
+                        double* __restrict__ n2o) {
   const int c = blockIdx.x * 128 + threadIdx.x;
   const int i = blockIdx.y;
   if (c >= dp) return;
@@ -231,42 +210,12 @@ s2_stats_finish_kernel(const float* __restrict__ T, int ldt, int64_t chunk_strid
       out[pl] = acc * s / 15.0;      // exact for the 0/1 columns (acc = 15 k, s = 1): N and A1FREQ stay bit-exact
     }
   }
-  double* o = sums + ((int64_t)i * 3) * dp + c;
+  const int nsum = nnz ? 4 : 3;
+  double* o = sums + ((int64_t)i * nsum) * dp + c;
   o[0] = out[0];
   o[dp] = out[1];
   o[2 * dp] = out[2];
-}
-
-// binary traits on hard calls: same tensor sums, laid out for s2_bt_finalize_kernel ([row][4][dp]: S1, S2, Sm, Se = 0,
-// unit = 1), plus the counts check_sparse_G needs: non-zero calls n1 + n2 and hom-alt calls n2 from the column of F
-// that flags the analysed samples (n1 = 2 S1 - S2, n2 = (S2 - S1) / 2).  grid: (ceil(dp/128), rows_p), block 128.
-__global__ void __launch_bounds__(128)
-s2_bt_bed_finish_kernel(const float* __restrict__ T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                        const double* __restrict__ scale, double* __restrict__ sums4, double* __restrict__ nnz,
-                        double* __restrict__ n2o) {
-  const int c = blockIdx.x * 128 + threadIdx.x;
-  const int i = blockIdx.y;
-  if (c >= dp) return;
-  double out[3] = {0.0, 0.0, 0.0};
-  if (c < D) {
-    const int r0 = (c / kStatQ) * 128 + (c % kStatQ) * kLimbs;
-    const double s = scale[c];
-#pragma unroll
-    for (int pl = 0; pl < 3; ++pl) {
-      double acc = 0.0;
-#pragma unroll
-      for (int l = kLimbs - 1; l >= 0; --l) {
-        double d = 0.0;
-        for (int ch = 0; ch < nchunk; ++ch) d += (double)T[(int64_t)ch * chunk_stride + (int64_t)(pl * rows_p + i) * ldt + r0 + l];
-        acc = acc * (1.0 / 30.0) + d;
-      }
-      out[pl] = acc * s / 15.0;
-    }
-  }
-  double* o = sums4 + ((int64_t)i * 4) * dp + c;
-  o[0] = out[0];
-  o[dp] = out[1];
-  o[2 * dp] = out[2];
+  if (!nnz) return;
   o[3 * dp] = 0.0;
   if (c == 0) {
     const double hom = (out[1] - out[0]) * 0.5;
@@ -290,28 +239,16 @@ __global__ void gp_to_dz_kernel(const uint32_t* __restrict__ gp, int64_t words_p
   }
 }
 
-void launch_s2_bt_bed_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                             const double* scale, double* sums4, double* nnz, double* n2, cudaStream_t s) {
+void launch_s2_tensor_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
+                             const double* scale, double* sums, double* nnz, double* n2, cudaStream_t s) {
   dim3 grid((unsigned)ceil_div(dp, 128), rows_p);
-  s2_bt_bed_finish_kernel<<<grid, 128, 0, s>>>(T, ldt, chunk_stride, nchunk, rows_p, dp, D, scale, sums4, nnz, n2);
+  s2_tensor_finish_kernel<<<grid, 128, 0, s>>>(T, ldt, chunk_stride, nchunk, rows_p, dp, D, scale, sums, nnz, n2);
 }
 
 void launch_gp_to_dz(const uint32_t* gp, int rows_p, uint32_t* dz, int64_t npad, cudaStream_t s) {
   const int64_t wpr = npad / 16;
   dim3 grid((unsigned)ceil_div(wpr, 256), rows_p);
   gp_to_dz_kernel<<<grid, 256, 0, s>>>(gp, wpr, dz, npad);
-}
-
-void launch_bed_expand3_fp8(const uint32_t* gp, int rows_p, uint8_t* z, int64_t npad, cudaStream_t s) {
-  const int64_t wpr = npad / 16;
-  dim3 grid((unsigned)ceil_div(wpr, 256), rows_p);
-  bed_expand3_fp8_kernel<<<grid, 256, 0, s>>>(gp, wpr, rows_p, z, npad);
-}
-
-void launch_s2_stats_finish(const float* T, int ldt, int64_t chunk_stride, int nchunk, int rows_p, int dp, int D,
-                            const double* scale, double* sums, cudaStream_t s) {
-  dim3 grid((unsigned)ceil_div(dp, 128), rows_p);
-  s2_stats_finish_kernel<<<grid, 128, 0, s>>>(T, ldt, chunk_stride, nchunk, rows_p, dp, D, scale, sums);
 }
 
 void launch_s2_stats(const uint32_t* gp, int64_t npad, const double* F, int dp, const int4* chunks, int nchunks,

@@ -2,10 +2,11 @@
 
 Step 2 forms every statistic from code-wise sums  S1 = sum g F,  S2 = sum g^2 F,  Sm = sum miss F  (and Se = sum e F for
 dosages, e = 4 p_hom + p_het) of one per-sample feature row F, and picks the kernels that form them from the input:
-  * 2-bit rows (.bed / .pgen): three int8 planes against radix-30 digit rows of F on the tensor cores, over sample
-    chunks that keep 60 * chunk < 2^24 (ceil(Npad / 2^18) chunks, more when the tiles would not fill the SMs), every
-    digit sum an exact integer, FP64 Horner after.  RG_B200_S2_STATS=f64, read at every rg_s2_set_chr, selects the FP64
-    CUDA-core kernel over chunks of 2048 samples instead;
+  * 2-bit rows (.bed / .pgen): three int8 planes (g, g^2, missing), built from the 2-bit rows inside the Gram kernel,
+    against radix-30 digit rows of F on the tensor cores, over sample chunks that keep 60 * chunk < 2^24
+    (ceil(Npad / 2^18) chunks, more when the tiles would not fill the SMs), every digit sum an exact integer, FP64
+    Horner after.  RG_B200_S2_STATS=f64, read at every rg_s2_set_chr, selects the FP64 CUDA-core kernel over chunks of
+    2048 samples instead;
   * 8-bit dosages: dosage_relayout_kernel (one 8-byte load per four samples when they are consecutive and the address is
     8-byte aligned, per-sample loads otherwise: odd file rows mix both) and dosage_stats_kernel over chunks of 2048
     samples and tiles of 16 feature columns, the last tile partly live, then a fixed-order sum of the chunks and of
