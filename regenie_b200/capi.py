@@ -325,6 +325,7 @@ class Step2:
         h = C.c_void_p()
         check(L.rg_step2_create(C.byref(cfg), _ptr(X), _ptr(mask), _ptr(ia), C.byref(h)))
         self.h = h
+        self.last_bs = None                 # variants of the last block call that succeeded (what interaction() reads)
 
     def close(self):
         if getattr(self, "h", None):
@@ -365,6 +366,7 @@ class Step2:
             sample_idx = np.ascontiguousarray(sample_idx, dtype=np.int32)
         check(lib().rg_s2_block_bed(self.h, _ptr(packed), row_stride, bs, _ptr(sample_idx), int(ref_first),
                                     float(min_mac), C.byref(so)))
+        self.last_bs = int(bs)
         return o
 
     def _out(self, bs, with_info=False):
@@ -392,6 +394,7 @@ class Step2:
         """rg_s2_block_bed on a raw (host or DEVICE) address; `out` = a (dict, S2Out) pair from _out() to reuse."""
         o, so = out or self._out(bs)
         check(lib().rg_s2_block_bed(self.h, C.c_void_p(ptr), int(row_stride), int(bs), None, 0, float(min_mac), C.byref(so)))
+        self.last_bs = int(bs)
         return o
 
     def block_bgen8_bt_raw(self, probs_ptr, miss_ptr, n_file, bs, out=None, min_mac=5.0):
@@ -402,6 +405,7 @@ class Step2:
         o, so = out or self._out(bs, with_info=True)
         check(L.rg_s2_block_bgen8_bt(self.h, C.c_void_p(probs_ptr), C.c_void_p(miss_ptr), int(n_file), int(bs), None, 0,
                                      float(min_mac), C.byref(so), _ptr(o["info"])))
+        self.last_bs = int(bs)
         return o
 
     # ---- binary traits on BGEN 8-bit dosages
@@ -433,6 +437,7 @@ class Step2:
             sample_idx = np.ascontiguousarray(sample_idx, dtype=np.int32)
         check(L.rg_s2_block_bed_bt(self.h, _ptr(packed), packed.shape[1], bs, _ptr(sample_idx), int(ref_first),
                                    float(min_mac), C.byref(so)))
+        self.last_bs = int(bs)
         return o
 
     def block_bgen8(self, probs, missing=None, sample_idx=None, ref_first=False, min_mac=5.0):
@@ -459,6 +464,7 @@ class Step2:
             sample_idx = np.ascontiguousarray(sample_idx, dtype=np.int32)
         check(getattr(L, _fn)(self.h, _ptr(probs), _ptr(missing), n_file, bs, _ptr(sample_idx),
                                      int(ref_first), float(min_mac), C.byref(so), _ptr(o["info"])))
+        self.last_bs = int(bs)
         return o
 
     def bgen_inflate(self, comp, comp_offs, n_file):
@@ -494,8 +500,18 @@ class Step2:
         st = S2IntChr(E.ctypes.data, K, *[keep[k].ctypes.data if K else None for k in (1, 2, 3)])
         check(L.rg_s2_set_interaction(self.h, C.byref(st)))
 
-    def interaction(self, bs, rare_mac=1000.0, min_mac=5.0, force_robust=False, force_hc4=False, no_robust=False):
-        """rg_s2_interaction on the resident block: (status [bs, P], coef [bs, P, 2], vcov [bs, P, 2, 2])."""
+    def interaction(self, bs=None, rare_mac=1000.0, min_mac=5.0, force_robust=False, force_hc4=False, no_robust=False):
+        """rg_s2_interaction on the resident block: (status [bs, P], coef [bs, P, 2], vcov [bs, P, 2, 2]).
+
+        The library writes one row per variant of the last block call, so the outputs are sized for that block; `bs`, when
+        given, must equal its size.  Raises ValueError, without calling the library, when no block call has succeeded on
+        this handle or when `bs` differs."""
+        if self.last_bs is None:
+            raise ValueError("interaction() needs a block call first")
+        if bs is None:
+            bs = self.last_bs
+        elif int(bs) != self.last_bs:
+            raise ValueError("interaction(bs=%d): the last block had %d variants" % (int(bs), self.last_bs))
         L = lib()
         L.rg_s2_interaction.argtypes = [C.c_void_p] * 5
         P = self.P
@@ -508,7 +524,11 @@ class Step2:
     def debug(self, name, dtype, count):
         """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block; "s2_gp"
         (uint32 [rows_p][Npad/16]), "s2_T" (float32 [chunk][3 rows_p][drows]) and "s2_FD" (int8 [drows][Npad]): the 2-bit
-        rows, tensor sums and digit rows of F of the last 2-bit block."""
+        rows, tensor sums and digit rows of F of the last 2-bit block.  GxE interaction: "int_F" (float64 [Npad][nf]),
+        the feature rows rg_s2_set_interaction built; of the last interaction() call since then, "int_paths" (int64 x 8:
+        sample chunks, Npad, nf, robust columns nr, HLM columns per trait K, trait groups of the meat kernel, host slabs
+        of the feature rows, bs), "int_route" (int8 [bs]: 0 none, 1 robust, 2 HLM) and "int_sums" (float64 [bs][nf],
+        defined at the columns the variant's route reads)."""
         return debug_fetch(self, name, dtype, count)
 
     def firth(self, variant_idx, trait_idx):

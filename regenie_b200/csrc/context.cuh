@@ -198,6 +198,7 @@ struct rg_ctx {
   bool s2_dz_qt = false;             // dz holds the words of the resident quantitative-trait block of this chromosome
   rg::DevBuf<int8_t> int_route;
   int int_K = 0, int_nr = 0, int_nf = 0;
+  int int_last_bs = 0;               // variants of the last rg_s2_interaction since rg_s2_set_interaction (0: none)
   rg::DevBuf<double> int_F, int_E, int_part, int_sums, int_var, int_meat, int_out;
   rg::DevBuf<uint8_t> int_pow2;
   rg::DevBuf<int32_t> int_status;

@@ -388,6 +388,8 @@ struct SpaArgs {
 void launch_s2_spa(const SpaArgs& a, cudaStream_t s);
 
 // ---- s2_interaction.cu
+constexpr int kIntTG = 8;            // traits per CTA of the meat kernel (blockIdx.z = trait group)
+constexpr int64_t kIntSlab = 16384;  // samples per host slab of the feature rows (rg_s2_set_interaction)
 struct S2IntArgs {
   int bs, C, P, dp, K, nf, nr, nchunks, var_stride;
   int force_robust, force_hc4, no_robust;

@@ -802,6 +802,22 @@ static DebugView s2_debug_view(const rg_ctx* h, const std::string& n) {
   if (n == "s2_gp") return dev_view(h->gp.p, rp * (h->Npad / 16) * 4);
   if (n == "s2_T" && h->s2_tc) return dev_view(h->s2_T.p, (size_t)h->s2_nchunk * 3 * rp * h->s2_drows * 4);
   if (n == "s2_FD" && h->s2_tc) return dev_view(h->s2_FD.p, (size_t)h->s2_drows * h->Npad);
+  // GxE interaction state of the chromosome: its feature rows [Npad][nf] once rg_s2_set_interaction has run; the shape,
+  // the routes [bs] and the chunk-reduced sums [bs][nf] (defined where the variant's route reads them) of the last
+  // rg_s2_interaction call since then
+  if (n.compare(0, 4, "int_") == 0) {
+    RG_CHECK(h->int_set, "no interaction state on this handle: " + n);
+    if (n == "int_F") return dev_view(h->int_F.p, (size_t)h->Npad * h->int_nf * 8);
+    RG_CHECK(h->int_last_bs > 0, "no rg_s2_interaction call since rg_s2_set_interaction: " + n);
+    const int bs = h->int_last_bs;
+    if (n == "int_paths") {
+      const int64_t v[8] = {h->nchunks, h->Npad, h->int_nf, h->int_nr, h->int_K, ceil_div(h->P, kIntTG),
+                            ceil_div(h->Npad, kIntSlab), bs};
+      return host_view(v, 8);
+    }
+    if (n == "int_route") return dev_view(h->int_route.p, (size_t)bs);
+    if (n == "int_sums") return dev_view(h->int_sums.p, (size_t)bs * h->int_nf * 8);
+  }
   throw Error{"unknown Step-2 debug buffer: " + n};
 }
 

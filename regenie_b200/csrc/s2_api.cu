@@ -144,6 +144,7 @@ static void s2_set_chr(rg_ctx* h, const double* res, const double* scf_sv) {
   RG_CUDA(cudaStreamSynchronize(h->stream));
   h->s2_chr_set = true;
   h->int_set = false;                                                // rg_s2_set_interaction follows, per chromosome
+  h->int_last_bs = 0;
   h->s2_dz_qt = false;
 }
 
@@ -533,7 +534,7 @@ static void s2_set_interaction(rg_ctx* h, const rg_s2_int_chr* st) {
   RG_CUDA(cudaMemcpyAsync(h->int_E.p, E.data(), Npad * 8, cudaMemcpyHostToDevice, h->stream));
   RG_CUDA(cudaMemcpyAsync(h->int_pow2.p, pow2.data(), nf, cudaMemcpyHostToDevice, h->stream));
   // the rows go up in slabs of kSlab samples, so the host holds one slab of them (and of F) at a time
-  constexpr int64_t kSlab = 16384;
+  constexpr int64_t kSlab = kIntSlab;
   std::vector<double> Fh((size_t)kSlab * dp), F((size_t)kSlab * nf);
   for (int64_t s0 = 0; s0 < Npad; s0 += kSlab) {
     const int64_t ns = std::min(kSlab, Npad - s0);
@@ -563,6 +564,7 @@ static void s2_set_interaction(rg_ctx* h, const rg_s2_int_chr* st) {
   }
   RG_CUDA(cudaStreamSynchronize(h->stream));
   h->int_K = K; h->int_nr = nr; h->int_nf = nf;
+  h->int_last_bs = 0;
   h->int_set = true;
 }
 
@@ -599,6 +601,7 @@ static void s2_interaction(rg_ctx* h, const rg_s2_int_opts* o, int32_t* status, 
   a.coef = h->int_out.p; a.vcov = h->int_out.p + (size_t)bs * P * 2;
   launch_s2_interaction(a, h->int_pow2.p, h->int_part.p, s);
   h->launches += 5;
+  h->int_last_bs = bs;
   RG_CUDA(cudaMemcpyAsync(status, a.status, (size_t)bs * P * 4, cudaMemcpyDeviceToHost, s));
   RG_CUDA(cudaMemcpyAsync(coef, a.coef, (size_t)bs * P * 2 * 8, cudaMemcpyDeviceToHost, s));
   RG_CUDA(cudaMemcpyAsync(vcov, a.vcov, (size_t)bs * P * 4 * 8, cudaMemcpyDeviceToHost, s));

@@ -180,7 +180,6 @@ __global__ void s2_int_finish_kernel(S2IntArgs a) {
 
 // meat of one robust variant over one sample chunk, for kIntTG traits at a time (all of them when P <= kIntTG): the
 // leverage h_i of a sample is formed once, then per trait sum w_i H_i H_i^T (3 entries) and sum e_i^2
-constexpr int kIntTG = 8;
 __global__ void __launch_bounds__(256) s2_int_meat_kernel(S2IntArgs a) {
   const int v = blockIdx.y, p0 = blockIdx.z * kIntTG;
   const double* W = a.var + (int64_t)v * a.var_stride;
