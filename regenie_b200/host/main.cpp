@@ -1358,24 +1358,34 @@ struct S2Input : GenoInput {
     if (b + 1 < blocks.size()) pending = fetch(b + 1);
   }
 
-  const int32_t* sidx() const { return subset ? sample_idx.data() : nullptr; }
-
   void set_non_par(rg_handle h, size_t b) {
     if (non_par_flags(p, snps, blocks[b], npf)) rg_check(rg_s2_set_non_par(h, npf.data(), blocks[b].size));
   }
 
-  // the dosages of block b for the block calls: the fetched bytes, or the payloads inflated on the device
-  void dosages(rg_handle h, size_t b, const uint8_t** pd, const uint8_t** md) {
-    *pd = probs[b & 1].data();
-    *md = pmiss[b & 1].data();
-    if (dev_inflate) rg_check(rg_bgen_inflate(h, comp[b & 1].data(), comp_offs[b & 1].data(), (int64_t)n_file, blocks[b].size, pd, md));
+  // the genotypes of one block as a block call takes them: 8-bit dosages `g` with their missingness bytes `miss`, or
+  // 2-bit rows `g` of `stride` bytes
+  struct Rows { const uint8_t *g, *miss; int64_t stride; int bs; };
+
+  // block b for the block calls: the fetched bytes, the payloads inflated on the device, or the .pgen records decoded there
+  Rows block(rg_handle h, size_t b) {
+    Rows k{nullptr, nullptr, (int64_t)g.row_stride, blocks[b].size};
+    if (use_bgen) {
+      k.g = probs[b & 1].data();
+      k.miss = pmiss[b & 1].data();
+      if (dev_inflate) rg_check(rg_bgen_inflate(h, comp[b & 1].data(), comp_offs[b & 1].data(), (int64_t)n_file, k.bs, &k.g, &k.miss));
+    } else {
+      k.g = rows[b & 1].data();
+      if (pgen_dev) pgen_rows_device(h, pbatch[b & 1], k.bs, (int64_t)g.pg->n_file, (int)b, &k.g, &k.stride);
+    }
+    return k;
   }
 
-  // the 2-bit rows of block b for the block calls: the fetched rows, or the .pgen records decoded on the device
-  void hard_calls(rg_handle h, size_t b, const uint8_t** r, int64_t* stride) {
-    *r = rows[b & 1].data();
-    *stride = (int64_t)g.row_stride;
-    if (pgen_dev) pgen_rows_device(h, pbatch[b & 1], blocks[b].size, (int64_t)g.pg->n_file, (int)b, r, stride);
+  // the one place that calls the four block routes: the route of the input kind and of the trait kind `bt` on h
+  void test(rg_handle h, bool bt, const Rows& k, double min_mac, const rg_s2_out& o, double* info) const {
+    if (use_bgen && bt) rg_check(rg_s2_block_bgen8_bt(h, k.g, k.miss, (int64_t)n_file, k.bs, sidx(), p.ref_first, min_mac, &o, info));
+    else if (use_bgen) rg_check(rg_s2_block_bgen8(h, k.g, k.miss, (int64_t)n_file, k.bs, sidx(), p.ref_first, min_mac, &o, info));
+    else if (bt) rg_check(rg_s2_block_bed_bt(h, k.g, k.stride, k.bs, sidx(), p.ref_first, min_mac, &o));
+    else rg_check(rg_s2_block_bed(h, k.g, k.stride, k.bs, sidx(), p.ref_first, min_mac, &o));
   }
 
   // --test dominant / recessive: the fetched bytes of block b recoded in place for the second pass
@@ -1408,353 +1418,302 @@ void s2_row_start(const S2Input& in, size_t b, int v, const S2Results& r, const 
                             in.use_bgen ? in.info1[b & 1][v] : -1.0);
 }
 
-void run_step2_qt(const Params& p, Log& log) {
-  S2Input in(p, false, log);
-  const Pheno& ph = in.ph;
-  const int64_t N = ph.N;
-  const int P = ph.P;
-  rg_handle h = nullptr;
-  HandleGuard guard{h};
-  require_device();
-  in.create_handle(ph.mask.data(), ph.strict, &h);
-
-  S2Writers w;
-  w.open(p, ph, in.use_bgen);
-  std::vector<std::string>& obuf = w.obuf;                   // rows of the current block, one buffer per trait
-  std::string head_s;
-  GenoCounts gc(p.no_split, p.bsize, P, in.use_bgen ? 0 : in.g.row_stride, p.ref_first);
-  in.start(log);
-  // --test dominant / recessive: the second pass on the recoded genotypes keeps its counts in r2 (see Recode)
-  S2Results r, r2;
-  r.init(p.bsize, P);
-  if (p.test_type) r2.init(p.bsize, P);
-  const rg_s2_out out = r.out(), out2 = r2.out(r);
-  const Recode recode(p.test_type, p.ref_first);
-  // --htp: test_string + wgr_string + correction_type (src/Data.cpp:2075-2102)
-  const std::string htp_model = std::string(test_name(p.test_type)) + (p.ignore_pred ? "" : "-WGR") + "-LR";
-  std::vector<double> res((size_t)N * P), scf(P);
-  int cur_chr = -1;
-  size_t n_ignored = 0;
-  for (size_t b = in.b_first; b < in.blocks.size(); ++b) {
-    const int chrom = in.blocks[b].chrom, bs = in.blocks[b].size;
-    if (chrom != cur_chr) {
-      cur_chr = chrom;
-      log << "Chromosome " << chrom << "\n";
-      // blup_read_chr + compute_res (src/Step2_Models.cpp:96-124, src/Data.cpp:2386-2404)
-      for (int i = 0; i < P; ++i) {
-        const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
-        double ssq = 0.0;
-        for (int64_t s = 0; s < N; ++s) {
-          const double rv = (ph.Y[(size_t)i * N + s] - blup[s]) * ph.mask[(size_t)i * N + s];
-          res[(size_t)i * N + s] = rv;
-          ssq += rv * rv;
-        }
-        const double psd = std::sqrt(ssq) / std::sqrt(ph.neff[i] - ph.C);
-        for (int64_t s = 0; s < N; ++s) res[(size_t)i * N + s] /= psd;
-        scf[i] = ph.scale_Y[i] * psd;
-      }
-      rg_check(rg_s2_set_sex(h, chrom == 23 ? in.male.data() : nullptr));
-      rg_check(rg_s2_set_chr(h, res.data(), scf.data()));
-    }
-    in.next(b);
-    if (!in.use_bgen)
-      gc.run(in.rows[b & 1].data(), (size_t)bs * in.g.row_stride, bs, [&](const uint8_t* rw, const rg_s2_out* o) {
-        rg_check(rg_s2_block_bed(h, rw, (int64_t)in.g.row_stride, bs, in.sidx(), p.ref_first, 0.0, o));
-      });
-    in.set_non_par(h, b);
-    if (in.use_bgen) {
-      const uint8_t *pd, *md;
-      in.dosages(h, b, &pd, &md);
-      rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, p.min_mac, &out, r.info.data()));
-      if (p.test_type) {
-        in.recode(recode, b);
-        rg_check(rg_s2_block_bgen8(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &out2, r2.info.data()));
-      }
-    } else {
-      const uint8_t* rows;
-      int64_t stride;
-      in.hard_calls(h, b, &rows, &stride);
-      rg_check(rg_s2_block_bed(h, rows, stride, bs, in.sidx(), p.ref_first, p.min_mac, &out));
-      if (p.test_type) {
-        in.recode(recode, b);
-        rg_check(rg_s2_block_bed(h, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &out2));
-      }
-    }
-    if (p.test_type) merge_recode_flags(bs, r.flags.data(), r2.flags.data(), r2.af_all.data());
-    for (int v = 0; v < bs; ++v) {
-      if (r.flags[v] & 3) { ++n_ignored; continue; }          // no row for ignored variants (split mode)
-      if (in.use_info1 && p.min_info > 0 && in.info1[b & 1][v] < p.min_info) { ++n_ignored; continue; }
-      s2_row_start(in, b, v, r, gc, w, head_s);
-      for (int i = 0; i < P; ++i) {
-        const size_t e = (size_t)v * P + i;
-        const bool have = !(r.mac[e] < p.min_mac) &&           // ignored_trait (src/Geno.cpp:3102)
-                          !(in.use_bgen && r.info[e] < p.min_info);   // --minINFO (src/Geno.cpp:3142-3146)
-        if (p.no_split) { append_sumstats_all_trait(w.obuf_all, have, r.beta[e], r.se[e], r.chisq[e], get_logp(r.chisq[e]), true); continue; }
-        if (!have) continue;
-        if (p.htp) {
-          // print_sum_stats_htp for a quantitative trait, with the genotype counts of the trait's samples.  SCORE / SKATV
-          // are the numerator and denominator of the statistic (dt_thr->scores / skat_var, src/Step2_Models.cpp:391-394,
-          // :421-424): se = scf / sqrt(denum), stat = num / sqrt(denum).
-          HtpRow hr;
-          hr.model = htp_model.c_str();
-          hr.beta = r.beta[e]; hr.se = r.se[e]; hr.chisq = r.chisq[e]; hr.logp = get_logp(r.chisq[e]); hr.af = r.af[e]; hr.mac = r.mac[e];
-          for (int k = 0; k < 3; ++k) hr.gc[k] = in.htp_cnt[b & 1][e * 6 + k];
-          if (in.use_bgen) hr.info = r.info[e];                // dosages: the trait's INFO
-          const double sqrt_den = scf[i] / r.se[e];
-          hr.score = r.stat[e] * sqrt_den; hr.skat_var = sqrt_den * sqrt_den;
-          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, hr);
-          continue;
-        }
-        append_sumstats_row(obuf[i], head_s, r.af[e], in.use_bgen, in.use_bgen ? r.info[e] : -1.0, r.ns[e], test_name(p.test_type),
-                            r.beta[e], r.se[e], r.chisq[e], get_logp(r.chisq[e]), true);   // print_sum_stats_single :2502-2540
-      }
-      if (p.no_split) w.obuf_all += " NA\n";
-    }
-    w.flush();
-    log << " block [" << b + 1 << "/" << in.blocks.size() << "] : done\n";
+// check_blup-like list of --use-null-firth (src/Step2_Models.cpp:1896-1927): the file of each trait, "" where none is named
+std::vector<std::string> read_null_firth_list(const std::string& list, const std::vector<std::string>& names) {
+  std::vector<std::string> files(names.size());
+  LineReader fr(list);
+  std::string line;
+  std::set<std::string> seen;
+  while (fr.getline(line)) {
+    const auto t = split_ws(line);
+    if (t.empty()) continue;
+    if (t.size() != 2) throw Fail("incorrectly formatted blup list file : " + list);
+    const auto it = std::find(names.begin(), names.end(), t[0]);
+    if (it == names.end()) continue;                         // unrecognised phenotypes are ignored
+    if (!seen.insert(t[0]).second) throw Fail("phenotype '" + t[0] + "' appears more than once in file.");
+    { std::ifstream probe_f(t[1]); if (!probe_f) throw Fail("file " + t[1] + " cannot be opened."); }
+    files[(size_t)(it - names.begin())] = t[1];
   }
-  w.close();
-  log << "\nNumber of ignored tests due to low MAC or low variance : " << n_ignored << "\n";
+  return files;
 }
 
-// Step 2 for binary traits (--bt [--firth --approx]) on BGEN dosages or .bed hard calls.
-// Control flow of Data::test_snps_fast for trait_mode 1 (src/Data.cpp:2230-2383): per chromosome the null
-// logistic / null Firth fits (host, O(N C^2)), per block the score test and the Firth fallback (GPU).
-void run_step2_bt(const Params& p, Log& log) {
-  S2Input in(p, true, log);
-  const Pheno& ph = in.ph;
-  const int64_t N = ph.N;
-  const int P = ph.P, C = ph.C;
-  const double z_thr = z_threshold(p.p_thresh);
-  // --htp: test_string + wgr_string + correction_type (src/Data.cpp:2075-2102)
-  const std::string htp_model = std::string(test_name(p.test_type)) + (p.ignore_pred ? "" : "-WGR") + (p.firth ? "-FIRTH" : p.spa ? "-SPA" : "-LOG");
-  if (p.firth) log << " * using approximate Firth correction for logistic regression p-values less than " << p.p_thresh << "\n";
-  std::vector<std::string> null_firth_files;                 // check_blup-like list (src/Step2_Models.cpp:1896-1927)
-  if (p.firth && !p.null_firth_list.empty()) {
-    log << " * reading null Firth estimates using file : [" << p.null_firth_list << "]\n";
-    null_firth_files.assign(P, "");
-    LineReader fr(p.null_firth_list);
-    std::string line;
-    std::set<std::string> seen;
-    while (fr.getline(line)) {
-      const auto t = split_ws(line);
-      if (t.empty()) continue;
-      if (t.size() != 2) throw Fail("incorrectly formatted blup list file : " + p.null_firth_list);
-      const auto it = std::find(ph.names.begin(), ph.names.end(), t[0]);
-      if (it == ph.names.end()) continue;                    // unrecognised phenotypes are ignored
-      if (!seen.insert(t[0]).second) throw Fail("phenotype '" + t[0] + "' appears more than once in file.");
-      { std::ifstream probe_f(t[1]); if (!probe_f) throw Fail("file " + t[1] + " cannot be opened."); }
-      null_firth_files[(size_t)(it - ph.names.begin())] = t[1];
+// get_beta_start_firth (src/Step2_Models.cpp:1936-1980): the starting values of chromosome `chrom` in a trait's null Firth
+// file; empty when it has no row for the chromosome
+std::vector<double> read_null_firth_start(const std::string& file, int chrom, int C) {
+  std::vector<double> start;
+  LineReader fr(file);
+  std::string line;
+  while (fr.getline(line)) {
+    const auto t = split_ws(line);
+    if (t.empty()) throw Fail("error reading null firth estimates file");
+    if (chr_str_to_int(t[0]) != chrom) continue;
+    if ((int)t.size() - 1 > C) throw Fail("file has more predictors than included in analysis (=" + std::to_string(t.size()) + " vs " + std::to_string(C) + ")");
+    for (size_t j = 1; j < t.size(); ++j) {
+      const double v = convert_double(t[j]);
+      if (v == kMissing) throw Fail("no missing values allowed in file");
+      start.push_back(v);
     }
+    break;
   }
-  if (p.spa) log << " * using SPA correction for logistic regression p-values less than " << p.p_thresh << "\n";
-
-  rg_handle h = nullptr;
-  HandleGuard guard{h};
-  require_device();
-  in.create_handle(ph.mask.data(), ph.strict, &h);
-
-  S2Writers w;
-  w.open(p, ph, in.use_bgen);
-  std::vector<std::string>& obuf = w.obuf;                   // rows of the current block, one buffer per trait
-  std::string head_s;
-  GenoCounts gc(p.no_split, p.bsize, P, in.use_bgen ? 0 : in.g.row_stride, p.ref_first);
-  // --af-cc (update_af_cc / compute_aaf_info, src/Geno.cpp:3069-3075, :3120-3127): a second handle whose sample masks are
-  // the cases of each trait returns their allele frequency and count from the same block bytes; controls follow by
-  // difference of the (exactly reconstructed) allele sums.
-  rg_handle hc = nullptr;
-  HandleGuard guard_cases{hc};
-  S2Results rc;
-  if (p.af_cc) {
-    std::vector<uint8_t> mask_case(ph.mask.size());
-    for (size_t e = 0; e < mask_case.size(); ++e) mask_case[e] = ph.mask[e] && ph.Y_raw[e] == 1.0;
-    in.create_handle(mask_case.data(), false, &hc);          // not strict: per-trait masks differ from the analysis set here
-    const std::vector<double> zero((size_t)N * P, 0.0), one(P, 1.0);
-    rg_check(rg_s2_set_chr(hc, zero.data(), one.data()));
-    rc.init(p.bsize, P);
-  }
-  const rg_s2_out outc = rc.out();
-  const double unit = in.use_bgen ? 255.0 : 1.0;             // allele sums are multiples of 1 / unit
-  in.start(log);
-  S2Results r, r2;                                           // r2: counts of the --test recode pass, see run_step2_qt
-  r.init(p.bsize, P);
-  if (p.test_type) r2.init(p.bsize, P);
-  const rg_s2_out out = r.out(), out2 = r2.out(r);
-  const Recode recode(p.test_type, p.ref_first);
-  int cur_chr = -1;
-  size_t n_ignored = 0, n_firth = 0, n_fail = 0;
-  for (size_t b = in.b_first; b < in.blocks.size(); ++b) {
-    const int chrom = in.blocks[b].chrom, bs = in.blocks[b].size;
-    if (chrom != cur_chr) {
-      cur_chr = chrom;
-      log << "Chromosome " << chrom << "\n";
-      std::vector<double> gsm((size_t)P * N), gs((size_t)P * N), yres((size_t)P * N), xg((size_t)P * C * N), off, yhat;
-      if (p.firth) off.resize((size_t)P * N);
-      if (p.spa) yhat.resize((size_t)P * N);
-      for (int i = 0; i < P; ++i) {
-        const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
-        // --use-null-firth: starting values of this chromosome from the Step-1 file (get_beta_start_firth, :1936-1980)
-        std::vector<double> fstart;
-        if (p.firth && !null_firth_files.empty() && !null_firth_files[i].empty()) {
-          LineReader fr(null_firth_files[i]);
-          std::string line;
-          while (fr.getline(line)) {
-            const auto t = split_ws(line);
-            if (t.empty()) throw Fail("error reading null firth estimates file");
-            if (chr_str_to_int(t[0]) != chrom) continue;
-            if ((int)t.size() - 1 > C) throw Fail("file has more predictors than included in analysis (=" + std::to_string(t.size()) + " vs " + std::to_string(C) + ")");
-            for (size_t j = 1; j < t.size(); ++j) {
-              const double v = convert_double(t[j]);
-              if (v == kMissing) throw Fail("no missing values allowed in file");
-              fstart.push_back(v);
-            }
-            break;
-          }
-        }
-        const BtNull nm = fit_bt_null(ph.names[i], &ph.Y_raw[(size_t)i * N], ph.X.data(), N, C, blup.data(),
-                                      &ph.mask[(size_t)i * N], p.firth, fstart.empty() ? nullptr : &fstart);
-        std::copy(nm.gamma_sqrt_mask.begin(), nm.gamma_sqrt_mask.end(), gsm.begin() + (size_t)i * N);
-        std::copy(nm.gamma_sqrt.begin(), nm.gamma_sqrt.end(), gs.begin() + (size_t)i * N);
-        std::copy(nm.yres.begin(), nm.yres.end(), yres.begin() + (size_t)i * N);
-        std::copy(nm.x_gamma.begin(), nm.x_gamma.end(), xg.begin() + (size_t)i * C * N);
-        if (p.firth) std::copy(nm.firth_offset.begin(), nm.firth_offset.end(), off.begin() + (size_t)i * N);
-        if (p.spa) std::copy(nm.y_hat_p.begin(), nm.y_hat_p.end(), yhat.begin() + (size_t)i * N);
-      }
-      rg_check(rg_s2_set_sex(h, chrom == 23 ? in.male.data() : nullptr));
-      rg_s2_bt_chr st{gsm.data(), gs.data(), yres.data(), xg.data(), ph.Y_raw.data(), p.firth ? off.data() : nullptr,
-                      p.spa ? yhat.data() : nullptr};
-      rg_check(rg_s2_set_chr_bt(h, &st));
-    }
-    in.next(b);
-    if (!in.use_bgen)
-      gc.run(in.rows[b & 1].data(), (size_t)bs * in.g.row_stride, bs, [&](const uint8_t* rw, const rg_s2_out* o) {
-        rg_check(rg_s2_block_bed_bt(h, rw, (int64_t)in.g.row_stride, bs, in.sidx(), p.ref_first, 0.0, o));
-      });
-    in.set_non_par(h, b);
-    if (in.use_bgen) {
-      const uint8_t *pd, *md;
-      in.dosages(h, b, &pd, &md);
-      rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, p.min_mac, &out, r.info.data()));
-      if (hc) rg_check(rg_s2_block_bgen8(hc, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &outc, rc.info.data()));
-      if (p.test_type) {
-        in.recode(recode, b);
-        rg_check(rg_s2_block_bgen8_bt(h, pd, md, (int64_t)in.n_file, bs, in.sidx(), p.ref_first, 0.0, &out2, r2.info.data()));
-      }
-    } else {
-      const uint8_t* rows;
-      int64_t stride;
-      in.hard_calls(h, b, &rows, &stride);
-      rg_check(rg_s2_block_bed_bt(h, rows, stride, bs, in.sidx(), p.ref_first, p.min_mac, &out));
-      if (hc) rg_check(rg_s2_block_bed(hc, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &outc));
-      if (p.test_type) {
-        in.recode(recode, b);
-        rg_check(rg_s2_block_bed_bt(h, rows, stride, bs, in.sidx(), p.ref_first, 0.0, &out2));
-      }
-    }
-    if (p.test_type) merge_recode_flags(bs, r.flags.data(), r2.flags.data(), r2.af_all.data());
-    if (in.use_info1)                                        // ignored_snp: counts as one ignored variant, no Firth / SPA
-      for (int v = 0; v < bs; ++v) if (p.min_info > 0 && in.info1[b & 1][v] < p.min_info) r.flags[v] |= 1;
-    // Firth fallback for |z| above the --pThresh threshold (check_pval_snp, src/Step2_Models.cpp:1988-2041)
-    std::vector<int32_t> sel_v, sel_t, fstatus;
-    std::vector<double> fbeta, fse, flrt;
-    std::map<std::pair<int, int>, int> fidx;
-    std::map<std::pair<int, int>, double> spa_logp;
-    if (p.firth || p.spa) {
-      for (int v = 0; v < bs; ++v) {
-        if (r.flags[v] & (1 | 16)) continue;
-        for (int i = 0; i < P; ++i) {
-          const size_t e = (size_t)v * P + i;
-          if (r.mac[e] < p.min_mac || !(std::fabs(r.stat[e]) > z_thr)) continue;
-          fidx[{v, i}] = (int)sel_v.size();
-          sel_v.push_back(v); sel_t.push_back(i);
-        }
-      }
-      const size_t nsel = sel_v.size();
-      fbeta.resize(nsel); fse.resize(nsel); flrt.resize(nsel); fstatus.resize(nsel);
-      if (p.firth) {
-        rg_check(rg_s2_firth(h, (int32_t)nsel, sel_v.data(), sel_t.data(), fbeta.data(), fse.data(), flrt.data(), fstatus.data()));
-      } else {
-        // check_pval_snp, SPA branch (src/Step2_Models.cpp:2021-2029): SE from the score test, beta from the SPA chi-square
-        std::vector<double> pv(nsel);
-        rg_check(rg_s2_spa(h, (int32_t)nsel, sel_v.data(), sel_t.data(), pv.data(), fstatus.data()));
-        for (size_t k = 0; k < nsel; ++k) {
-          const size_t e = (size_t)sel_v[k] * P + sel_t[k];
-          const double pval = std::max(10.0 * std::numeric_limits<double>::min(), pv[k]);
-          flrt[k] = chisq1_from_pvalue(pval);
-          fse[k] = r.se[e];
-          fbeta[k] = (r.beta[e] < 0 ? -1.0 : 1.0) * std::sqrt(flrt[k]) * r.se[e];
-          spa_logp[{sel_v[k], sel_t[k]}] = -std::log10(pval);
-        }
-      }
-      n_firth += nsel;
-    }
-    for (int v = 0; v < bs; ++v) {
-      if (r.flags[v] & (1 | 16)) { ++n_ignored; continue; }
-      s2_row_start(in, b, v, r, gc, w, head_s);
-      for (int i = 0; i < P; ++i) {
-        const size_t e = (size_t)v * P + i;
-        const bool have = !(r.mac[e] < p.min_mac) && !(in.use_bgen && r.info[e] < p.min_info);   // ignored_trait, --minINFO
-        if (!have) {
-          if (p.no_split) append_sumstats_all_trait(w.obuf_all, false, 0, 0, 0, 0, false);
-          continue;
-        }
-        double bo = r.beta[e], so = r.se[e], co = r.chisq[e];
-        bool pass = true;
-        auto f = fidx.find({v, i});
-        if (f != fidx.end()) {
-          if ((fstatus[f->second] & 15) == 0) { bo = fbeta[f->second]; so = fse[f->second]; co = flrt[f->second]; }
-          else { pass = false; ++n_fail; }
-        }
-        double lp = get_logp(co);
-        if (p.spa && pass && f != fidx.end()) lp = spa_logp[{v, i}];   // SPA reports -log10 of its own p-value
-        AfCc cc;
-        if (hc) {
-          const double s_all = std::round(r.af[e] * 2.0 * r.ns[e] * unit), s_case = std::round(rc.af[e] * 2.0 * rc.ns[e] * unit);
-          cc.ns_case = rc.ns[e];
-          cc.ns_control = r.ns[e] - rc.ns[e];
-          cc.af_case = rc.af[e];
-          cc.af_control = (s_all - s_case) / unit / (2.0 * cc.ns_control);
-        }
-        if (p.htp) {
-          // print_sum_stats_htp for a binary trait (src/Step2_Models.cpp:2542-2646), with the genotype counts of the
-          // trait's cases and controls.  SCORE / SKATV (compute_score_bt :523-526, :546): stats * sqrt(denum) with the
-          // sign of the minor-allele flip undone, and denum = 1 / se^2 of the score test; cal_factor (check_pval_snp
-          // :1993, :2027) = 1 without a correction, stats^2 / corrected chi-square with one.  After a FAILED correction
-          // the reference prints whatever cal_factor the thread held before (it returns before the assignment): 1 here.
-          HtpRow hr;
-          hr.model = htp_model.c_str(); hr.bt = true; hr.firth = p.firth;
-          hr.beta = bo; hr.se = so; hr.chisq = co; hr.logp = lp; hr.af = r.af[e]; hr.mac = r.mac[e]; hr.test_pass = pass;
-          for (int k = 0; k < 6; ++k) hr.gc[k] = in.htp_cnt[b & 1][e * 6 + k];
-          if (in.use_bgen) hr.info = r.info[e];                // dosages: the trait's INFO
-          const double sqrt_den = 1.0 / r.se[e];
-          hr.score = r.stat[e] * sqrt_den * ((r.flags[v] & 8) ? -1.0 : 1.0); hr.skat_var = sqrt_den * sqrt_den;
-          hr.cal_factor = (f != fidx.end() && pass) ? (co == 0 ? 0.0 : r.stat[e] * r.stat[e] / co) : 1.0;
-          append_htp_row(obuf[i], head_s, ph.names[i], p.htp_cohort, hr);
-          continue;
-        }
-        if (p.no_split) append_sumstats_all_trait(w.obuf_all, true, bo, so, co, lp, pass);
-        else append_sumstats_row(obuf[i], head_s, r.af[e], in.use_bgen, in.use_bgen ? r.info[e] : -1.0, r.ns[e], test_name(p.test_type),
-                                 bo, so, co, lp, pass, (hc && p.af_cc) ? &cc : nullptr);
-      }
-      if (p.no_split) w.obuf_all += " NA\n";
-    }
-    w.flush();
-    log << " block [" << b + 1 << "/" << in.blocks.size() << "] : done\n";
-  }
-  w.close();
-  log << "\nNumber of ignored tests due to low MAC or low variance : " << n_ignored << "\n";
-  if (p.firth) log << "Number of tests with Firth correction : " << n_firth << " (" << n_fail << " failed)\n";
-  if (p.spa) log << "Number of tests with SPA correction : " << n_firth << " (" << n_fail << " failed)\n";
+  return start;
 }
 
-void run_step2(const Params& p_in, Log& log) {
-  Params p = p_in;
+// the options Step 2 switches off
+Params step2_options(Params p, Log& log) {
   if (p.af_cc && (!p.bt || p.no_split)) {                    // src/Regenie.cpp:1076-1079
     log << "WARNING: disabling option --af-cc (only for BTs in step 2 in native output format split by trait).\n";
     p.af_cc = false;
   }
   if (p.htp) p.af_cc = false;                                // HTP rows carry genotype counts, not the --af-cc columns
-  if (p.bt) run_step2_bt(p, log); else run_step2_qt(p, log);
+  return p;
+}
+
+// Step 2 (Data::test_snps_fast, src/Data.cpp:2230-2383) for either trait kind as phases over one state; run_step2 lists
+// them.  Per chromosome: the residuals of a quantitative trait, the null logistic / null Firth fits of a binary one (host,
+// O(N C^2)).  Per block: the score tests (GPU) and, for a binary trait, the Firth or SPA correction (GPU).
+struct Step2 {
+  // the test of one (variant, trait) as its row prints it: the score test, or its Firth / SPA correction
+  struct Test {
+    bool have = false, pass = true, corrected = false;
+    double beta = 0, se = 0, chisq = 0, logp = 0;
+    AfCc cc;                                                 // --af-cc
+  };
+  const Params p;
+  Log& log;
+  S2Input in;
+  const Pheno& ph;
+  const bool binary;
+  const int64_t N;
+  const int P;
+  rg_handle h = nullptr, hc = nullptr;                       // hc: --af-cc, sample masks = the cases of each trait
+  HandleGuard guard{h}, guard_cases{hc};
+  S2Writers w;
+  GenoCounts gc;
+  const Recode recode;
+  S2Results r, r2, rc;                                       // r2: the --test recode pass (see Recode); rc: the cases, on hc
+  const std::string htp_model;                               // --htp: test_string + wgr_string + correction_type (src/Data.cpp:2075-2102)
+  std::vector<std::string> null_firth;                       // --use-null-firth: the file of each trait, or ""
+  std::vector<double> scf;                                   // quantitative traits: scale of the residuals (BETA, --htp SKATV)
+  std::vector<Test> t;                                       // [bs][P] of the current block
+  std::string head_s;
+  size_t n_ignored = 0, n_corr = 0, n_fail = 0;
+
+  Step2(const Params& p_in, Log& log_)
+      : p(step2_options(p_in, log_)), log(log_), in(p, p.bt, log_), ph(in.ph), binary(p.bt), N(ph.N), P(ph.P),
+        gc(p.no_split, p.bsize, P, in.use_bgen ? 0 : in.g.row_stride, p.ref_first), recode(p.test_type, p.ref_first),
+        htp_model(std::string(test_name(p.test_type)) + (p.ignore_pred ? "" : "-WGR") + (!binary ? "-LR" : p.firth ? "-FIRTH" : p.spa ? "-SPA" : "-LOG")) {
+    if (binary && p.firth) log << " * using approximate Firth correction for logistic regression p-values less than " << p.p_thresh << "\n";
+    if (binary && p.firth && !p.null_firth_list.empty()) {
+      log << " * reading null Firth estimates using file : [" << p.null_firth_list << "]\n";
+      null_firth = read_null_firth_list(p.null_firth_list, ph.names);
+    }
+    if (binary && p.spa) log << " * using SPA correction for logistic regression p-values less than " << p.p_thresh << "\n";
+  }
+
+  // the handles, the output files and the fetch of the first block
+  void open() {
+    require_device();
+    in.create_handle(ph.mask.data(), ph.strict, &h);
+    w.open(p, ph, in.use_bgen);
+    // --af-cc (update_af_cc / compute_aaf_info, src/Geno.cpp:3069-3075, :3120-3127): a second handle whose sample masks
+    // are the cases of each trait returns their allele frequency and count from the same block bytes; controls follow by
+    // difference of the (exactly reconstructed) allele sums.
+    if (p.af_cc) {
+      std::vector<uint8_t> mask_case(ph.mask.size());
+      for (size_t e = 0; e < mask_case.size(); ++e) mask_case[e] = ph.mask[e] && ph.Y_raw[e] == 1.0;
+      in.create_handle(mask_case.data(), false, &hc);        // not strict: per-trait masks differ from the analysis set here
+      const std::vector<double> zero((size_t)N * P, 0.0), one(P, 1.0);
+      rg_check(rg_s2_set_chr(hc, zero.data(), one.data()));
+      rc.init(p.bsize, P);
+    }
+    in.start(log);
+    r.init(p.bsize, P);
+    if (p.test_type) r2.init(p.bsize, P);
+  }
+
+  void chromosome(int chrom) {
+    log << "Chromosome " << chrom << "\n";
+    if (binary) null_fits(chrom); else residuals(chrom);
+  }
+  void set_sex(int chrom) { rg_check(rg_s2_set_sex(h, chrom == 23 ? in.male.data() : nullptr)); }
+
+  // blup_read_chr + compute_res (src/Step2_Models.cpp:96-124, src/Data.cpp:2386-2404)
+  void residuals(int chrom) {
+    std::vector<double> res((size_t)N * P);
+    scf.resize(P);
+    for (int i = 0; i < P; ++i) {
+      const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
+      double ssq = 0.0;
+      for (int64_t s = 0; s < N; ++s) {
+        const double rv = (ph.Y[(size_t)i * N + s] - blup[s]) * ph.mask[(size_t)i * N + s];
+        res[(size_t)i * N + s] = rv;
+        ssq += rv * rv;
+      }
+      const double psd = std::sqrt(ssq) / std::sqrt(ph.neff[i] - ph.C);
+      for (int64_t s = 0; s < N; ++s) res[(size_t)i * N + s] /= psd;
+      scf[i] = ph.scale_Y[i] * psd;
+    }
+    set_sex(chrom);
+    rg_check(rg_s2_set_chr(h, res.data(), scf.data()));
+  }
+
+  void null_fits(int chrom) {
+    const int C = ph.C;
+    std::vector<double> gsm((size_t)P * N), gs((size_t)P * N), yres((size_t)P * N), xg((size_t)P * C * N), off, yhat;
+    if (p.firth) off.resize((size_t)P * N);
+    if (p.spa) yhat.resize((size_t)P * N);
+    for (int i = 0; i < P; ++i) {
+      const std::vector<double> blup = blup_for_chr(in.locos[i], in.ss, ph, i, chrom);
+      const std::vector<double> fstart = null_firth.empty() || null_firth[i].empty() ? std::vector<double>() : read_null_firth_start(null_firth[i], chrom, C);
+      const BtNull nm = fit_bt_null(ph.names[i], &ph.Y_raw[(size_t)i * N], ph.X.data(), N, C, blup.data(),
+                                    &ph.mask[(size_t)i * N], p.firth, fstart.empty() ? nullptr : &fstart);
+      std::copy(nm.gamma_sqrt_mask.begin(), nm.gamma_sqrt_mask.end(), gsm.begin() + (size_t)i * N);
+      std::copy(nm.gamma_sqrt.begin(), nm.gamma_sqrt.end(), gs.begin() + (size_t)i * N);
+      std::copy(nm.yres.begin(), nm.yres.end(), yres.begin() + (size_t)i * N);
+      std::copy(nm.x_gamma.begin(), nm.x_gamma.end(), xg.begin() + (size_t)i * C * N);
+      if (p.firth) std::copy(nm.firth_offset.begin(), nm.firth_offset.end(), off.begin() + (size_t)i * N);
+      if (p.spa) std::copy(nm.y_hat_p.begin(), nm.y_hat_p.end(), yhat.begin() + (size_t)i * N);
+    }
+    set_sex(chrom);
+    rg_s2_bt_chr st{gsm.data(), gs.data(), yres.data(), xg.data(), ph.Y_raw.data(), p.firth ? off.data() : nullptr,
+                    p.spa ? yhat.data() : nullptr};
+    rg_check(rg_s2_set_chr_bt(h, &st));
+  }
+
+  // The block calls of block b.  Their order is part of the results: the library applies rg_s2_set_non_par to the next
+  // call on h, so the --no-split counts run before it, and Firth / SPA read the block the last call on h left resident.
+  void passes(size_t b) {
+    const int bs = in.blocks[b].size;
+    in.next(b);
+    if (!in.use_bgen)
+      gc.run(in.rows[b & 1].data(), (size_t)bs * in.g.row_stride, bs, [&](const uint8_t* rw, const rg_s2_out* o) {
+        in.test(h, binary, {rw, nullptr, (int64_t)in.g.row_stride, bs}, 0.0, *o, nullptr);
+      });
+    in.set_non_par(h, b);
+    const S2Input::Rows k = in.block(h, b);
+    in.test(h, binary, k, p.min_mac, r.out(), r.info.data());
+    if (hc) in.test(hc, false, k, 0.0, rc.out(), rc.info.data());
+    if (p.test_type) {
+      in.recode(recode, b);
+      in.test(h, binary, k, 0.0, r2.out(r), r2.info.data());
+      merge_recode_flags(bs, r.flags.data(), r2.flags.data(), r2.af_all.data());
+    }
+    // --minINFO (src/Geno.cpp:2074): the variant is ignored (counted once, no Firth / SPA), as a MAC failure is
+    if (in.use_info1 && p.min_info > 0)
+      for (int v = 0; v < bs; ++v) if (in.info1[b & 1][v] < p.min_info) r.flags[v] |= 1;
+  }
+
+  // no row, no correction: bit 0 (MAC, --minINFO) of either trait kind, bit 1 (scale_fac) of the quantitative routes and
+  // bit 4 (score denominator) of the binary ones; neither kind's routes set the other's bit, so one mask serves both
+  static bool ignored(int32_t flags) { return flags & (1 | 2 | 16); }
+
+  void tests(int bs) {
+    t.assign((size_t)bs * P, Test());
+    for (size_t e = 0; e < t.size(); ++e) {
+      Test& x = t[e];
+      x.have = !(r.mac[e] < p.min_mac) && !(in.use_bgen && r.info[e] < p.min_info);   // ignored_trait (src/Geno.cpp:3102), --minINFO (:3142-3146)
+      x.beta = r.beta[e]; x.se = r.se[e]; x.chisq = r.chisq[e]; x.logp = get_logp(x.chisq);
+      if (!hc) continue;
+      const double unit = in.use_bgen ? 255.0 : 1.0;         // allele sums are multiples of 1 / unit
+      const double s_all = std::round(r.af[e] * 2.0 * r.ns[e] * unit), s_case = std::round(rc.af[e] * 2.0 * rc.ns[e] * unit);
+      x.cc.ns_case = rc.ns[e];
+      x.cc.ns_control = r.ns[e] - rc.ns[e];
+      x.cc.af_case = rc.af[e];
+      x.cc.af_control = (s_all - s_case) / unit / (2.0 * x.cc.ns_control);
+    }
+    if (binary && (p.firth || p.spa)) correct(bs);
+  }
+
+  // Firth or SPA for |z| above the --pThresh threshold (check_pval_snp, src/Step2_Models.cpp:1988-2041)
+  void correct(int bs) {
+    const double z_thr = z_threshold(p.p_thresh);
+    std::vector<int32_t> sel_v, sel_t;
+    for (int v = 0; v < bs; ++v) {
+      if (ignored(r.flags[v])) continue;
+      for (int i = 0; i < P; ++i) {
+        const size_t e = (size_t)v * P + i;
+        if (r.mac[e] < p.min_mac || !(std::fabs(r.stat[e]) > z_thr)) continue;
+        sel_v.push_back(v); sel_t.push_back(i);
+      }
+    }
+    const size_t nsel = sel_v.size();
+    std::vector<double> fbeta(nsel), fse(nsel), flrt(nsel), pv(nsel);
+    std::vector<int32_t> fstatus(nsel);
+    if (p.firth) rg_check(rg_s2_firth(h, (int32_t)nsel, sel_v.data(), sel_t.data(), fbeta.data(), fse.data(), flrt.data(), fstatus.data()));
+    else rg_check(rg_s2_spa(h, (int32_t)nsel, sel_v.data(), sel_t.data(), pv.data(), fstatus.data()));
+    for (size_t k = 0; k < nsel; ++k) {
+      Test& x = t[(size_t)sel_v[k] * P + sel_t[k]];
+      x.corrected = true;
+      x.pass = (fstatus[k] & 15) == 0;
+      if (!x.pass) continue;
+      if (p.firth) { x.beta = fbeta[k]; x.se = fse[k]; x.chisq = flrt[k]; x.logp = get_logp(x.chisq); continue; }
+      // check_pval_snp, SPA branch (src/Step2_Models.cpp:2021-2029): SE from the score test, beta from the SPA chi-square,
+      // and -log10 of SPA's own p-value
+      const double pval = std::max(10.0 * std::numeric_limits<double>::min(), pv[k]);
+      x.chisq = chisq1_from_pvalue(pval);
+      x.beta = (x.beta < 0 ? -1.0 : 1.0) * std::sqrt(x.chisq) * x.se;
+      x.logp = -std::log10(pval);
+    }
+    n_corr += nsel;
+  }
+
+  void write_rows(size_t b) {
+    for (int v = 0; v < in.blocks[b].size; ++v) {
+      if (ignored(r.flags[v])) { ++n_ignored; continue; }
+      s2_row_start(in, b, v, r, gc, w, head_s);
+      for (int i = 0; i < P; ++i) {
+        const size_t e = (size_t)v * P + i;
+        const Test& x = t[e];
+        n_fail += x.have && !x.pass;
+        if (p.no_split) { append_sumstats_all_trait(w.obuf_all, x.have, x.beta, x.se, x.chisq, x.logp, x.pass); continue; }
+        if (!x.have) continue;
+        if (p.htp) {
+          // print_sum_stats_htp (src/Step2_Models.cpp:2542-2646) with the genotype counts of the trait's samples (of its
+          // cases and controls apart for a binary trait).  SCORE / SKATV are the numerator and denominator of the statistic
+          // (:391-394, :421-424; compute_score_bt :523-526, :546): stat * sqrt(denum), se = scf / sqrt(denum) (scf = 1 for
+          // a binary trait), with the sign of the minor-allele flip undone (bit 3, binary routes only).  cal_factor
+          // (check_pval_snp :1993, :2027) of a binary trait = 1 without a correction, stats^2 / corrected chi-square with
+          // one; after a FAILED correction the reference prints whatever cal_factor the thread held before (it returns
+          // before the assignment): 1 here.  A quantitative trait keeps the default, which prints the same SKATV.
+          HtpRow hr;
+          hr.model = htp_model.c_str(); hr.bt = binary; hr.firth = p.firth;
+          hr.beta = x.beta; hr.se = x.se; hr.chisq = x.chisq; hr.logp = x.logp; hr.af = r.af[e]; hr.mac = r.mac[e]; hr.test_pass = x.pass;
+          for (int k = 0; k < 6; ++k) hr.gc[k] = in.htp_cnt[b & 1][e * 6 + k];   // the controls' 3..5 print for a binary trait only
+          if (in.use_bgen) hr.info = r.info[e];                // dosages: the trait's INFO
+          const double sqrt_den = (binary ? 1.0 : scf[i]) / r.se[e];
+          hr.score = r.stat[e] * sqrt_den * ((r.flags[v] & 8) ? -1.0 : 1.0); hr.skat_var = sqrt_den * sqrt_den;
+          if (binary) hr.cal_factor = (x.corrected && x.pass) ? (x.chisq == 0 ? 0.0 : r.stat[e] * r.stat[e] / x.chisq) : 1.0;
+          append_htp_row(w.obuf[i], head_s, ph.names[i], p.htp_cohort, hr);
+          continue;
+        }
+        append_sumstats_row(w.obuf[i], head_s, r.af[e], in.use_bgen, in.use_bgen ? r.info[e] : -1.0, r.ns[e], test_name(p.test_type),
+                            x.beta, x.se, x.chisq, x.logp, x.pass, hc ? &x.cc : nullptr);   // print_sum_stats_single :2502-2540
+      }
+      if (p.no_split) w.obuf_all += " NA\n";
+    }
+    w.flush();
+    log << " block [" << b + 1 << "/" << in.blocks.size() << "] : done\n";
+  }
+
+  void close() {
+    w.close();
+    log << "\nNumber of ignored tests due to low MAC or low variance : " << n_ignored << "\n";
+    if (binary && p.firth) log << "Number of tests with Firth correction : " << n_corr << " (" << n_fail << " failed)\n";
+    if (binary && p.spa) log << "Number of tests with SPA correction : " << n_corr << " (" << n_fail << " failed)\n";
+  }
+};
+
+void run_step2(const Params& p, Log& log) {
+  Step2 s(p, log);                 // the options, the genotype file, the phenotypes and predictions, the null Firth list
+  s.open();
+  int cur_chr = -1;
+  for (size_t b = s.in.b_first; b < s.in.blocks.size(); ++b) {
+    if (s.in.blocks[b].chrom != cur_chr) s.chromosome(cur_chr = s.in.blocks[b].chrom);
+    s.passes(b);
+    s.tests(s.in.blocks[b].size);
+    s.write_rows(b);
+  }
+  s.close();
 }
 
 }  // namespace

@@ -35,6 +35,7 @@ struct rg_ctx {
   std::vector<uint32_t> pgen_rows;
   std::vector<uint8_t> stage[4];                               // rg_s2_stage slots (host copies)
   int last_bs = 0;
+  int ordinal = 0;                                             // creation order of the handles, from 1 (RG_MOCK_TRACE)
   bool qt_chr = false, bt_chr = false;                         // rg_s2_set_chr / rg_s2_set_chr_bt has run
 };
 
@@ -42,6 +43,25 @@ namespace {
 thread_local std::string g_err;                               // one driver thread per device: errors stay with their thread
 std::mutex g_W_mu;                                            // level-0 slabs of a phenotype land in its owner's W
 int fail(const std::string& m) { g_err = m; return 1; }
+
+// RG_MOCK_TRACE=<file>: one line per Step-2 entry point - its name, the handle's creation ordinal, bs or n_sel, min_mac, the
+// non-PAR flags pending on the handle, and for the set_* calls a checksum of the bytes uploaded - so that a driver change
+// can be checked for the calls it makes, their order and their handle, which the output files alone do not show
+std::mutex g_trace_mu;
+int g_handles = 0;
+uint64_t fnv(const void* p, size_t n, uint64_t s = 1469598103934665603ull) {
+  for (size_t i = 0; i < n; ++i) s = (s ^ ((const uint8_t*)p)[i]) * 1099511628211ull;
+  return s;
+}
+void trace(const char* name, const rg_ctx* h, long n, double min_mac = -1, uint64_t sum = 0) {
+  static const char* path = getenv("RG_MOCK_TRACE");
+  if (!path) return;
+  std::lock_guard<std::mutex> lk(g_trace_mu);
+  if (FILE* f = fopen(path, "a")) {                           // opened per line: the driver leaves through _exit
+    fprintf(f, "%s %d %ld %g %zu %016llx\n", name, h ? h->ordinal : 0, n, min_mac, h ? h->nonpar.size() : 0, (unsigned long long)sum);
+    fclose(f);
+  }
+}
 
 // PLINK 1 code -> ALT-allele count as the driver's kernels see it (ref-last): 00 -> 2, 01 -> missing, 10 -> 1, 11 -> 0
 inline int bed_call(const uint8_t* row, int64_t s) {
@@ -128,6 +148,7 @@ int rg_sync(rg_handle) { return 0; }
 int rg_step1_create(const rg_step1_config* cfg, const double*, const double* Y, const uint8_t* mask, const uint8_t* in_analysis,
                     const int64_t*, const double*, const double*, rg_handle* out) {
   rg_ctx* h = new rg_ctx;
+  h->ordinal = ++g_handles;
   h->kind = 1; h->N = cfg->n_samples; h->P = cfg->n_pheno; h->C = cfg->n_cov; h->K = cfg->n_folds; h->R = cfg->n_ridge_l0;
   h->R1 = cfg->n_ridge_l1; h->nb = cfg->total_blocks; h->bs_max = cfg->max_block_size;
   h->Y.assign(Y, Y + (size_t)h->N * h->P);
@@ -261,25 +282,39 @@ int rg_prs(rg_handle h, double* out) {
 // ------------------------------------------------------------------ step 2
 int rg_step2_create(const rg_step2_config* cfg, const double*, const uint8_t* mask, const uint8_t* in_analysis, rg_handle* out) {
   rg_ctx* h = new rg_ctx;
+  h->ordinal = ++g_handles;
   h->kind = 2; h->N = cfg->n_samples; h->P = cfg->n_pheno; h->C = cfg->n_cov; h->bs_max = cfg->max_block_size;
   h->mask.assign(mask, mask + (size_t)h->N * h->P);
   h->in_analysis.assign(in_analysis, in_analysis + h->N);
   h->last_stat.assign((size_t)h->bs_max * h->P, 0.0);
+  trace("rg_step2_create", h, h->bs_max, -1, fnv(mask, (size_t)h->N * h->P));
   *out = h;
   return 0;
 }
 int rg_s2_set_chr(rg_handle h, const double* res, const double* scf) {
+  trace("rg_s2_set_chr", h, 0, -1, fnv(scf, (size_t)h->P * 8, fnv(res, (size_t)h->N * h->P * 8)));
   h->res.assign(res, res + (size_t)h->N * h->P);
   h->scf.assign(scf, scf + h->P);
   h->qt_chr = true;
   return 0;
 }
 int rg_s2_set_sex(rg_handle h, const uint8_t* male) {
+  trace("rg_s2_set_sex", h, male ? h->N : 0, -1, male ? fnv(male, h->N) : 0);
   if (male) h->male.assign(male, male + h->N); else h->male.clear();
   return 0;
 }
-int rg_s2_set_non_par(rg_handle h, const uint8_t* flags, int32_t n) { h->nonpar.assign(flags, flags + n); return 0; }
+int rg_s2_set_non_par(rg_handle h, const uint8_t* flags, int32_t n) {
+  trace("rg_s2_set_non_par", h, n, -1, fnv(flags, n));
+  h->nonpar.assign(flags, flags + n);
+  return 0;
+}
 int rg_s2_set_chr_bt(rg_handle h, const rg_s2_bt_chr* st) {
+  const size_t NP = (size_t)h->N * h->P * 8;
+  uint64_t sum = fnv(st->yres, NP, fnv(st->gamma_sqrt, NP, fnv(st->gamma_sqrt_mask, NP)));
+  sum = fnv(st->y_raw, NP, fnv(st->x_gamma, NP * h->C, sum));
+  if (st->firth_offset) sum = fnv(st->firth_offset, NP, sum);
+  if (st->y_hat_p) sum = fnv(st->y_hat_p, NP, sum);
+  trace("rg_s2_set_chr_bt", h, 0, -1, sum);
   h->res.assign(st->yres, st->yres + (size_t)h->N * h->P);
   for (size_t e = 0; e < h->res.size(); ++e) h->res[e] *= 25.0 * st->gamma_sqrt_mask[e];   // enough |z| > threshold cases
   h->scf.assign(h->P, 1.0);
@@ -311,21 +346,26 @@ static int block_bgen8(rg_handle h, bool bt, const uint8_t* probs, const uint8_t
 }
 int rg_s2_block_bed(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
                     double min_mac, const rg_s2_out* o) {
+  trace("rg_s2_block_bed", h, bs, min_mac);
   return block_bed(h, false, packed, row_stride, bs, sample_idx, ref_first, min_mac, o);
 }
 int rg_s2_block_bed_bt(rg_handle h, const uint8_t* packed, int64_t row_stride, int32_t bs, const int32_t* sample_idx, int32_t ref_first,
                        double min_mac, const rg_s2_out* o) {
+  trace("rg_s2_block_bed_bt", h, bs, min_mac);
   return block_bed(h, true, packed, row_stride, bs, sample_idx, ref_first, min_mac, o);
 }
 int rg_s2_block_bgen8(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
                       int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
+  trace("rg_s2_block_bgen8", h, bs, min_mac);
   return block_bgen8(h, false, probs, pm, n_file, bs, sample_idx, ref_first, min_mac, o, info);
 }
 int rg_s2_block_bgen8_bt(rg_handle h, const uint8_t* probs, const uint8_t* pm, int64_t n_file, int32_t bs, const int32_t* sample_idx,
                          int32_t ref_first, double min_mac, const rg_s2_out* o, double* info) {
+  trace("rg_s2_block_bgen8_bt", h, bs, min_mac);
   return block_bgen8(h, true, probs, pm, n_file, bs, sample_idx, ref_first, min_mac, o, info);
 }
 int rg_s2_firth(rg_handle h, int32_t n, const int32_t* vi, const int32_t* ti, double* beta, double* se, double* lrt, int32_t* status) {
+  trace("rg_s2_firth", h, n);
   for (int k = 0; k < n; ++k) {
     if (vi[k] < 0 || vi[k] >= h->last_bs || ti[k] < 0 || ti[k] >= h->P) return fail("mock: bad Firth selection");
     const double z = h->last_stat[(size_t)vi[k] * h->P + ti[k]];
@@ -335,6 +375,7 @@ int rg_s2_firth(rg_handle h, int32_t n, const int32_t* vi, const int32_t* ti, do
   return 0;
 }
 int rg_s2_spa(rg_handle h, int32_t n, const int32_t* vi, const int32_t* ti, double* pval, int32_t* status) {
+  trace("rg_s2_spa", h, n);
   for (int k = 0; k < n; ++k) {
     if (vi[k] < 0 || vi[k] >= h->last_bs || ti[k] < 0 || ti[k] >= h->P) return fail("mock: bad SPA selection");
     pval[k] = std::erfc(std::fabs(h->last_stat[(size_t)vi[k] * h->P + ti[k]]) * 0.6);
@@ -345,6 +386,7 @@ int rg_s2_spa(rg_handle h, int32_t n, const int32_t* vi, const int32_t* ti, doub
 // zlib on the host: the mock's block entry points take host pointers
 int rg_bgen_inflate(rg_handle h, const uint8_t* comp, const uint64_t* offs, int64_t n_file, int32_t bs, const uint8_t** probs,
                     const uint8_t** miss) {
+  trace("rg_bgen_inflate", h, bs);
   h->inflate_probs.resize((size_t)bs * n_file * 2);
   h->inflate_miss.resize((size_t)bs * n_file);
   std::vector<uint8_t> raw(10 + 3 * (size_t)n_file);
@@ -363,6 +405,7 @@ int rg_bgen_inflate(rg_handle h, const uint8_t* comp, const uint64_t* offs, int6
 // the device decoder's arithmetic (csrc/pgen_core.h), lanes run serially; rows live in the handle like the device buffer
 int rg_pgen_decode(rg_handle h, const rg_pgen_block* b, const uint8_t** rows_dev, int64_t* row_stride) {
   if (!h || !b || !rows_dev || !row_stride || !b->bytes || b->bs <= 0 || b->n_file <= 0) return fail("mock: bad pgen block");
+  trace("rg_pgen_decode", h, b->bs);
   const uint32_t n = (uint32_t)b->n_file, words = ((n + 15) / 16 + 3) / 4 * 4;
   h->pgen_rows.assign((size_t)b->bs * words, 0u);
   for (int j = 0; j < b->bs; ++j) {
@@ -382,6 +425,7 @@ int rg_pgen_decode(rg_handle h, const rg_pgen_block* b, const uint8_t** rows_dev
 // staging: a plain copy into the slot (what the block call later reads is the bytes as they were when staged)
 int rg_s2_stage(rg_handle h, int32_t slot, const void* host, int64_t bytes, const uint8_t** dev) {
   if (!h || !host || !dev || bytes <= 0 || slot < 0 || slot > 3) return fail("mock: bad staging arguments");
+  trace("rg_s2_stage", h, (long)bytes, -1, fnv(host, (size_t)bytes));
   h->stage[slot].assign((const uint8_t*)host, (const uint8_t*)host + bytes);
   *dev = h->stage[slot].data();
   return 0;
