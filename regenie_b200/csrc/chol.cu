@@ -139,22 +139,27 @@ chol_diag_kernel(double* __restrict__ cm, int64_t stride, int ld, int k,
   }
 }
 
-// Backward substitution  L^T beta = y  for all right-hand sides, one 1024-thread CTA per matrix,
-// sweeping 64-column blocks from the last to the first.  y lives in the RHS rows (row nC+p,
-// contiguous over columns); beta overwrites it.  The diagonal solves are GEMVs with the stored
-// M = L_kk^-T; the sweep  y[:, j] -= L[k+r][j] beta[r]  streams the 64 panel rows once.
+// Backward substitution  L^T beta = y  for all right-hand sides, sweeping 64-column blocks from
+// the last to the first.  y lives in the RHS rows (row nC+p, contiguous over columns); beta
+// overwrites it.  The diagonal solves are GEMVs with the stored M = L_kk^-T; the sweep
+// y[:, j] -= L[k+r][j] beta[r]  streams the 64 panel rows once.
+// grid: (batch, ceil(P / BS_RHS)): one CTA per matrix and group of at most BS_RHS right-hand sides, so the shared
+// memory is bounded whatever the trait count; every right-hand side goes through the same arithmetic in any group.
 constexpr int BS_THREADS = 256;
 constexpr int BS_JT = 2;        // columns per thread in the sweep (two batches of rows are held in registers)
 constexpr int BS_PC = 10;   // right-hand sides per register pass
+constexpr int BS_RHS = 64;  // right-hand sides per CTA
 
 __global__ void __launch_bounds__(BS_THREADS)
-chol_backsolve_kernel(double* __restrict__ cm, int64_t stride, int ld, int nC, int P,
+chol_backsolve_kernel(double* __restrict__ cm, int64_t stride, int ld, int nC, int P_all,
                       const double* __restrict__ inv, int64_t inv_stride) {
   extern __shared__ double back_sm[];
+  const int P = min(BS_RHS, P_all - (int)blockIdx.y * BS_RHS);   // right-hand sides of this CTA
   double* Ms = back_sm;                    // [TB][TB+1]
   double* ys = Ms + TB * (TB + 1);         // [TB][P]  y block
   double* bs = ys + TB * P;                // [TB][P]  beta block
   double* A = cm + (int64_t)blockIdx.x * stride;
+  double* Y = A + (int64_t)(nC + blockIdx.y * BS_RHS) * ld;     // this CTA's right-hand-side rows
   const double* Minv = inv + (int64_t)blockIdx.x * inv_stride;
   for (int kb = nC / TB - 1; kb >= 0; --kb) {
     const int k = kb * TB;
@@ -163,7 +168,7 @@ chol_backsolve_kernel(double* __restrict__ cm, int64_t stride, int ld, int nC, i
       Ms[(e / TB) * (TB + 1) + (e % TB)] = Minv[(int64_t)kb * TB * TB + e];
     for (int e = threadIdx.x; e < TB * P; e += BS_THREADS) {
       const int r = e % TB, p = e / TB;
-      ys[r * P + p] = A[(int64_t)(nC + p) * ld + k + r];
+      ys[r * P + p] = Y[(int64_t)p * ld + k + r];
     }
     __syncthreads();
     // beta = L_kk^-T y = M y   (M upper triangular: M[r][c], c >= r)
@@ -172,7 +177,7 @@ chol_backsolve_kernel(double* __restrict__ cm, int64_t stride, int ld, int nC, i
       double s = 0.0;
       for (int c = r; c < TB; ++c) s = fma(Ms[r * (TB + 1) + c], ys[c * P + p], s);
       bs[r * P + p] = s;
-      A[(int64_t)(nC + p) * ld + k + r] = s;
+      Y[(int64_t)p * ld + k + r] = s;
     }
     __syncthreads();
     // y[p][j] -= sum_r L[k+r][j] * beta[r][p]   for all j < k   (coalesced over j; each thread owns BS_JT columns).
@@ -224,7 +229,7 @@ chol_backsolve_kernel(double* __restrict__ cm, int64_t stride, int ld, int nC, i
           if (j < k)
 #pragma unroll
             for (int qq = 0; qq < BS_PC; ++qq)
-              if (qq < np) A[(int64_t)(nC + p0 + qq) * ld + j] -= acc[m][qq];
+              if (qq < np) Y[(int64_t)(p0 + qq) * ld + j] -= acc[m][qq];
         }
       }
     }
@@ -247,10 +252,10 @@ void launch_chol_factor(double* cm, int64_t stride, int nC, int n_aug, int batch
 
 void launch_chol_backsolve(double* cm, int64_t stride, int nC, int P, int batch, const double* inv,
                            cudaStream_t s) {
-  const size_t smem = ((size_t)TB * (TB + 1) + (size_t)2 * TB * P) * sizeof(double);
+  const size_t smem = ((size_t)TB * (TB + 1) + (size_t)2 * TB * std::min(P, BS_RHS)) * sizeof(double);
   ensure_dyn_smem(reinterpret_cast<const void*>(chol_backsolve_kernel), smem);
   const int64_t inv_stride = (int64_t)(nC / TB) * TB * TB;
-  chol_backsolve_kernel<<<batch, BS_THREADS, smem, s>>>(cm, stride, nC, nC, P, inv, inv_stride);
+  chol_backsolve_kernel<<<dim3(batch, (unsigned)ceil_div(P, BS_RHS)), BS_THREADS, smem, s>>>(cm, stride, nC, nC, P, inv, inv_stride);
 }
 
 int chol_num_launches(int nC) { return 2 * (nC / TB); }

@@ -82,7 +82,14 @@ inline void ensure_dyn_smem(const void* func, size_t bytes) {
   std::lock_guard<std::mutex> lock(mu);
   size_t& cur = done[std::make_pair(dev, func)];
   if (bytes > cur) {
-    RG_CUDA(cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    const cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) {
+      // a refused request also sets the runtime's last error: clear it, or the next launch check of any handle in the
+      // process would report it
+      cudaGetLastError();
+      throw Error{"cannot give a kernel " + std::to_string(bytes) + " bytes of dynamic shared memory: " +
+                  cudaGetErrorString(e)};
+    }
     cur = bytes;
   }
 }

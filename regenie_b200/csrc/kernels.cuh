@@ -186,7 +186,7 @@ void launch_dense_from_dosage(const uint8_t* probs, const uint8_t* miss, int64_t
 void launch_dense_from_f64(const double* G, int64_t n_file, int bs, const int32_t* file_idx_pad, double* gd, int64_t npad,
                            cudaStream_t s);
 void launch_dense_prepare(double* gd, int64_t npad, int bs, const int32_t* file_idx_pad, const double* xy, int cpp, int C,
-                          long long n_analyzed, double numtol, double* mu, double* sd, unsigned long long* err_slot,
+                          long long n_analyzed, double numtol, double* mu, double* inv_sd, unsigned long long* err_slot,
                           long long err_base, cudaStream_t s);
 void launch_dense_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y, int64_t part_y_stride,
                            const int2* fold_chunks, int K, int R, const double* lambda, int bs, int nC, int P, double* cm,

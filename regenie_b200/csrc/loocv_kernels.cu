@@ -6,6 +6,8 @@
 // quantities are  h_i = |t_i|^2,  yhat_i = t_i . u  with  t_i = L^-1 g_i,  u = L^-1 b :  the sample
 // vectors ride along as extra right-hand-side ROWS of the batched Cholesky (forward substitution
 // fused into the factorisation), so no eigensolver is needed.
+#include <algorithm>
+
 #include "kernels.cuh"
 
 namespace rg {
@@ -34,17 +36,18 @@ __global__ void l0_loocv_fill_kernel(const uint32_t* __restrict__ gp, int64_t wo
 
 // One warp per sample: h = |t|^2, yhat_p = t . u_p, LOO prediction, mask, raw store + partial sums.
 // grid: (Npad/128, R); block 128 threads = 4 warps, each warp loops over 32 samples of the tile.
+// The phenotypes run in tiles of pt <= kMaxPhenoTile whose u rows fit in shared memory (fewer for a wide block).
 __global__ void __launch_bounds__(128)
 l0_loocv_pred_kernel(const double* __restrict__ cm, int64_t cm_stride, int nC, int bs, int Ppad, int P, int R,
                      const double* __restrict__ xy, int cpp, int C, const uint8_t* __restrict__ mask, int64_t npad,
-                     double* const* __restrict__ W, int col0, double* __restrict__ part, int Qp) {
-  extern __shared__ double us[];                 // u_p rows [P][nC]
+                     double* const* __restrict__ W, int col0, double* __restrict__ part, int Qp, int pt) {
+  extern __shared__ double us[];                 // u_p rows [pt][nC]
   __shared__ double red[2][4][kMaxPhenoTile];
   const int r = blockIdx.y;
   const double* A = cm + (int64_t)r * cm_stride;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int p0 = 0; p0 < P; p0 += kMaxPhenoTile) {
-    const int np = min(kMaxPhenoTile, P - p0);
+  for (int p0 = 0; p0 < P; p0 += pt) {
+    const int np = min(pt, P - p0);
     __syncthreads();
     for (int e = threadIdx.x; e < np * nC; e += 128) us[e] = A[(int64_t)(nC + p0 + e / nC) * nC + e % nC];
     __syncthreads();
@@ -230,11 +233,22 @@ void launch_l0_loocv_fill(const uint32_t* gp, int64_t npad, int bs, int nC, cons
 void launch_l0_loocv_pred(const double* cm, int64_t cm_stride, int nC, int bs, int Ppad, int P, int R,
                           const double* xy, int cpp, int C, const uint8_t* mask, int64_t npad, double* const* W,
                           int col0, double* part, int Qp, cudaStream_t s) {
-  const size_t smem = (size_t)std::min(P, kMaxPhenoTile) * nC * sizeof(double);
+  // the u rows of a phenotype tile in the dynamic shared memory the device allows next to the kernel's static arrays
+  static const int64_t fit = [] {
+    int dev = 0, optin = 0;
+    RG_CUDA(cudaGetDevice(&dev));
+    RG_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+    cudaFuncAttributes fa;
+    RG_CUDA(cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(l0_loocv_pred_kernel)));
+    return (int64_t)(optin - (int)fa.sharedSizeBytes) / (int64_t)sizeof(double);
+  }();
+  const int pt = (int)std::min<int64_t>({(int64_t)P, (int64_t)kMaxPhenoTile, fit / nC});
+  RG_CHECK(pt >= 1, "LOOCV level 0: block too wide for the prediction kernel (nC = " + std::to_string(nC) + ")");
+  const size_t smem = (size_t)pt * nC * sizeof(double);
   ensure_dyn_smem(reinterpret_cast<const void*>(l0_loocv_pred_kernel), smem);
   dim3 grid((unsigned)(npad / 128), R);
   l0_loocv_pred_kernel<<<grid, 128, smem, s>>>(cm, cm_stride, nC, bs, Ppad, P, R, xy, cpp, C, mask, npad, W,
-                                              col0, part, Qp);
+                                              col0, part, Qp, pt);
 }
 
 void launch_l0_loocv_std_apply(double* const* W, int64_t npad, int col0, int P, int Q, const uint8_t* mask,
