@@ -150,6 +150,8 @@ int rg_l0_load_W(rg_handle h, int32_t block_id, int32_t ph, const double* in_NxR
  *   tau      [P x R1] row-major: params.tau[ph] AFTER the B(1-h)/h map
  *   cumsum   [5 x P x R1] out: l1_ests.cumsum_values[0..4] (Sx, Sy, Sx2, Sy2, Sxy)
  *   best_idx [P] out: argmin_j (Sx2 + Sy2 - 2 Sxy)/Neff
+ * Only the phenotypes this handle fits (rg_l1_select) are written: the cumsum rows and best_idx entries of the others
+ * keep what the caller passed (pass zeroed buffers to get zeros there).
  */
 int rg_l1_fit(rg_handle h, const double* tau, double* cumsum, int32_t* best_idx);
 
@@ -180,6 +182,7 @@ int rg_prs(rg_handle h, double* prs_out);
  *   y_raw  [N x P] phenotypes_raw (0/1), offset [N x P] m_ests.offset_nullreg (covariate-only logistic fit)
  *   tau    [P x R1] ridge values (B (1-h)/h * 3/pi^2, src/Step1_Models.cpp:2115-2117)
  *   cumsum [6][P][R1]  Sx, Sy, Sx2, Sy2, Sxy, -logLik (cumsum_values[0..5]);  best_idx = argmin -logLik/Neff
+ * As in rg_l1_fit, phenotypes this handle does not fit keep the cumsum rows and best_idx entries the caller passed.
  */
 int rg_l1_fit_bt(rg_handle h, const double* y_raw, const double* offset, const double* tau, double* cumsum,
                  int32_t* best_idx);

@@ -143,7 +143,7 @@ struct rg_ctx {
   std::vector<void*> W_peer_mapped;                  // cudaIpcOpenMemHandle results to close
   std::vector<uint8_t> l1_select;                    // phenotypes this handle fits at level 1
   bool l1_bt = false;                                // logistic level 1: l1_hvec holds f_i = (y - p) / (1 - q w)
-  rg::DevBuf<double> lg_Ws, lg_eta, lg_p, lg_wm, lg_res, lg_off, lg_beta, lg_score, lg_q, lg_devp, lg_scal;
+  rg::DevBuf<double> lg_Ws, lg_eta, lg_wm, lg_res, lg_off, lg_beta, lg_score, lg_q, lg_devp, lg_scal;
   rg::DevBuf<int8_t> lg_ym;
   rg::DevBuf<int2> lg_all_chunks;                    // one entry covering every sample chunk
 

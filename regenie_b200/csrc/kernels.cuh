@@ -12,6 +12,10 @@ constexpr int kLimbs = 9;          // radix-30 digits per coefficient (44 bits)
 constexpr int kLimbsI8 = 5;        // radix-254 int8 digits per coefficient of the INT8 prediction kernel (40 bits)
 constexpr int kLimbQI8 = 50;       // outputs per INT8 prediction pass (5 x 50 = 250 <= 256 digit rows)   // phenotypes per register pass of the LOOCV prediction kernel
 
+// ---- s2_kernels.cu: out[e] = sum_c part[c * per + e] over the nchunks partial vectors, added in chunk order, so the
+// result does not depend on the launch shape (Step-2 statistics, level-1 CV sums and deviances)
+void launch_partial_sum(const double* part, int nchunks, int64_t per, double* out, cudaStream_t s);
+
 // ---- bed_kernels.cu
 // bit 2k set where the 2-bit code k of w is 3 (missing)
 __device__ __forceinline__ uint32_t miss_bits(uint32_t w) { return w & (w >> 1) & 0x55555555u; }
@@ -277,8 +281,7 @@ void launch_rows_sqnorm(const double* rows, int nC, int B, double* out, int ntil
 // ---- l1_logistic.cu
 void launch_l1_scale_rows(const double* W, int64_t ldw, int B, const double* wm, double* Ws, cudaStream_t s);
 void launch_l1_bt_eta(const double* W, int64_t ldw, int B, const double* beta, const double* offset, const int8_t* ym,
-                      double* eta, double* pv, double* wm, double* resid, double* dev_part, double* dev_out,
-                      cudaStream_t s);
+                      double* eta, double* wm, double* resid, double* dev_part, double* dev_out, cudaStream_t s);
 void launch_l1_bt_score(const double* part_y, int nchunks, int B, int nC, double tau, const double* beta, double* score,
                         double* rhs_row, cudaStream_t s);
 void launch_l1_bt_loo_sums(const double* eta, const double* q, const double* wm, const double* resid, const int8_t* ym,

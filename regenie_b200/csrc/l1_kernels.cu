@@ -148,15 +148,6 @@ l1_pred_sums_kernel(const double* __restrict__ W, int64_t ldw, int B, int R1,
   }
 }
 
-// fixed-order final reduction of the per-tile sums.  grid: 1, block 64
-__global__ void l1_sum_reduce_kernel(const double* __restrict__ part_out, int ntiles, double* __restrict__ out) {
-  const int v = threadIdx.x;
-  if (v >= kMaxRidge * 3 + 2) return;
-  double s = 0.0;
-  for (int t = 0; t < ntiles; ++t) s += part_out[(int64_t)t * (kMaxRidge * 3 + 2) + v];
-  out[v] = s;
-}
-
 // Per-chromosome predictions for the selected tau (src/Data.cpp:1246-1251):
 //   pred[t][chr] = W_f[t, cols(chr)] . beta_f[cols(chr), best]
 // grid: (Npad/128); thread = sample; chr_col_start[nchr+1] are column offsets in chromosome order.
@@ -200,7 +191,7 @@ void launch_l1_pred_sums(const double* W, int64_t ldw, int B, int R1, const doub
                          int ntiles, double* out, cudaStream_t s) {
   l1_pred_sums_kernel<<<ntiles, 128, (size_t)R1 * 256 * sizeof(double), s>>>(W, ldw, B, R1, beta, ldb, tile_fold, xy, cpp,
                                                                      ycol, part_out);
-  l1_sum_reduce_kernel<<<1, 64, 0, s>>>(part_out, ntiles, out);
+  launch_partial_sum(part_out, ntiles, kMaxRidge * 3 + 2, out, s);
 }
 
 void launch_l1_chr_pred(const double* W, int64_t ldw, int nchr, const int32_t* chr_col_start, const double* beta,

@@ -25,13 +25,12 @@ __global__ void l1_scale_rows_kernel(const double* __restrict__ W, int64_t ldw, 
   if (t < ldw) Ws[c * ldw + t] = W[c * ldw + t] * sqrt(wm[t]);
 }
 
-// eta = offset + W beta, p, w m, (y - p) m and the deviance partial of each 128-sample tile.
+// eta = offset + W beta, w m, (y - p) m and the deviance partial of each 128-sample tile.
 // grid: Npad/128, block 128 (thread = sample), dynamic smem: B doubles.
 __global__ void __launch_bounds__(128)
 l1_bt_eta_kernel(const double* __restrict__ W, int64_t ldw, int B, const double* __restrict__ beta,
                  const double* __restrict__ offset, const int8_t* __restrict__ ym, double* __restrict__ eta,
-                 double* __restrict__ pv, double* __restrict__ wm, double* __restrict__ resid,
-                 double* __restrict__ dev_part) {
+                 double* __restrict__ wm, double* __restrict__ resid, double* __restrict__ dev_part) {
   extern __shared__ double sb[];
   __shared__ double red[128];
   for (int c = threadIdx.x; c < B; c += 128) sb[c] = beta[c];
@@ -42,7 +41,6 @@ l1_bt_eta_kernel(const double* __restrict__ W, int64_t ldw, int B, const double*
   const int8_t code = ym[t];
   const double p = l1_pvec(e);
   eta[t] = e;
-  pv[t] = p;
   wm[t] = code ? p * (1.0 - p) : 0.0;
   resid[t] = code ? ((code == 2 ? 1.0 : 0.0) - p) : 0.0;
   red[threadIdx.x] = code ? -2.0 * ((code == 1) ? log(1.0 - p) : log(p)) : 0.0;
@@ -52,15 +50,6 @@ l1_bt_eta_kernel(const double* __restrict__ W, int64_t ldw, int B, const double*
     __syncthreads();
   }
   if (threadIdx.x == 0) dev_part[blockIdx.x] = red[0];
-}
-
-// fixed-order sum of nvals interleaved partial vectors: out[k] = sum_tile part[tile * nvals + k].  1 block.
-__global__ void l1_vec_reduce_kernel(const double* __restrict__ part, int ntiles, int nvals, double* __restrict__ out) {
-  const int k = threadIdx.x;
-  if (k >= nvals) return;
-  double s = 0.0;
-  for (int i = 0; i < ntiles; ++i) s += part[(int64_t)i * nvals + k];
-  out[k] = s;
 }
 
 // score = W^T resid - tau beta from the chunk partials of l1_xty; also written into the RHS row of the system.
@@ -134,11 +123,10 @@ void launch_l1_scale_rows(const double* W, int64_t ldw, int B, const double* wm,
   l1_scale_rows_kernel<<<grid, 256, 0, s>>>(W, ldw, wm, Ws);
 }
 void launch_l1_bt_eta(const double* W, int64_t ldw, int B, const double* beta, const double* offset, const int8_t* ym,
-                      double* eta, double* pv, double* wm, double* resid, double* dev_part, double* dev_out,
-                      cudaStream_t s) {
+                      double* eta, double* wm, double* resid, double* dev_part, double* dev_out, cudaStream_t s) {
   const int ntiles = (int)(ldw / 128);
-  l1_bt_eta_kernel<<<ntiles, 128, B * sizeof(double), s>>>(W, ldw, B, beta, offset, ym, eta, pv, wm, resid, dev_part);
-  l1_vec_reduce_kernel<<<1, 32, 0, s>>>(dev_part, ntiles, 1, dev_out);
+  l1_bt_eta_kernel<<<ntiles, 128, B * sizeof(double), s>>>(W, ldw, B, beta, offset, ym, eta, wm, resid, dev_part);
+  launch_partial_sum(dev_part, ntiles, 1, dev_out, s);
 }
 void launch_l1_bt_score(const double* part_y, int nchunks, int B, int nC, double tau, const double* beta, double* score,
                         double* rhs_row, cudaStream_t s) {
@@ -148,7 +136,7 @@ void launch_l1_bt_loo_sums(const double* eta, const double* q, const double* wm,
                            double eps, double* fvec, double* part, double* out6, int64_t npad, cudaStream_t s) {
   const int ntiles = (int)(npad / 128);
   l1_bt_loo_sums_kernel<<<ntiles, 128, 0, s>>>(eta, q, wm, resid, ym, eps, fvec, part);
-  l1_vec_reduce_kernel<<<1, 32, 0, s>>>(part, ntiles, 6, out6);
+  launch_partial_sum(part, ntiles, 6, out6, s);
 }
 void launch_l1_bt_chr_pred(const double* W, int64_t ldw, int nC, const double* zrows, const double* fvec,
                            const double* bvec, int nchr, const int32_t* chr_col_start, double* pred, int64_t npad,

@@ -165,15 +165,6 @@ l1_loocv_sums_kernel(const double* __restrict__ cm, int64_t cm_stride, int nC, i
   }
 }
 
-// fixed-order reduction: out[j][3].  grid: 1, block 32
-__global__ void l1_loocv_sum_reduce_kernel(const double* __restrict__ part, int ntiles, int R1, double* __restrict__ out) {
-  const int e = threadIdx.x;
-  if (e >= R1 * 3) return;
-  double s = 0.0;
-  for (int t = 0; t < ntiles; ++t) s += part[(int64_t)t * R1 * 3 + e];
-  out[e] = s;
-}
-
 // make_predictions_loocv (src/Data.cpp:1296-1328) for the selected tau: rows `trow` hold t_i = L^-1 w_i
 // (copy taken before the row backsolve), rows `zrow` hold z_i = H w_i.  Warp per sample.
 //   yres_i = y_i - w_i.b;  pred[i][chr] = w_i[chr].b[chr] - (w_i[chr].z_i[chr]) * yres_i / (1 - h_i)
@@ -267,7 +258,7 @@ void launch_l1_loocv_sums(const double* cm, int64_t cm_stride, int nC, int B, in
                           int ycol, double* part, int R1, int ntiles, double* out, cudaStream_t s) {
   dim3 grid(ntiles, R1);
   l1_loocv_sums_kernel<<<grid, 128, 0, s>>>(cm, cm_stride, nC, B, nrow0, xy, cpp, ycol, part, R1);
-  l1_loocv_sum_reduce_kernel<<<1, 32, 0, s>>>(part, ntiles, R1, out);
+  launch_partial_sum(part, ntiles, R1 * 3, out, s);   // out[j][3]
 }
 
 void launch_rows_sqnorm(const double* rows, int nC, int B, double* out, int ntiles, cudaStream_t s) {

@@ -71,7 +71,7 @@ __global__ void dosage_relayout_kernel(const uint8_t* __restrict__ probs, const 
 // and the dz words of the 64 rows, loaded with coalesced 256-byte row segments (the first version read them per thread with
 // a stride of one whole row: 592 us per 400 variants at N = 100k, ~10x its FP64 bound; four threads per row also quadruple
 // the warps that feed the FP64 pipe).  Summation order per (row, column): samples ascending inside the chunk; chunks are
-// added in order by dosage_reduce_kernel - fixed, independent of the launch shape.
+// added in order by partial_sum_kernel - fixed, independent of the launch shape.
 constexpr int kDzRows = 64;
 constexpr int kDzSubS = 64;
 
@@ -239,15 +239,6 @@ __global__ void s2_bt_finalize_kernel(S2BtFinalizeArgs a) {
   }
 }
 
-// fixed-order sum over chunks.
-__global__ void dosage_reduce_kernel(const double* __restrict__ part, int nchunks, int64_t per, double* __restrict__ sums) {
-  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (e >= per) return;
-  double s = 0.0;
-  for (int c = 0; c < nchunks; ++c) s += part[(int64_t)c * per + e];
-  sums[e] = s;
-}
-
 __global__ void dosage_scale_kernel(const double* __restrict__ s4, int rows_p, int dp, double* __restrict__ s3,
                                     double* __restrict__ se) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -282,8 +273,7 @@ void launch_dosage_stats(const uint32_t* dz, int64_t npad, const double* F, int 
   const int groups = grid.z > 1 ? 4 : (int)ceil_div(ncol, 4);
   if ((int)grid.z * kDzCols < dp || groups < 4) RG_CUDA(cudaMemsetAsync(part, 0, (size_t)nchunks * rows_p * 4 * dp * sizeof(double), s));
   dosage_stats_kernel<<<grid, 64 * groups, 0, s>>>(dz, npad, F, dp, ncol, chunks, rows_p, part, part_cnt);
-  const int64_t per = (int64_t)rows_p * 4 * dp;
-  dosage_reduce_kernel<<<(unsigned)ceil_div(per, 256), 256, 0, s>>>(part, nchunks, per, sums);
+  launch_partial_sum(part, nchunks, (int64_t)rows_p * 4 * dp, sums, s);
   dosage_count_reduce_kernel<<<(unsigned)ceil_div(rows_p, 256), 256, 0, s>>>(part_cnt, nchunks, rows_p, nnz, n510);
 }
 

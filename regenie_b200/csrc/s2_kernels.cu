@@ -71,13 +71,13 @@ s2_stats_kernel(const uint32_t* __restrict__ gp, int64_t words_per_row, const do
   }
 }
 
-// fixed-order sum over chunks.  grid: ceil(rows_p*3*dp/256)
-__global__ void s2_reduce_kernel(const double* __restrict__ part, int nchunks, int64_t per, double* __restrict__ sums) {
+// out[e] = sum_c part[c * per + e], chunks added in order.  grid: ceil(per/256)
+__global__ void partial_sum_kernel(const double* __restrict__ part, int nchunks, int64_t per, double* __restrict__ out) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (e >= per) return;
   double s = 0.0;
   for (int c = 0; c < nchunks; ++c) s += part[(int64_t)c * per + e];
-  sums[e] = s;
+  out[e] = s;
 }
 
 // one thread per variant
@@ -255,8 +255,11 @@ void launch_s2_stats(const uint32_t* gp, int64_t npad, const double* F, int dp, 
                      int rows_p, double* part, double* sums, cudaStream_t s) {
   dim3 grid(rows_p / 128, nchunks, dp / kS2Cols);
   s2_stats_kernel<<<grid, 128, 0, s>>>(gp, npad / 16, F, dp, chunks, rows_p, part);
-  const int64_t per = (int64_t)rows_p * 3 * dp;
-  s2_reduce_kernel<<<(unsigned)ceil_div(per, 256), 256, 0, s>>>(part, nchunks, per, sums);
+  launch_partial_sum(part, nchunks, (int64_t)rows_p * 3 * dp, sums, s);
+}
+
+void launch_partial_sum(const double* part, int nchunks, int64_t per, double* out, cudaStream_t s) {
+  partial_sum_kernel<<<(unsigned)ceil_div(per, 256), 256, 0, s>>>(part, nchunks, per, out);
 }
 
 void launch_s2_finalize(const S2FinalizeArgs& a, cudaStream_t s) {

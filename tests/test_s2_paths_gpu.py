@@ -474,7 +474,7 @@ def _check_tensor_sums(got, planes, F, rows, exact_cols):
 
 @pytest.mark.parametrize("P", [3, 50])
 def test_qt_f64_statistics_fallback(tmp_path, monkeypatch, P):
-    """RG_B200_S2_STATS=f64 at N = 3000 (Npad 3072: two FP64 chunks): s2_stats_kernel + s2_reduce_kernel against the
+    """RG_B200_S2_STATS=f64 at N = 3000 (Npad 3072: two FP64 chunks): s2_stats_kernel + partial_sum_kernel against the
     oracle, then against the tensor-core path on the same inputs."""
     assert _run_case_f64(tmp_path, monkeypatch, N=3000, M=256, P=P, miss=0.02) > 200
 
