@@ -234,21 +234,28 @@ potrf128_kernel(float* __restrict__ Lplain, float* __restrict__ Mplain, float* _
 // integers, so atomicMax is exact and order-independent).  A system is finished as soon as one step's correction
 // satisfied  max|dx| <= tol * max|x|; finished systems are skipped by every later launch.
 // Stopping rule.  dx_s = (LL^T)^-1 (b - A x_{s-1}) is the forward error of the PREVIOUS iterate up to the contraction
-// factor rho = ||I - (LL^T)^-1 A||, and rho itself is what the P right-hand sides sample: dx_1 / x = ||(I - XA) x|| / ||x||.
-//   (a) dx_s <= tol x                      : x_{s-1} was already within tol, x_s is better by rho           (rigorous)
-//   (b) kMxSafety (dx_s / x)^2 <= tol      : predicted error of x_s = rho dx_s with rho <= kMxSafety dx_s/x.  kMxSafety = 64
-//       covers the worst ratio sqrt(n) = 32..45 between the operator norm and its gain on a generic vector; with the
-//       benchmark's dx_1/x = 2.6e-6 the predicted bound is 4e-10 and the measured error of x_1 8e-12.
+// factor rho = ||I - (LL^T)^-1 A||, so the error of x_s is about rho dx_s.  rho is estimated from the corrections the
+// P right-hand sides have seen, rho_s = dx_s / dx_{s-1} with dx_0 := x: x_0 = (LL^T)^-1 b carries a relative error of
+// about rho, so dx_1 / x samples rho, and each later correction is the previous one shrunk by rho.
+//   (a) dx_s <= tol x                          : x_{s-1} was already within tol, x_s is better by rho       (rigorous)
+//   (b) kMxSafety rho_s dx_s <= tol x          : predicted error of x_s = rho dx_s with rho <= kMxSafety rho_s.
+//       kMxSafety = 64 covers the worst ratio sqrt(n) = 32..45 between the operator norm and its gain on a generic
+//       vector.  At s = 1 this is kMxSafety (dx_1 / x)^2 <= tol; with the benchmark's dx_1/x = 2.6e-6 the predicted
+//       bound is 4e-10 and the measured error of x_1 8e-12.  Estimating rho by dx_s / x at s >= 2 instead would take
+//       rho^s for rho and accept errors up to ~60x tol for rho ~ 1e-3 .. 1.6e-2 (on an H100, kappa ~ 2e4 .. 3e5).
 // A negative tol (rg_dbg_mixed_solve) keeps only (a).
 constexpr float kMxSafety = 64.f;
 __device__ __forceinline__ bool mx_finished(const unsigned int* conv, int nmat, int m, int upto_step, float tol) {
   const bool strict = tol < 0.f;                      // the host passes -tol for the strict rule
   const float t = fabsf(tol);
+  float prev = 0.f;                                   // dx_{s-1}; dx_0 := x
   for (int s = 1; s <= upto_step; ++s) {
     const float dx = __uint_as_float(conv[((int64_t)s * nmat + m) * 2]);
     const float xx = __uint_as_float(conv[((int64_t)s * nmat + m) * 2 + 1]);
+    if (s == 1) prev = xx;
     if (dx <= t * xx) return true;
-    if (!strict && kMxSafety * dx * dx <= t * xx * xx) return true;
+    if (!strict && kMxSafety * dx * dx <= t * xx * prev) return true;
+    prev = dx;
   }
   return false;
 }
