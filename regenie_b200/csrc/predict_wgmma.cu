@@ -20,6 +20,9 @@
 // The epilogue also leaves per-tile column sums (sum, sum of squares) of the raw predictions for the standardisation.
 #include <stdlib.h>
 
+#include <algorithm>
+#include <atomic>
+
 #include "kernels.cuh"
 #include "wgmma_sm90.cuh"
 
@@ -37,14 +40,13 @@ constexpr int PI_A_WORDS = PT_BM / 16;             // 2-bit words per SNP row of
 constexpr int PI_A_BYTES = PT_BK * PI_A_WORDS * 4; // 4 KiB: 128 SNP rows x 128 samples of 2-bit codes
 constexpr int PI_B_BYTES = PI_BN * PT_BK;          // 32 KiB: 256 digit rows x 128 k bytes
 constexpr int PI_STAGE_BYTES = PI_A_BYTES + PI_B_BYTES;
-constexpr int PI_THREADS = 288;                    // 2 consumer warpgroups (samples 0-63 / 64-127), 1 TMA warp
-constexpr int PI_QH = kLimbQI8 / 2;                // outputs per epilogue thread (25)
-constexpr int PI_LDE = PI_BN + 1;                  // row stride (int32) of the staged accumulator tile
-constexpr int PI_LDV = PT_BM + 1;                  // row stride (double) of the staged prediction tile
+constexpr int PI_THREADS = 384;                    // 2 MMA warpgroups (samples 0-63 / 64-127), 1 epilogue warpgroup
+constexpr int PI_LDV = PT_BM + 1;                  // row stride (double) of the handoff tile V[output][sample]
+constexpr int PI_EG = 10;                          // outputs per group of independent chains in the epilogue
 constexpr int PI_MAX_ROWS = 2048;                  // rows_p bound of the INT8 route (2 rows_p <= 4096)
-static_assert(kLimbsI8 * kLimbQI8 <= PI_BN && kLimbQI8 % 2 == 0, "INT8 prediction layout");
-static_assert(PT_BM * PI_LDE * 4 <= PI_STAGES * PI_STAGE_BYTES, "the accumulator tile reuses the stage buffers");
-static_assert((kLimbQI8 * PI_LDV + 4 * kLimbQI8) * 8 <= PI_STAGES * PI_STAGE_BYTES, "so does the prediction tile");
+// the handoff's limb walk: limb l of output q is column q + 50 l, and 50 = 6 x 8 + 2 moves it one quad lane per limb
+static_assert(kLimbsI8 == 5 && kLimbQI8 == 50 && kLimbsI8 * kLimbQI8 <= PI_BN, "INT8 prediction layout");
+static_assert(kLimbQI8 % PI_EG == 0, "epilogue output groups");
 
 }  // namespace
 
@@ -113,9 +115,23 @@ l0_coef_i8_kernel(const double* __restrict__ cm, int64_t cm_stride, int ldc, int
   }
 }
 
-// grid: (Npad / 128 sample tiles, q groups); 288 threads.
+// Persistent: grid = min(items, SMs), items = (sample tile, q group) pairs, item = tile * ngroups + g, and CTA b runs
+// items b, b + grid, b + 2 grid, ...  384 threads: warpgroups 0 and 1 run the MMAs of an item (one 64-sample half each)
+// and keep the stage ring full themselves, warpgroup 2 runs the epilogue of the previous item meanwhile.
+//   - ring: the k-blocks of all of a CTA's items form one sequence it = k nkb + kb over PI_STAGES stages.  Each MMA
+//     warpgroup counts its release of a stage in rel[s]; the second of the two loads k-block it + PI_STAGES into it, so
+//     the next item's first stages are in flight while this item's last MMAs run, and nothing ever waits for a stage
+//     to empty.
+//   - handoff: after its last MMA of an item, an MMA warpgroup reduces the five limbs of each output to the FP64 Horner
+//     sum (the limbs of output q sit in columns q + 50 l, spread over the four threads of a quad) and writes it to
+//     V[q][sample], which does not alias the stages; arrivals on hfull publish V, the epilogue's arrivals on hfree
+//     give it back.
+//   - epilogue: thread = sample, all 50 outputs: scale, covariate correction, mask, store to W, then the tile's column
+//     sums (sum, sum of squares) from V in sample order, the two 64-sample halves added.  It loads the item's scales,
+//     cvec, W columns, mask bytes and covariates before it waits for V.
 __global__ void __launch_bounds__(PI_THREADS, 1)
-l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmD, PredictTcArgs a) {
+l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmD, PredictTcArgs a,
+                     int ntiles) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -123,64 +139,152 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_const
   const uint32_t sB = base;                                         // [NST][32 KiB], 1 KiB aligned (128B swizzle)
   const uint32_t sA = base + PI_STAGES * PI_B_BYTES;                // [NST][4 KiB]
   uint64_t* bars = reinterpret_cast<uint64_t*>(gen_base + PI_STAGES * PI_STAGE_BYTES);
-  const uint32_t full_bar = smem_u32(bars);
-  const uint32_t empty_bar = smem_u32(bars + PI_STAGES);
-  double* s_scale = reinterpret_cast<double*>(bars + 2 * PI_STAGES);   // [kLimbQI8]
-  double* s_cvec = s_scale + kLimbQI8;                                  // [kLimbQI8][C]
+  const uint32_t full_bar = smem_u32(bars);                         // [NST]
+  const uint32_t hfull = smem_u32(bars + PI_STAGES);
+  const uint32_t hfree = smem_u32(bars + PI_STAGES + 1);
+  uint32_t* rel = reinterpret_cast<uint32_t*>(bars + PI_STAGES + 2);   // [NST] stage releases
+  double* V = reinterpret_cast<double*>(gen_base + PI_STAGES * PI_STAGE_BYTES + 128);   // [kLimbQI8][PI_LDV]
+  double* Vs = V + kLimbQI8 * PI_LDV;                                  // [2 sample halves][kLimbQI8][2]
+  double* s_scale = Vs + 4 * kLimbQI8;                                 // [kLimbQI8]
+  double* s_cvec = s_scale + kLimbQI8;                                 // [kLimbQI8][C]
   double** s_dst = reinterpret_cast<double**>(s_cvec + kLimbQI8 * a.C);                     // [kLimbQI8] W columns
   const uint8_t** s_msk = reinterpret_cast<const uint8_t**>(s_cvec + kLimbQI8 * (a.C + 1));  // [kLimbQI8] mask rows
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role
-  const int tile = blockIdx.x, g = blockIdx.y;
-  const int f = a.tile_fold[tile];
+  const int nk = (ntiles * a.ngroups - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // items of this CTA
   const int nkh = a.rows_p / PT_BK;                 // k-blocks per plane
   const int nkb = 2 * nkh;
-  const int q0 = g * kLimbQI8;
-  const int nq = min(kLimbQI8, a.Q - q0);
+  auto item_of = [&](int k) { return (int)blockIdx.x + k * (int)gridDim.x; };
 
-  if (warp == 8 && lane == 0) {
-    for (int s = 0; s < PI_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < PI_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); rel[s] = 0; }
+    mbar_init(hfull, 256);
+    mbar_init(hfree, 128);
     fence_barrier_init();
     prefetch_tmap(&tmG);
     prefetch_tmap(&tmD);
   }
-  for (int e = threadIdx.x; e < kLimbQI8; e += PI_THREADS) {
-    const int q = q0 + e, r = q / a.P, p = q % a.P;
-    s_scale[e] = (e < nq) ? a.scale[(int64_t)f * a.Qp + q] / 127.0 : 0.0;
-    s_dst[e] = (e < nq) ? a.W[p] + (int64_t)(a.col0 + r) * a.npad : nullptr;
-    s_msk[e] = (e < nq) ? a.mask + (int64_t)p * a.npad : nullptr;
-  }
-  for (int e = threadIdx.x; e < kLimbQI8 * a.C; e += PI_THREADS) {
-    const int qq = e / a.C, c = e % a.C;
-    s_cvec[e] = (qq < nq) ? a.cvec[((int64_t)f * a.Qp + q0 + qq) * a.C + c] : 0.0;
-  }
   __syncthreads();
 
-  if (warp == 8) {
-    if (lane == 0) {
-      // ===== TMA producer: A = 128 SNP rows x 8 words (128 samples) of 2-bit codes, the G0 rows and then the same rows
-      // for the Miss plane; B = 256 digit rows x 128 k bytes =====
-      const int drow0 = (f * a.ngroups + g) * PI_BN;
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % PI_STAGES;
-        const uint32_t ph = (kb / PI_STAGES) & 1;
-        mbar_wait(empty_bar + 8 * s, ph ^ 1);
-        mbar_expect_tx(full_bar + 8 * s, PI_STAGE_BYTES);
-        tma_load_2d(sA + s * PI_A_BYTES, &tmG, full_bar + 8 * s, tile * PI_A_WORDS, (kb % nkh) * PT_BK);
-        tma_load_2d(sB + s * PI_B_BYTES, &tmD, full_bar + 8 * s, kb * PT_BK, drow0);
-        tma_load_2d(sB + s * PI_B_BYTES + 16384, &tmD, full_bar + 8 * s, kb * PT_BK, drow0 + 128);
+  if (warp >= 8) {
+    // ===== epilogue warpgroup: gives 16 of its 168 registers per thread to the MMA warpgroups =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 152;\n" ::: "memory");
+    const int ct = threadIdx.x - 256;               // sample of the tile
+    for (int k = 0; k < nk; ++k) {
+      const int tile = item_of(k) / a.ngroups, g = item_of(k) % a.ngroups;
+      const int f = a.tile_fold[tile];
+      const int q0 = g * kLimbQI8;
+      const int nq = min(kLimbQI8, a.Q - q0);
+      // the previous item's readers of these are past its last named barrier
+      for (int e = ct; e < kLimbQI8; e += 128) {
+        const int q = q0 + e, r = q / a.P, p = q % a.P;
+        s_scale[e] = (e < nq) ? a.scale[(int64_t)f * a.Qp + q] / 127.0 : 0.0;
+        s_dst[e] = (e < nq) ? a.W[p] + (int64_t)(a.col0 + r) * a.npad : nullptr;
+        s_msk[e] = (e < nq) ? a.mask + (int64_t)p * a.npad : nullptr;
+      }
+      for (int e = ct; e < kLimbQI8 * a.C; e += 128) {
+        const int qq = e / a.C, c = e % a.C;
+        s_cvec[e] = (qq < nq) ? a.cvec[((int64_t)f * a.Qp + q0 + qq) * a.C + c] : 0.0;
+      }
+      named_sync(1, 128);
+      const int t = tile * PT_BM + ct;
+      // every global load of the epilogue is issued here, ahead of the stores below, so that the 50 mask rows cost one
+      // memory latency rather than one each (the compiler may not move a load across a store through another pointer)
+      uint32_t mk[kLimbQI8];
+#pragma unroll
+      for (int j = 0; j < kLimbQI8; ++j) mk[j] = (j < nq) ? s_msk[j][t] : 0u;
+      double xr[kMaxCov];
+      for (int c = 0; c < a.C; ++c) xr[c] = a.xy[(int64_t)t * a.cpp + c];
+      mbar_wait(hfull, k & 1);
+      // outputs in groups of PI_EG, the covariates outermost inside a group: the same operations per output, in the
+      // same order, as independent chains
+#pragma unroll
+      for (int j0 = 0; j0 < kLimbQI8; j0 += PI_EG) {
+        double val[PI_EG];
+#pragma unroll
+        for (int j = 0; j < PI_EG; ++j) val[j] = V[(j0 + j) * PI_LDV + ct] * s_scale[j0 + j];
+        for (int c = 0; c < a.C; ++c) {
+#pragma unroll
+          for (int j = 0; j < PI_EG; ++j) val[j] -= xr[c] * s_cvec[(j0 + j) * a.C + c];
+        }
+#pragma unroll
+        for (int j = 0; j < PI_EG; ++j) {
+          const int qq = j0 + j;
+          double v = 0.0;
+          if (qq < nq) {
+            v = val[j] * (double)mk[qq];
+            s_dst[qq][t] = v;
+          }
+          V[qq * PI_LDV + ct] = v;
+        }
+      }
+      named_sync(1, 128);
+      if (ct < 2 * kLimbQI8) {
+        const int qq = ct % kLimbQI8, sh = ct / kLimbQI8;
+        const double* v = V + qq * PI_LDV + sh * (PT_BM / 2);
+        double s1 = 0.0, s2 = 0.0;
+#pragma unroll 8
+        for (int i = 0; i < PT_BM / 2; ++i) {
+          s1 += v[i];
+          s2 = fma(v[i], v[i], s2);
+        }
+        Vs[(sh * kLimbQI8 + qq) * 2 + 0] = s1;
+        Vs[(sh * kLimbQI8 + qq) * 2 + 1] = s2;
+      }
+      named_sync(1, 128);
+      mbar_arrive(hfree);                           // V is read: the MMA warpgroups may write the next item's
+      if (ct < nq) {
+        a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 0] = Vs[ct * 2 + 0] + Vs[(kLimbQI8 + ct) * 2 + 0];
+        a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 1] = Vs[ct * 2 + 1] + Vs[(kLimbQI8 + ct) * 2 + 1];
       }
     }
     return;
   }
 
-  // ===== consumers: warpgroup wg = samples 64 wg .. 64 wg + 63 x all 256 digit rows =====
+  // ===== MMA warpgroups: warpgroup wg = samples 64 wg .. 64 wg + 63 x all 256 digit rows =====
   // Thread (warp w of the warpgroup, lane l, r = l / 4, t4 = l % 4) holds fragment rows r and r + 8 of its warp's 16,
   // which are the samples 2 r and 2 r + 1 of the warp's 16 (from 64 wg + 16 w): the nibble at bit 4 r of word 4 wg + w
   // of each SNP row.  Its k are the quads 4 t4 .. +3 and 16 + 4 t4 .. +3 of each MMA's 32.  At load j, lane t4 reads row
   // 4 t4 + (j + t4) % 4 of its quad, so the four t4 of an instruction meet four distinct banks and the eight lanes of
   // each t4 read one word (broadcast); qsel undoes the rotation.
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 176;\n" ::: "memory");
   const int wg = warp >> 2, w = warp & 3, r = lane >> 2, t4 = lane & 3;
+  const bool leader = w == 0 && lane == 0;
+  // Ring cursor of the leaders (both track it; the second releaser of a stage issues): item ck, k-block ckb, the fold
+  // of item ck and, loaded one item ahead, of item ck + 1.
+  int ck = 0, ckb = 0, cf = 0, cfn = 0;
+  if (leader) {
+    cf = a.tile_fold[item_of(0) / a.ngroups];
+    if (nk > 1) cfn = a.tile_fold[item_of(1) / a.ngroups];
+  }
+  // A = 128 SNP rows x 8 words (128 samples) of 2-bit codes, the G0 rows and then the same rows for the Miss plane;
+  // B = 256 digit rows x 128 k bytes
+  auto refill = [&](bool issue) {
+    if (ck >= nk) return;
+    if (issue) {
+      const int s = (ck * nkb + ckb) % PI_STAGES;
+      const uint32_t fb = full_bar + 8 * s;
+      const int drow0 = (cf * a.ngroups + item_of(ck) % a.ngroups) * PI_BN;
+      mbar_expect_tx(fb, PI_STAGE_BYTES);
+      tma_load_2d(sA + s * PI_A_BYTES, &tmG, fb, (item_of(ck) / a.ngroups) * PI_A_WORDS, (ckb % nkh) * PT_BK);
+      tma_load_2d(sB + s * PI_B_BYTES, &tmD, fb, ckb * PT_BK, drow0);
+      tma_load_2d(sB + s * PI_B_BYTES + 16384, &tmD, fb, ckb * PT_BK, drow0 + 128);
+    }
+    if (++ckb == nkb) {
+      ckb = 0;
+      ++ck;
+      cf = cfn;
+      if (ck + 1 < nk) cfn = a.tile_fold[item_of(ck + 1) / a.ngroups];
+    }
+  };
+  // this warpgroup's MMAs have read stage it % PI_STAGES for the last time in round it
+  auto release = [&](int it) {
+    if (leader) refill(atomicAdd(&rel[it % PI_STAGES], 1u) & 1u);
+  };
+  if (leader) {
+    for (int s = 0; s < PI_STAGES; ++s) refill(wg == 0);
+  }
+
   int aoff[4];                                      // byte offset of load j inside a 16-row quad slice of the A stage
   uint32_t qsel = 0;                                // byte k of a quad comes from load (k - t4) % 4
 #pragma unroll
@@ -212,110 +316,76 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_const
   };
   // One commit group per MMA, two fragment register sets: while MMA u runs, MMA u - 1 is retired (freeing its fragment
   // registers, and at the first MMA of a stage the previous stage's buffers) and the fragment of MMA u + 1 is built.
-  // Double-buffering whole stages would need 32 fragment registers beside the 128 accumulators, more than the 168 a
-  // thread gets at 288 threads per SM.
+  // Double-buffering whole stages would need 32 fragment registers beside the 128 accumulators, more than the 176 an
+  // MMA thread gets.
   int32_t acc[128];
-#pragma unroll
-  for (int i = 0; i < 128; ++i) acc[i] = 0;
-  fence_regs(acc);
   uint32_t afr[2][4];
-  mbar_wait(full_bar, 0);
-  build(0, 0, false, afr[0]);
-  for (int kb = 0; kb < nkb; ++kb) {
-    const int s = kb % PI_STAGES;
-    const bool miss = kb >= nkh;
-    const uint64_t db = desc_k128(sB + s * PI_B_BYTES);
+  const double inv254 = 1.0 / 254.0;
+  int it = 0;                                       // ring round of the current k-block
+  for (int k = 0; k < nk; ++k) {
 #pragma unroll
-    for (int kk = 0; kk < PT_BK / 32; ++kk) {
-      wgmma_fence();
-      // +32 bytes (K of one MMA) inside the 128-byte swizzle atom: +2 in 16-byte units
-      wgmma_s8_rs_n256(acc, afr[kk & 1], db + (uint64_t)(2 * kk));
-      wgmma_commit();
-      wgmma_wait<1>();
-      if (kk == 0 && kb > 0 && w == 0 && lane == 0) mbar_arrive(empty_bar + 8 * ((kb - 1) % PI_STAGES));
-      if (kk + 1 < PT_BK / 32) {
-        build(s, kk + 1, miss, afr[(kk + 1) & 1]);
-      } else if (kb + 1 < nkb) {
-        mbar_wait(full_bar + 8 * ((kb + 1) % PI_STAGES), ((kb + 1) / PI_STAGES) & 1);
-        build((kb + 1) % PI_STAGES, 0, kb + 1 >= nkh, afr[0]);
+    for (int i = 0; i < 128; ++i) acc[i] = 0;
+    fence_regs(acc);
+    mbar_wait(full_bar + 8 * (it % PI_STAGES), (it / PI_STAGES) & 1);
+    build(it % PI_STAGES, 0, false, afr[0]);
+    for (int kb = 0; kb < nkb; ++kb, ++it) {
+      const int s = it % PI_STAGES;
+      const bool miss = kb >= nkh;
+      const uint64_t db = desc_k128(sB + s * PI_B_BYTES);
+#pragma unroll
+      for (int kk = 0; kk < PT_BK / 32; ++kk) {
+        wgmma_fence();
+        // +32 bytes (K of one MMA) inside the 128-byte swizzle atom: +2 in 16-byte units
+        wgmma_s8_rs_n256(acc, afr[kk & 1], db + (uint64_t)(2 * kk));
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kk == 0 && kb > 0) release(it - 1);
+        if (kk + 1 < PT_BK / 32) {
+          build(s, kk + 1, miss, afr[(kk + 1) & 1]);
+        } else if (kb + 1 < nkb) {
+          mbar_wait(full_bar + 8 * ((it + 1) % PI_STAGES), ((it + 1) / PI_STAGES) & 1);
+          build((it + 1) % PI_STAGES, 0, kb + 1 >= nkh, afr[0]);
+        }
       }
     }
-  }
-  wgmma_wait<0>();
-  fence_regs(acc);
+    wgmma_wait<0>();
+    fence_regs(acc);
+    release(it - 1);
 
-  // ===== epilogue: accumulators -> shared memory tile E[sample][digit row] (the stage buffers are free once every
-  // consumer is past its last MMA) -> thread = (sample, half of the outputs).  Limb sums are exact int32 multiples of 8;
-  // FP64 Horner from the lowest limb up.
-  named_sync(1, 256);
-  int32_t* E = reinterpret_cast<int32_t*>(gen_base);
-  double* V = reinterpret_cast<double*>(gen_base);           // [kLimbQI8][PI_LDV], written once E is read
-  double* Vs = V + kLimbQI8 * PI_LDV;                          // [2 sample halves][kLimbQI8][2]
+    // ===== handoff: V[q][sample] = FP64 Horner of the five limb sums (exact int32 multiples of 8) from the lowest limb
+    // up.  Accumulator i of this thread is column 8 (i / 4) + 2 t4 + (i & 1) of sample 2 r + (i / 2) % 2.  The thread
+    // forms the outputs q = 8 m + 2 t4 + b; limb l of q is column q + 50 l = 8 (m + 6 l + c) + 2 ((t4 + l) % 4) + b with
+    // c = (t4 + l >= 4), held by quad lane (t4 + l) % 4, which (seen from that lane, t4' = (t4 + l) % 4) has c = (t4' < l).
+    mbar_wait(hfree, (k & 1) ^ 1);
+    const int smp0 = 64 * wg + 16 * w + 2 * r;
 #pragma unroll
-  for (int i = 0; i < 128; ++i) {
-    const int smp = 64 * wg + 16 * w + 2 * r + ((i >> 1) & 1);
-    const int col = 8 * (i >> 2) + 2 * t4 + (i & 1);
-    E[smp * PI_LDE + col] = acc[i];
-  }
-  named_sync(1, 256);
-  const int ct = threadIdx.x;                      // 0..255
-  const int half = ct >> 7;                        // warps 0-3: outputs 0-24, warps 4-7: outputs 25-49
-  {
-    const int smp = ct & 127;
-    const int t = tile * PT_BM + smp;
-    const int32_t* er = E + smp * PI_LDE + half * PI_QH;
-    // every global load of the epilogue is issued here, ahead of the stores below, so that the 25 mask rows cost one
-    // memory latency rather than one each (the compiler may not move a load across a store through another pointer)
-    uint32_t mk[PI_QH];
+    for (int hb = 0; hb < 2; ++hb) {
 #pragma unroll
-    for (int j = 0; j < PI_QH; ++j) mk[j] = (half * PI_QH + j < nq) ? s_msk[half * PI_QH + j][t] : 0u;
-    double xr[kMaxCov];
-    for (int c = 0; c < a.C; ++c) xr[c] = a.xy[(int64_t)t * a.cpp + c];
-    const double inv254 = 1.0 / 254.0;
-    double accd[PI_QH];
+      for (int m = 0; m < (kLimbQI8 + 7) / 8; ++m) {
 #pragma unroll
-    for (int j = 0; j < PI_QH; ++j) accd[j] = 0.0;
+        for (int b = 0; b < 2; ++b) {
+          int32_t e[kLimbsI8];
 #pragma unroll
-    for (int l = kLimbsI8 - 1; l >= 0; --l) {
+          for (int l = 0; l < kLimbsI8; ++l) {
+            const int i0 = 4 * (m + 6 * l) + 2 * hb + b;
+            if (l == 0) {
+              e[l] = acc[i0];
+            } else if (l == 4) {
+              e[l] = acc[i0 + 4];
+            } else {
+              const int32_t sv = t4 < l ? acc[i0 + 4] : acc[i0];
+              e[l] = __shfl_sync(0xffffffffu, sv, (lane & ~3) | ((t4 + l) & 3));
+            }
+          }
+          double d = 0.0;
 #pragma unroll
-      for (int j = 0; j < PI_QH; ++j) accd[j] = fma(accd[j], inv254, (double)(er[l * kLimbQI8 + j] >> 3));
-    }
-#pragma unroll
-    for (int j = 0; j < PI_QH; ++j) {
-      const int qq = half * PI_QH + j;
-      double val = 0.0;
-      if (qq < nq) {
-        val = accd[j] * s_scale[qq];
-        for (int c = 0; c < a.C; ++c) val -= xr[c] * s_cvec[qq * a.C + c];
-        val *= (double)mk[j];
-        s_dst[qq][t] = val;
+          for (int l = kLimbsI8 - 1; l >= 0; --l) d = fma(d, inv254, (double)(e[l] >> 3));
+          const int q = 8 * m + 2 * t4 + b;
+          if (q < kLimbQI8) V[q * PI_LDV + smp0 + hb] = d;
+        }
       }
-      accd[j] = val;
     }
-    // column sums of the tile (sum, sum of squares) in a fixed order: the values go through shared memory (over E, once
-    // every thread has read its row), transposed to V[output][sample]; thread (output, half of the samples) sums 64 of
-    // them in sample order, and the two halves are added
-    named_sync(1, 256);
-#pragma unroll
-    for (int j = 0; j < PI_QH; ++j) V[(half * PI_QH + j) * PI_LDV + smp] = accd[j];
-  }
-  named_sync(1, 256);
-  if (ct < 2 * kLimbQI8) {
-    const int qq = ct % kLimbQI8, sh = ct / kLimbQI8;
-    const double* v = V + qq * PI_LDV + sh * (PT_BM / 2);
-    double s1 = 0.0, s2 = 0.0;
-#pragma unroll 8
-    for (int i = 0; i < PT_BM / 2; ++i) {
-      s1 += v[i];
-      s2 = fma(v[i], v[i], s2);
-    }
-    Vs[(sh * kLimbQI8 + qq) * 2 + 0] = s1;
-    Vs[(sh * kLimbQI8 + qq) * 2 + 1] = s2;
-  }
-  named_sync(1, 256);
-  if (ct < nq) {
-    a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 0] = Vs[ct * 2 + 0] + Vs[(kLimbQI8 + ct) * 2 + 0];
-    a.part[((int64_t)tile * a.Qp + q0 + ct) * 2 + 1] = Vs[ct * 2 + 1] + Vs[(kLimbQI8 + ct) * 2 + 1];
+    mbar_arrive(hfull);
   }
 }
 
@@ -406,13 +476,29 @@ void launch_l0_coef_i8(const double* cm, int64_t cm_stride, int ldc, int nC, int
                                          scale, dig, ngroups);
 }
 
+// SMs of the current device, read once per device
+static int sm_count() {
+  static std::atomic<int> n_sm[64];
+  int dev = 0;
+  RG_CUDA(cudaGetDevice(&dev));
+  RG_CHECK(dev < 64, "INT8 prediction: device ordinal above 63");
+  int n = n_sm[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    RG_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+    n_sm[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
+
 void launch_l0_predict_i8(const CUtensorMap& tmG, const CUtensorMap& tmD, const PredictTcArgs& a, int ntiles,
                           cudaStream_t s) {
   RG_CHECK(2 * a.rows_p <= 4096, "INT8 prediction: 2 * rows_p <= 4096 (int32 Horner bound)");
-  const size_t smem = (size_t)PI_STAGES * PI_STAGE_BYTES + 1024 + 128 +
-                      ((size_t)kLimbQI8 * (3 + a.C)) * sizeof(double);   // scales, cvec, 2 pointers
+  // stages, barriers, V, its column sums, then scales, cvec and 2 pointers per output
+  const size_t smem = 1024 + (size_t)PI_STAGES * PI_STAGE_BYTES + 128 +
+                      ((size_t)kLimbQI8 * PI_LDV + 4 * kLimbQI8 + (size_t)kLimbQI8 * (3 + a.C)) * sizeof(double);
   ensure_dyn_smem(reinterpret_cast<const void*>(l0_predict_i8_kernel), smem);
-  l0_predict_i8_kernel<<<dim3(ntiles, a.ngroups), PI_THREADS, smem, s>>>(tmG, tmD, a);
+  const int grid = (int)std::min<int64_t>((int64_t)ntiles * a.ngroups, sm_count());
+  l0_predict_i8_kernel<<<grid, PI_THREADS, smem, s>>>(tmG, tmD, a, ntiles);
 }
 
 }  // namespace rg
