@@ -72,6 +72,82 @@ struct DevBuf {
   DevBuf& operator=(const DevBuf&) = delete;
 };
 
+// Pinned host memory, grown like DevBuf.
+template <typename T>
+struct PinnedBuf {
+  T* p = nullptr;
+  size_t n = 0;
+  void alloc(size_t count) {
+    if (count <= n && p) return;
+    release();
+    RG_CUDA(cudaMallocHost(&p, count * sizeof(T)));
+    n = count;
+  }
+  void release() {
+    if (p) cudaFreeHost(p);
+    p = nullptr;
+    n = 0;
+  }
+  ~PinnedBuf() { release(); }
+  PinnedBuf() = default;
+  PinnedBuf(const PinnedBuf&) = delete;
+  PinnedBuf& operator=(const PinnedBuf&) = delete;
+};
+
+// A non-blocking stream, created by ensure() on first use.  The destructor drains it before destroying it, so a member
+// declared after the buffers its work reads is gone, with its work, before they are freed.
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(Stream&& o) noexcept : s(o.s) { o.s = nullptr; }
+  Stream& operator=(Stream&& o) noexcept {
+    std::swap(s, o.s);
+    return *this;
+  }
+  ~Stream() {
+    if (!s) return;
+    cudaStreamSynchronize(s);
+    cudaStreamDestroy(s);
+  }
+  cudaStream_t ensure() {
+    if (!s) RG_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+    return s;
+  }
+  operator cudaStream_t() const { return s; }
+};
+
+// An event, created by ensure() on first use (without timing unless asked for).
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(Event&& o) noexcept : e(o.e) { o.e = nullptr; }
+  Event& operator=(Event&& o) noexcept {
+    std::swap(e, o.e);
+    return *this;
+  }
+  ~Event() {
+    if (e) cudaEventDestroy(e);
+  }
+  cudaEvent_t ensure(unsigned flags = cudaEventDisableTiming) {
+    if (!e) RG_CUDA(cudaEventCreateWithFlags(&e, flags));
+    return e;
+  }
+  operator cudaEvent_t() const { return e; }
+};
+
+// Another process's device allocation mapped into this one, unmapped by the destructor.
+struct IpcMapping {
+  void* p = nullptr;
+  explicit IpcMapping(const cudaIpcMemHandle_t& mh) {
+    RG_CUDA(cudaIpcOpenMemHandle(&p, mh, cudaIpcMemLazyEnablePeerAccess));
+  }
+  IpcMapping(IpcMapping&& o) noexcept : p(o.p) { o.p = nullptr; }
+  IpcMapping& operator=(IpcMapping&&) = delete;
+  ~IpcMapping() {
+    if (p) cudaIpcCloseMemHandle(p);
+  }
+};
+
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a property of (kernel, DEVICE): several handles on different GPUs may
 // live in one process (rgb200 --gpus N, one host thread per GPU), so the "already set" memo is kept per device.
 inline void ensure_dyn_smem(const void* func, size_t bytes) {

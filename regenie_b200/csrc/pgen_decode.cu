@@ -94,7 +94,6 @@ void pgen_check_errors(rg_ctx* h) {
 }
 
 static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_dev, int64_t* row_stride) {
-  RG_CHECK(h->kind == 1 || h->kind == 2, "bad handle");
   RG_CHECK(b->bs > 0 && b->bs <= h->bs_max, "block size out of range");
   RG_CHECK(b->n_file > 0 && b->n_file < (1ll << 31), "bad sample count");
   RG_CHECK(b->n_rec > 0 && b->n_rec <= 2 * b->bs && b->n_bytes >= 0 && b->n_bytes < (1ll << 40), "bad record table");
@@ -114,16 +113,10 @@ static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_
   RG_CUDA(cudaSetDevice(h->device));
 
   // where the rows go: Step 1 - the input buffer and stream of the lane the next rg_l0_block_bed call takes
-  cudaStream_t s = h->stream;
-  rg::DevBuf<uint8_t>* rows = &h->pgen_rows;
-  rg::DevBuf<uint8_t>* in = &h->pgen_in;
-  if (h->kind == 1) {
-    RG_CHECK(!h->lanes.empty(), "handle has no lanes");
-    rg_ctx::Lane& L = *h->lanes[h->next_lane];
-    s = L.stream;
-    rows = &L.packed_dev;
-    in = &L.pgen_in;
-  }
+  Step1State::Lane* L = h->s1 ? h->s1->lanes[h->s1->next_lane].get() : nullptr;
+  const cudaStream_t s = L ? L->stream : h->stream;
+  rg::DevBuf<uint8_t>& rows = L ? L->packed_dev : h->s2->pgen_rows;
+  rg::DevBuf<uint8_t>& in = L ? L->pgen_in : h->s2->pgen_in;
   const uint32_t n = (uint32_t)b->n_file;
   const uint32_t words = (uint32_t)round_up(ceil_div(n, 16), 4);          // rows are multiples of 16 bytes
   const size_t stride = (size_t)words * 4;
@@ -132,7 +125,7 @@ static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_
     RG_CUDA(cudaMemset(h->pgen_err.p, 0, 8));
   }
   // the host rows of a .bed call may have used the same buffer with another stride: size it for the larger of the two
-  rows->alloc(std::max((size_t)h->bs_max * stride, rows->n));
+  rows.alloc(std::max((size_t)h->bs_max * stride, rows.n));
 
   // one blob: [off u64 n_rec][len u32 n_rec][own i32 bs][base i32 bs][type u8 n_rec] | pad to 16 | record bytes
   const size_t o_len = (size_t)b->n_rec * 8, o_own = o_len + (size_t)b->n_rec * 4, o_base = o_own + (size_t)b->bs * 4,
@@ -144,17 +137,17 @@ static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_
   memcpy(meta.data() + o_base, b->base, (size_t)b->bs * 4);
   memcpy(meta.data() + o_type, b->rec_type, (size_t)b->n_rec);
   const size_t total = o_bytes + (size_t)b->n_bytes + 16;
-  if (total > in->n) in->alloc(total + total / 4 + 4096);                  // grows rarely
-  RG_CUDA(cudaMemcpyAsync(in->p, meta.data(), o_bytes, cudaMemcpyHostToDevice, s));   // pageable: staged before return
-  copy_to_device(in->p + o_bytes, b->bytes, (size_t)b->n_bytes, s);
+  if (total > in.n) in.alloc(total + total / 4 + 4096);                  // grows rarely
+  RG_CUDA(cudaMemcpyAsync(in.p, meta.data(), o_bytes, cudaMemcpyHostToDevice, s));   // pageable: staged before return
+  copy_to_device(in.p + o_bytes, b->bytes, (size_t)b->n_bytes, s);
   PgenMeta m;
-  m.bytes = in->p + o_bytes;
-  m.off = reinterpret_cast<const uint64_t*>(in->p);
-  m.len = reinterpret_cast<const uint32_t*>(in->p + o_len);
-  m.own = reinterpret_cast<const int32_t*>(in->p + o_own);
-  m.base = reinterpret_cast<const int32_t*>(in->p + o_base);
-  m.type = in->p + o_type;
-  uint32_t* out = reinterpret_cast<uint32_t*>(rows->p);
+  m.bytes = in.p + o_bytes;
+  m.off = reinterpret_cast<const uint64_t*>(in.p);
+  m.len = reinterpret_cast<const uint32_t*>(in.p + o_len);
+  m.own = reinterpret_cast<const int32_t*>(in.p + o_own);
+  m.base = reinterpret_cast<const int32_t*>(in.p + o_base);
+  m.type = in.p + o_type;
+  uint32_t* out = reinterpret_cast<uint32_t*>(rows.p);
   const uint32_t tag = (uint32_t)(b->block_id + 1);
   const unsigned gx = (unsigned)std::min<int64_t>(64, ceil_div(words, kFillThreads));
   pgen_fill_kernel<<<dim3(gx, (unsigned)b->bs), kFillThreads, 0, s>>>(m, n, words, out, h->pgen_err.p, tag);
@@ -163,11 +156,11 @@ static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_
                                                                                        h->pgen_err.p, tag);
   RG_CUDA(cudaGetLastError());
   h->launches += 2;
-  if (h->kind == 2) {
+  if (h->s2) {
     RG_CUDA(cudaStreamSynchronize(s));
     pgen_check_errors(h);
   }
-  *rows_dev = rows->p;
+  *rows_dev = rows.p;
   *row_stride = (int64_t)stride;
 }
 

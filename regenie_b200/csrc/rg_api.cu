@@ -29,18 +29,17 @@ void copy_to_device(void* dst, const void* src, size_t bytes, cudaStream_t strea
 struct ScopedTimer {
   rg_ctx* h;
   std::string name;
-  cudaEvent_t a = nullptr, b = nullptr;
+  Event a, b;
   cudaStream_t st;
   ScopedTimer(rg_ctx* h_, const char* n, cudaStream_t s_) : h(h_), name(n), st(s_) {
     if (!h->timing) return;
-    cudaEventCreate(&a);
-    cudaEventCreate(&b);
-    cudaEventRecord(a, st);
+    cudaEventRecord(a.ensure(cudaEventDefault), st);
+    b.ensure(cudaEventDefault);
   }
   ~ScopedTimer() {
     if (!h->timing) return;
     cudaEventRecord(b, st);
-    h->pending.emplace_back(name, a, b);
+    h->pending.emplace_back(name, std::move(a), std::move(b));
   }
 };
 
@@ -52,8 +51,6 @@ void flush_timers(rg_ctx* h) {
     auto& acc = h->timers[std::get<0>(t)];
     acc.first += ms;
     acc.second += 1;
-    cudaEventDestroy(std::get<1>(t));
-    cudaEventDestroy(std::get<2>(t));
   }
   h->pending.clear();
 }
@@ -73,57 +70,57 @@ void require_gpu(int device) {
 }
 
 // Build the padded fold layout + all device state shared by the blocks.
-static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint8_t* mask,
+static void build_layout(rg_ctx* h, Step1State& s1, const double* X, const double* Y, const uint8_t* mask,
                          const uint8_t* in_analysis, const int64_t* fold_sizes) {
   const int64_t N = h->N;
-  const int K = h->K, C = h->C, P = h->P;
-  h->fold_sizes.assign(K, 0);
-  if (h->loocv) {
-    h->fold_sizes[0] = N;
+  const int K = s1.K, C = h->C, P = h->P;
+  s1.fold_sizes.assign(K, 0);
+  if (s1.loocv) {
+    s1.fold_sizes[0] = N;
   } else {
     int64_t tot = 0;
     for (int f = 0; f < K; ++f) {
       RG_CHECK(fold_sizes[f] > 0, "fold sizes must be positive");
-      h->fold_sizes[f] = fold_sizes[f];
+      s1.fold_sizes[f] = fold_sizes[f];
       tot += fold_sizes[f];
     }
     RG_CHECK(tot == N, "fold sizes must sum to n_samples");
   }
-  h->fold_pad_start.assign(K, 0);
-  h->fold_pad_len.assign(K, 0);
+  s1.fold_pad_start.assign(K, 0);
+  s1.fold_pad_len.assign(K, 0);
   int64_t off = 0;
   for (int f = 0; f < K; ++f) {
-    h->fold_pad_start[f] = off;
-    h->fold_pad_len[f] = round_up(h->fold_sizes[f], kFoldPad);
-    off += h->fold_pad_len[f];
+    s1.fold_pad_start[f] = off;
+    s1.fold_pad_len[f] = round_up(s1.fold_sizes[f], kFoldPad);
+    off += s1.fold_pad_len[f];
   }
   h->Npad = off;
   RG_CHECK(h->Npad < (1ll << 31), "padded sample count must fit in int32");
-  h->pad_of.assign(N, 0);
+  s1.pad_of.assign(N, 0);
   h->src_of.assign(h->Npad, -1);
   std::vector<int32_t> tile_fold(h->Npad / 128);
   {
     int64_t s = 0;
     for (int f = 0; f < K; ++f) {
-      for (int64_t o = 0; o < h->fold_sizes[f]; ++o, ++s) {
-        h->pad_of[s] = (int32_t)(h->fold_pad_start[f] + o);
-        h->src_of[h->fold_pad_start[f] + o] = (int32_t)s;
+      for (int64_t o = 0; o < s1.fold_sizes[f]; ++o, ++s) {
+        s1.pad_of[s] = (int32_t)(s1.fold_pad_start[f] + o);
+        h->src_of[s1.fold_pad_start[f] + o] = (int32_t)s;
       }
-      for (int64_t t = h->fold_pad_start[f]; t < h->fold_pad_start[f] + h->fold_pad_len[f]; t += 128)
+      for (int64_t t = s1.fold_pad_start[f]; t < s1.fold_pad_start[f] + s1.fold_pad_len[f]; t += 128)
         tile_fold[t / 128] = f;
     }
   }
   h->in_analysis.assign(in_analysis, in_analysis + N);
 
   // (X | Y) sample-major, zero padded to cpp columns
-  h->cpp = (int)round_up(C + P, 16);
-  std::vector<double> xy((size_t)h->Npad * h->cpp, 0.0);
+  s1.cpp = (int)round_up(C + P, 16);
+  std::vector<double> xy((size_t)h->Npad * s1.cpp, 0.0);
   std::vector<uint8_t> maskp((size_t)P * h->Npad, 0), is_real(h->Npad, 0);
   h->maskh.assign(mask, mask + (size_t)N * P);
   for (int64_t s = 0; s < N; ++s) {
-    const int64_t t = h->pad_of[s];
+    const int64_t t = s1.pad_of[s];
     is_real[t] = 1;
-    double* r = &xy[(size_t)t * h->cpp];
+    double* r = &xy[(size_t)t * s1.cpp];
     for (int c = 0; c < C; ++c) r[c] = X[(size_t)c * N + s];
     for (int p = 0; p < P; ++p) {
       r[C + p] = Y[(size_t)p * N + s];
@@ -144,7 +141,7 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
     };
     int64_t s = 0;
     for (int f = 0; f < K; ++f)
-      for (int64_t o = 0; o < h->fold_sizes[f]; ++o, ++s)
+      for (int64_t o = 0; o < s1.fold_sizes[f]; ++o, ++s)
         for (int c = 0; c < C; ++c) {
           const double xc = X[(size_t)c * N + s];
           if (xc == 0.0) continue;
@@ -165,48 +162,39 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
   std::vector<int2> fold_chunks(K), fold_k(K);
   for (int f = 0; f < K; ++f) {
     fold_chunks[f].x = (int)chunks.size();
-    for (int64_t o = 0; o < h->fold_pad_len[f]; o += kStatChunk) {
-      const int len = (int)std::min<int64_t>(kStatChunk, h->fold_pad_len[f] - o);
-      chunks.push_back(make_int4((int)(h->fold_pad_start[f] + o), len, f, 0));
+    for (int64_t o = 0; o < s1.fold_pad_len[f]; o += kStatChunk) {
+      const int len = (int)std::min<int64_t>(kStatChunk, s1.fold_pad_len[f] - o);
+      chunks.push_back(make_int4((int)(s1.fold_pad_start[f] + o), len, f, 0));
     }
     fold_chunks[f].y = (int)chunks.size();
-    fold_k[f] = make_int2((int)(h->fold_pad_start[f] / 128), (int)(h->fold_pad_len[f] / 128));
+    fold_k[f] = make_int2((int)(s1.fold_pad_start[f] / 128), (int)(s1.fold_pad_len[f] / 128));
   }
-  h->nchunks = (int)chunks.size();
+  s1.nchunks = (int)chunks.size();
 
   cudaStream_t s = h->stream;
-  h->xy.alloc(xy.size());
-  h->mask.alloc(maskp.size());
-  h->is_real.alloc(is_real.size());
-  h->tile_fold.alloc(tile_fold.size());
-  h->chunks.alloc(chunks.size());
-  h->fold_chunks.alloc(K);
-  h->fold_k.alloc(K);
-  h->XtX_f.alloc(XtX.size());
-  h->XtY_f.alloc(XtY.size());
-  RG_CUDA(cudaMemcpyAsync(h->xy.p, xy.data(), xy.size() * 8, cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->mask.p, maskp.data(), maskp.size(), cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->is_real.p, is_real.data(), is_real.size(), cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->tile_fold.p, tile_fold.data(), tile_fold.size() * 4, cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->chunks.p, chunks.data(), chunks.size() * sizeof(int4), cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->fold_chunks.p, fold_chunks.data(), K * sizeof(int2), cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->fold_k.p, fold_k.data(), K * sizeof(int2), cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->XtX_f.p, XtX.data(), XtX.size() * 8, cudaMemcpyHostToDevice, s));
-  RG_CUDA(cudaMemcpyAsync(h->XtY_f.p, XtY.data(), XtY.size() * 8, cudaMemcpyHostToDevice, s));
+  upload(s1.xy, xy, s);
+  upload(s1.mask, maskp, s);
+  upload(s1.is_real, is_real, s);
+  upload(s1.tile_fold, tile_fold, s);
+  upload(s1.chunks, chunks, s);
+  upload(s1.fold_chunks, fold_chunks, s);
+  upload(s1.fold_k, fold_k, s);
+  upload(s1.XtX_f, XtX, s);
+  upload(s1.XtY_f, XtY, s);
   // statistics as extra Gram tiles: digit rows of (X | Y), once per run.  Exact while 30 * fold length < 2^24.
   {
     int64_t max_fold = 0;
-    for (int f = 0; f < K; ++f) max_fold = std::max(max_fold, h->fold_pad_len[f]);
+    for (int f = 0; f < K; ++f) max_fold = std::max(max_fold, s1.fold_pad_len[f]);
     const char* e = getenv("RG_B200_STATS");
-    h->stats_tc = !(e && std::string(e) == "f64") && max_fold * 30 < (1ll << 24);
-    if (h->stats_tc) {
+    s1.stats_tc = !(e && std::string(e) == "f64") && max_fold * 30 < (1ll << 24);
+    if (s1.stats_tc) {
       const int ngroups = (int)ceil_div(C + P, kStatQ);
-      h->stat_drows = ngroups * 128;          // an odd group count runs as 128 x 128 tiles (stat_bn)
-      h->xyD.alloc((size_t)h->stat_drows * h->Npad);
-      h->xy_scale.alloc(h->cpp);
-      RG_CUDA(cudaMemsetAsync(h->xyD.p, 0, (size_t)h->stat_drows * h->Npad, s));
-      launch_l0_xy_digits(h->xy.p, h->cpp, C + P, h->Npad, h->is_real.p, h->xy_scale.p, h->xyD.p, s);
-      make_gram_tensor_map(&h->tmD, h->xyD.p, h->Npad, h->stat_drows);
+      s1.stat_drows = ngroups * 128;          // an odd group count runs as 128 x 128 tiles (stat_bn)
+      s1.xyD.alloc((size_t)s1.stat_drows * h->Npad);
+      s1.xy_scale.alloc(s1.cpp);
+      RG_CUDA(cudaMemsetAsync(s1.xyD.p, 0, (size_t)s1.stat_drows * h->Npad, s));
+      launch_l0_xy_digits(s1.xy.p, s1.cpp, C + P, h->Npad, s1.is_real.p, s1.xy_scale.p, s1.xyD.p, s);
+      make_gram_tensor_map(&s1.tmD, s1.xyD.p, h->Npad, s1.stat_drows);
     }
   }
   // Miss rows of the Gram as sparse sums while a block has at most kMissSparseRate missing calls (miss_gram.cu)
@@ -214,26 +202,23 @@ static void build_layout(rg_ctx* h, const double* X, const double* Y, const uint
     // RG_B200_GRAM=dense: always the dense tiles; =sparse: a list for every call (tools/miss_rate_sweep.py)
     const char* e = getenv("RG_B200_GRAM");
     const std::string mode = e ? e : "";
-    h->gram_dense = mode == "dense";
+    s1.gram_dense = mode == "dense";
     const double rate = mode == "sparse" ? 1.0 : kMissSparseRate;
-    h->miss_cap = std::min<int64_t>((int64_t)(rate * h->bs_max * h->n_analyzed), INT32_MAX);
+    s1.miss_cap = std::min<int64_t>((int64_t)(rate * h->bs_max * h->n_analyzed), INT32_MAX);
     // the relayout's column tiles: 512 samples (32 words) each, cut at the fold ends so that a tile's calls belong to
     // one fold
     std::vector<int2> fold_ct(K);
-    h->miss_ctile_host.clear();
+    s1.miss_ctile_host.clear();
     for (int f = 0; f < K; ++f) {
-      fold_ct[f].x = (int)h->miss_ctile_host.size();
-      const int64_t w1 = (h->fold_pad_start[f] + h->fold_pad_len[f]) / 16;
-      for (int64_t w = h->fold_pad_start[f] / 16; w < w1; w += 32)
-        h->miss_ctile_host.push_back(make_int4((int)w, (int)std::min<int64_t>(32, w1 - w), f, 0));
-      fold_ct[f].y = (int)h->miss_ctile_host.size();
+      fold_ct[f].x = (int)s1.miss_ctile_host.size();
+      const int64_t w1 = (s1.fold_pad_start[f] + s1.fold_pad_len[f]) / 16;
+      for (int64_t w = s1.fold_pad_start[f] / 16; w < w1; w += 32)
+        s1.miss_ctile_host.push_back(make_int4((int)w, (int)std::min<int64_t>(32, w1 - w), f, 0));
+      fold_ct[f].y = (int)s1.miss_ctile_host.size();
     }
-    h->miss_nct = (int)h->miss_ctile_host.size();
-    h->miss_ctile.alloc(h->miss_nct);
-    h->miss_fold_ct.alloc(K);
-    RG_CUDA(cudaMemcpyAsync(h->miss_ctile.p, h->miss_ctile_host.data(), h->miss_nct * sizeof(int4),
-                            cudaMemcpyHostToDevice, s));
-    RG_CUDA(cudaMemcpyAsync(h->miss_fold_ct.p, fold_ct.data(), K * sizeof(int2), cudaMemcpyHostToDevice, s));
+    s1.miss_nct = (int)s1.miss_ctile_host.size();
+    upload(s1.miss_ctile, s1.miss_ctile_host, s);
+    upload(s1.miss_fold_ct, fold_ct, s);
   }
   RG_CUDA(cudaStreamSynchronize(s));   // host vectors go out of scope
 }
@@ -262,12 +247,9 @@ static void build_file_idx(rg_ctx* h, const int32_t* sample_idx_host) {
     }
     wb[w] = (wk[w] == 0) ? -1 : ((contiguous && base >= 0) ? base : -2);
   }
-  h->file_idx_pad.alloc(h->Npad);
-  h->word_base.alloc(nw);
-  h->word_keep.alloc(nw);
-  RG_CUDA(cudaMemcpyAsync(h->word_base.p, wb.data(), nw * 4, cudaMemcpyHostToDevice, h->stream));
-  RG_CUDA(cudaMemcpyAsync(h->word_keep.p, wk.data(), nw * 4, cudaMemcpyHostToDevice, h->stream));
-  RG_CUDA(cudaMemcpyAsync(h->file_idx_pad.p, fi.data(), fi.size() * 4, cudaMemcpyHostToDevice, h->stream));
+  upload(h->word_base, wb, h->stream);
+  upload(h->word_keep, wk, h->stream);
+  upload(h->file_idx_pad, fi, h->stream);
   RG_CUDA(cudaStreamSynchronize(h->stream));
   h->file_idx_valid = true;
 }
@@ -293,17 +275,29 @@ void ensure_file_idx(rg_ctx* h, const int32_t* sample_idx) {
 // Storage of the level-0 predictors, allocated on first use: one compact slab per phenotype this rank owns
 // (all of them unless rg_W_set_owned said otherwise); entries of phenotypes owned elsewhere stay null until
 // rg_W_attach_peer maps the owner's memory.
-void ensure_W(::rg_ctx* h) {
-  if (h->W.p) return;
+void ensure_W(rg_ctx* h, Step1State& s1) {
+  if (s1.W.p) return;
   size_t n_owned = 0;
-  for (int p = 0; p < h->P; ++p) n_owned += h->W_owned[p] ? 1 : 0;
-  const size_t per = (size_t)h->Npad * h->B;
-  h->W.alloc(std::max<size_t>(1, n_owned) * per);
-  RG_CUDA(cudaMemset(h->W.p, 0, std::max<size_t>(1, n_owned) * per * 8));
+  for (int p = 0; p < h->P; ++p) n_owned += s1.W_owned[p] ? 1 : 0;
+  const size_t per = (size_t)h->Npad * s1.B;
+  s1.W.alloc(std::max<size_t>(1, n_owned) * per);
+  RG_CUDA(cudaMemset(s1.W.p, 0, std::max<size_t>(1, n_owned) * per * 8));
   size_t slot = 0;
   for (int p = 0; p < h->P; ++p)
-    if (h->W_owned[p]) h->W_host_tab[p] = h->W.p + (slot++) * per;
-  RG_CUDA(cudaMemcpy(h->W_tab.p, h->W_host_tab.data(), h->P * sizeof(double*), cudaMemcpyHostToDevice));
+    if (s1.W_owned[p]) s1.W_host_tab[p] = s1.W.p + (slot++) * per;
+  RG_CUDA(cudaMemcpy(s1.W_tab.p, s1.W_host_tab.data(), h->P * sizeof(double*), cudaMemcpyHostToDevice));
+}
+
+// Points the phenotypes owned_by_peer at the owner's W, which is compact over the phenotypes the owner holds
+// (rg_W_set_owned with the same mask there), and leaves their level-1 fits to the owner.
+static void attach_W(rg_ctx* h, Step1State& s1, double* owner_W, const uint8_t* owned_by_peer) {
+  size_t slot = 0;
+  for (int p = 0; p < h->P; ++p)
+    if (owned_by_peer[p]) {
+      s1.W_host_tab[p] = owner_W + (slot++) * (size_t)h->Npad * s1.B;
+      s1.l1_select[p] = 0;
+    }
+  RG_CUDA(cudaMemcpy(s1.W_tab.p, s1.W_host_tab.data(), h->P * sizeof(double*), cudaMemcpyHostToDevice));
 }
 
 struct BlockDims {
@@ -314,20 +308,20 @@ static int mx_pp(int P) { return (int)round_up(P, 2); }
 constexpr int kMxSteps = 3;               // refinement steps of the mixed solver
 
 // Assembler arguments the FP64 and the mixed path share; each path adds the layout of its systems (nC, cm, cm_stride, ldc).
-static AssembleArgs assemble_args(const rg_ctx* h, const rg_ctx::Lane& L, const BlockDims& d) {
+static AssembleArgs assemble_args(const rg_ctx* h, const Step1State& s1, const Step1State::Lane& L, const BlockDims& d) {
   AssembleArgs aa;
-  aa.bs = d.bs; aa.rows_p = d.rows_p; aa.C = h->C; aa.K = h->K; aa.R = h->R; aa.loocv = h->loocv;
+  aa.bs = d.bs; aa.rows_p = d.rows_p; aa.C = h->C; aa.K = s1.K; aa.R = s1.R; aa.loocv = s1.loocv;
   aa.zz = L.zz.p; aa.ldz = 2 * d.rows_p; aa.zz_fold_stride = (int64_t)4 * d.rows_p * d.rows_p;
   aa.mu = L.mu.p; aa.inv_sd = L.inv_sd.p; aa.Bv = L.Bv.p; aa.Af = L.Af.p; aa.Qf = L.Qf.p;
-  aa.lambda = h->lambda.p;
+  aa.lambda = s1.lambda.p;
   return aa;
 }
 
 // The lane's FP64 systems [nmat][n_aug][nC] (LOOCV: the sample vectors ride along as right-hand-side rows) and the
 // inverses of their diagonal blocks, sized for the largest block of the run; the systems are zeroed when allocated.
-static void ensure_f64_systems(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cudaStream_t s) {
+static void ensure_f64_systems(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
   const int nC_max = (int)round_up(h->bs_max, 64);
-  const size_t need = (size_t)d.nmat * (nC_max + d.Ppad + (h->loocv ? h->Npad : 0)) * nC_max;
+  const size_t need = (size_t)d.nmat * (nC_max + d.Ppad + (s1.loocv ? h->Npad : 0)) * nC_max;
   if (L.cm.n < need) {
     L.cm.alloc(need);
     RG_CUDA(cudaMemsetAsync(L.cm.p, 0, need * 8, s));
@@ -337,42 +331,42 @@ static void ensure_f64_systems(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, c
 
 // LOOCV: closed-form leave-one-out predictions from the factorised systems (src/Step1_Models.cpp:654-663), standardised
 // into W (:694-706)
-static void enqueue_loocv_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cudaStream_t s) {
+static void enqueue_loocv_predict(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
   const int P = h->P;
-  launch_l0_loocv_pred(L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.bs, d.Ppad, P, h->R, h->xy.p, h->cpp, h->C, h->mask.p, h->Npad,
-                       h->W_tab.p, d.col0, L.part.p, d.Qp, s);
-  launch_l0_std_reduce_only(L.part.p, d.ntiles_s, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, s);
-  launch_l0_loocv_std_apply(h->W_tab.p, h->Npad, d.col0, P, d.Q, h->mask.p, L.mean_invsd.p, s);
+  launch_l0_loocv_pred(L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.bs, d.Ppad, P, s1.R, s1.xy.p, s1.cpp, h->C, s1.mask.p, h->Npad,
+                       s1.W_tab.p, d.col0, L.part.p, d.Qp, s);
+  launch_l0_std_reduce_only(L.part.p, d.ntiles_s, d.Qp, d.Q, P, s1.neff.p, L.mean_invsd.p, s);
+  launch_l0_loocv_std_apply(s1.W_tab.p, h->Npad, d.col0, P, d.Q, s1.mask.p, L.mean_invsd.p, s);
   h->launches += 3;
 }
 
 // FP64 path: assemble the K*R shifted systems, batched Cholesky (DMMA), backward substitution; LOOCV predictions
 // included (they read the factorisation directly).  Solutions end up in the right-hand-side rows of L.cm.
-static void enqueue_solve_f64(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cudaStream_t s) {
-  const int C = h->C, P = h->P, R = h->R;
-  ensure_f64_systems(h, L, d, s);
-  AssembleArgs aa = assemble_args(h, L, d);
+static void enqueue_solve_f64(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
+  const int C = h->C, P = h->P, R = s1.R;
+  ensure_f64_systems(h, s1, L, d, s);
+  AssembleArgs aa = assemble_args(h, s1, L, d);
   aa.nC = d.nC; aa.cm = L.cm.p; aa.cm_stride = (int64_t)d.n_aug * d.nC; aa.ldc = d.nC;
   {
     ScopedTimer t(h, "l0_assemble", s);
     launch_l0_assemble(aa, L.rhs.p, P, d.Ppad, d.nmat, s);
     h->launches += 2;
   }
-  if (h->loocv) {
+  if (s1.loocv) {
     ScopedTimer t(h, "loocv_fill", s);
-    launch_l0_loocv_fill(L.gp.p, h->Npad, d.bs, d.nC, L.mu.p, L.inv_sd.p, L.Bv.p, C, h->xy.p, h->cpp, L.cm.p, aa.cm_stride,
+    launch_l0_loocv_fill(L.gp.p, h->Npad, d.bs, d.nC, L.mu.p, L.inv_sd.p, L.Bv.p, C, s1.xy.p, s1.cpp, L.cm.p, aa.cm_stride,
                          d.nC + d.Ppad, R, s);
     h->launches += 1;
   }
   {
     ScopedTimer t(h, "chol_factor", s);
-    launch_chol_factor(L.cm.p, aa.cm_stride, d.nC, d.n_aug, d.nmat, L.inv.p, h->err_slot.p,
+    launch_chol_factor(L.cm.p, aa.cm_stride, d.nC, d.n_aug, d.nmat, L.inv.p, s1.err_slot.p,
                        (long long)(1ll << 40) + (long long)d.block_id * 1024, s);
     h->launches += chol_num_launches(d.nC);
   }
-  if (h->loocv) {
+  if (s1.loocv) {
     ScopedTimer t(h, "l0_predict", s);
-    enqueue_loocv_predict(h, L, d, s);
+    enqueue_loocv_predict(h, s1, L, d, s);
     return;
   }
   {
@@ -383,14 +377,14 @@ static void enqueue_solve_f64(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cu
 }
 
 // Mixed path: K symmetric FP64 fold systems -> tensor-core factorisation / inverse -> FP64 refinement.  Solutions in L.mx_x.
-static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, int n, cudaStream_t s) {
-  const int P = h->P, K = h->K, R = h->R;
+static void enqueue_solve_mixed(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, int n, cudaStream_t s) {
+  const int P = h->P, K = s1.K, R = s1.R;
   const int Pp = mx_pp(P);
   if (!L.mx) {
     L.mx = std::make_unique<MixedSolver>();
     L.mx_fail.alloc(1);
-    RG_CUDA(cudaMallocHost(&L.mx_fail_host, sizeof(unsigned int)));
-    RG_CUDA(cudaEventCreateWithFlags(&L.mx_ev, cudaEventDisableTiming));
+    L.mx_fail_host.alloc(1);
+    L.mx_ev.ensure();
   }
   // sized from the block being solved: with bsize > 2048 the largest blocks take the FP64 path, but a chromosome's short
   // last block still comes here (alloc is a no-op once the buffers are large enough)
@@ -403,7 +397,7 @@ static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, 
            "mixed solver: scratch smaller than the block's systems");
   L.mx->prepare(n, K, R, Pp);
   RG_CUDA(cudaMemsetAsync(L.mx_fail.p, 0, sizeof(unsigned int), s));
-  AssembleArgs aa = assemble_args(h, L, d);
+  AssembleArgs aa = assemble_args(h, s1, L, d);
   aa.nC = n; aa.cm = L.mx_Af.p; aa.cm_stride = (int64_t)n * n; aa.ldc = n;
   aa.planes = L.mx->a_planes();
   aa.lplanes = L.mx->l_planes();           // block column 0 of the factor: the solver skips its first update
@@ -414,37 +408,36 @@ static void enqueue_solve_mixed(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, 
   }
   {
     ScopedTimer t(h, "mx_solve", s);
-    L.mx->solve(L.mx_Af.p, h->lambda.p, L.mx_b.p, L.mx_x.p, L.mx_r.p, P, kMxSteps, h->mx_tol, L.mx_fail.p, s, true);
+    L.mx->solve(L.mx_Af.p, s1.lambda.p, L.mx_b.p, L.mx_x.p, L.mx_r.p, P, kMxSteps, s1.mx_tol, L.mx_fail.p, s, true);
     h->launches += MixedSolver::launches_per_solve(n, kMxSteps, P) - 1;
   }
 }
 
 // Tensor map of the lane's 2-bit rows.
-static const CUtensorMap& gp_map(const rg_ctx* h, rg_ctx::Lane& L, int rows_p) {
+static const CUtensorMap& gp_map(const rg_ctx* h, Step1State::Lane& L, int rows_p) {
   return gp_tensor_map(L.gmaps, L.gp.p, h->Npad, rows_p);
 }
 
 // Out-of-fold predictions from the coefficients x[m][p][i] at xsrc + m * xstride + (xrow0 + p) * xld + i.
-static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, const double* xsrc, int64_t xstride, int xld,
-                            int xrow0, cudaStream_t s) {
-  const int C = h->C, P = h->P, K = h->K, R = h->R;
+static void enqueue_predict(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, const double* xsrc,
+                            int64_t xstride, int xld, int xrow0, cudaStream_t s) {
+  const int C = h->C, P = h->P, K = s1.K, R = s1.R;
   const int64_t Npad = h->Npad;
   ScopedTimer t(h, "l0_predict", s);
   // raw predictions go to the lane's LOCAL scratch; the standardisation pass reads them there and writes the finished
   // columns into W - the owner's HBM, which may be another GPU's (then only plain stores cross NVLink)
   if (L.wraw.n < (size_t)P * R * Npad) {
     L.wraw.alloc((size_t)P * R * Npad);
-    L.wraw_tab.alloc(P);
     std::vector<double*> tab(P);
     for (int p = 0; p < P; ++p) tab[p] = L.wraw.p + (size_t)p * R * Npad;
-    RG_CUDA(cudaMemcpyAsync(L.wraw_tab.p, tab.data(), P * sizeof(double*), cudaMemcpyHostToDevice, s));
+    upload(L.wraw_tab, tab, s);
     RG_CUDA(cudaStreamSynchronize(s));           // tab goes out of scope (once per lane)
   }
   PredictArgs pa;
-  pa.bs = d.bs; pa.rows_p = d.rows_p; pa.C = C; pa.P = P; pa.R = R; pa.Qp = d.Qp; pa.cpp = h->cpp;
+  pa.bs = d.bs; pa.rows_p = d.rows_p; pa.C = C; pa.P = P; pa.R = R; pa.Qp = d.Qp; pa.cpp = s1.cpp;
   pa.col0 = 0; pa.npad = Npad; pa.words_per_row = Npad / 16;
-  pa.gp = L.gp.p; pa.tile_fold = h->tile_fold.p; pa.gam = L.gam.p; pa.gmu = L.gmu.p;
-  pa.cvec = L.cvec.p; pa.xy = h->xy.p; pa.mask = h->mask.p; pa.W = L.wraw_tab.p; pa.part = L.part.p;
+  pa.gp = L.gp.p; pa.tile_fold = s1.tile_fold.p; pa.gam = L.gam.p; pa.gmu = L.gmu.p;
+  pa.cvec = L.cvec.p; pa.xy = s1.xy.p; pa.mask = s1.mask.p; pa.W = L.wraw_tab.p; pa.part = L.part.p;
   // INT8 tensor cores (s8 wgmma, 5 radix-254 limbs) up to 2 rows_p = 4096; the FP64 CUDA-core kernel beyond (bsize > 2048).
   // Both leave per-tile column sums in L.part.
   const bool use_i8 = 2 * d.rows_p <= 4096;
@@ -473,73 +466,74 @@ static void enqueue_predict(rg_ctx* h, rg_ctx::Lane& L, const BlockDims& d, cons
     launch_l0_coef_i8(xsrc, xstride, xld, xrow0, R, P, d.Q, d.Qp, d.bs, d.rows_p, K, L.mu.p, L.inv_sd.p, L.Bv.p, C,
                       L.gam.p, L.gmu.p, L.cvec.p, L.dscale.p, L.dig.p, ngroups, s);
     PredictTcArgs ta;
-    ta.rows_p = d.rows_p; ta.C = C; ta.P = P; ta.Q = d.Q; ta.Qp = d.Qp; ta.cpp = h->cpp; ta.col0 = 0; ta.ngroups = ngroups;
-    ta.npad = Npad; ta.tile_fold = h->tile_fold.p; ta.scale = L.dscale.p; ta.cvec = L.cvec.p;
-    ta.xy = h->xy.p; ta.mask = h->mask.p; ta.W = L.wraw_tab.p; ta.part = L.part.p;
+    ta.rows_p = d.rows_p; ta.C = C; ta.P = P; ta.Q = d.Q; ta.Qp = d.Qp; ta.cpp = s1.cpp; ta.col0 = 0; ta.ngroups = ngroups;
+    ta.npad = Npad; ta.tile_fold = s1.tile_fold.p; ta.scale = L.dscale.p; ta.cvec = L.cvec.p;
+    ta.xy = s1.xy.p; ta.mask = s1.mask.p; ta.W = L.wraw_tab.p; ta.part = L.part.p;
     launch_l0_predict_i8(gp_map(h, L, d.rows_p), L.dmaps[d.rows_p], ta, d.ntiles_s, s);
     h->launches += 2;
   }
-  launch_l0_standardize(L.part.p, d.ntiles_s, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, h->W_tab.p, Npad, d.col0,
-                        h->is_real.p, s, L.wraw_tab.p, 0);
+  launch_l0_standardize(L.part.p, d.ntiles_s, d.Qp, d.Q, P, s1.neff.p, L.mean_invsd.p, s1.W_tab.p, Npad, d.col0,
+                        s1.is_real.p, s, L.wraw_tab.p, 0);
   h->launches += 2;
 }
 
-static BlockDims block_dims(const rg_ctx* h, int bs, int block_id) {
+static BlockDims block_dims(const rg_ctx* h, const Step1State& s1, int bs, int block_id) {
   BlockDims d;
   d.bs = bs; d.rows_p = (int)round_up(bs, kRowPad); d.nC = (int)round_up(bs, 64); d.Ppad = (int)round_up(h->P, 64);
-  d.n_aug = d.nC + d.Ppad + (h->loocv ? (int)h->Npad : 0);
-  d.nmat = (h->loocv ? 1 : h->K) * h->R;
-  d.Q = h->R * h->P; d.Qp = (int)round_up(d.Q, predict_qt());
-  d.col0 = block_id * h->R; d.block_id = block_id; d.ntiles_s = (int)(h->Npad / 128);
+  d.n_aug = d.nC + d.Ppad + (s1.loocv ? (int)h->Npad : 0);
+  d.nmat = (s1.loocv ? 1 : s1.K) * s1.R;
+  d.Q = s1.R * h->P; d.Qp = (int)round_up(d.Q, predict_qt());
+  d.col0 = block_id * s1.R; d.block_id = block_id; d.ntiles_s = (int)(h->Npad / 128);
   return d;
 }
 
 // Read the mixed-solver flag of the block this lane ran last; if the refinement did not converge (ill-conditioned
 // system) or a pivot was not positive, re-solve that block in FP64 from the lane's scratch (statistics, Grams and 2-bit
 // rows of the block are still there) and redo its predictions.
-void resolve_lane(rg_ctx* h, rg_ctx::Lane& L) {
+void resolve_lane(rg_ctx* h, Step1State& s1, Step1State::Lane& L) {
   if (!L.mx_pending) return;
   RG_CUDA(cudaEventSynchronize(L.mx_ev));
   L.mx_pending = false;
-  if (*L.mx_fail_host == 0) return;
-  h->mx_fallbacks += 1;
+  if (*L.mx_fail_host.p == 0) return;
+  s1.mx_fallbacks += 1;
   L.last_mx_n = 0;
-  const BlockDims d = block_dims(h, L.mx_bs, L.mx_block_id);
-  enqueue_solve_f64(h, L, d, L.stream);
-  enqueue_predict(h, L, d, L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.nC, L.stream);
+  const BlockDims d = block_dims(h, s1, L.mx_bs, L.mx_block_id);
+  enqueue_solve_f64(h, s1, L, d, L.stream);
+  enqueue_predict(h, s1, L, d, L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.nC, L.stream);
 }
 
 void sync_lanes(rg_ctx* h) {
   RG_CUDA(cudaSetDevice(h->device));
-  for (auto& l : h->lanes) resolve_lane(h, *l);
-  for (auto& l : h->lanes) RG_CUDA(cudaStreamSynchronize(l->stream));
+  if (!h->s1) return;
+  for (auto& l : h->s1->lanes) resolve_lane(h, *h->s1, *l);
+  for (auto& l : h->s1->lanes) RG_CUDA(cudaStreamSynchronize(l->stream));
 }
 
 // What both level-0 block routes do first: check the call, map the samples of the genotype file, take the next lane and
 // record the block's dimensions (rg_debug_fetch "dims").  Each route reads the flag of the lane's previous block itself
 // (resolve_lane), because the .bed route enqueues its input copy before the host waits on that flag.
-static rg_ctx::Lane& l0_begin_block(rg_ctx* h, int bs, int block_id, const int32_t* sample_idx, BlockDims& d) {
-  RG_CHECK(h->kind == 1, "handle is not a Step-1 handle");
+static Step1State::Lane& l0_begin_block(rg_ctx* h, Step1State& s1, int bs, int block_id, const int32_t* sample_idx, BlockDims& d) {
   RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
-  RG_CHECK(block_id >= 0 && block_id < h->total_blocks, "block_id out of range");
-  ensure_W(h);
+  RG_CHECK(block_id >= 0 && block_id < s1.total_blocks, "block_id out of range");
+  ensure_W(h, s1);
   for (int p = 0; p < h->P; ++p)
-    RG_CHECK(h->W_host_tab[p] != nullptr, "a phenotype has neither local storage nor an attached owner (rg_W_set_owned / rg_W_attach_peer)");
+    RG_CHECK(s1.W_host_tab[p] != nullptr, "a phenotype has neither local storage nor an attached owner (rg_W_set_owned / rg_W_attach_peer)");
   RG_CUDA(cudaSetDevice(h->device));
   ensure_file_idx(h, sample_idx);
-  rg_ctx::Lane& L = *h->lanes[h->next_lane];
-  h->last_lane = h->next_lane;
-  h->next_lane = (h->next_lane + 1) % (int)h->lanes.size();
-  d = block_dims(h, bs, block_id);
-  h->last_bs = bs; h->last_rows_p = d.rows_p; h->last_nC = d.nC; h->last_n_aug = d.n_aug; h->last_nmat = d.nmat;
+  Step1State::Lane& L = *s1.lanes[s1.next_lane];
+  s1.last_lane = s1.next_lane;
+  s1.next_lane = (s1.next_lane + 1) % (int)s1.lanes.size();
+  d = block_dims(h, s1, bs, block_id);
+  s1.last_bs = bs; s1.last_rows_p = d.rows_p; s1.last_nC = d.nC; s1.last_n_aug = d.n_aug; s1.last_nmat = d.nmat;
   return L;
 }
 
 static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, int bs,
                          const int32_t* sample_idx, int ref_first, int block_id) {
+  Step1State& s1 = step1(h);
   BlockDims d;
-  rg_ctx::Lane& L = l0_begin_block(h, bs, block_id, sample_idx, d);
-  const int C = h->C, P = h->P, K = h->K;
+  Step1State::Lane& L = l0_begin_block(h, s1, bs, block_id, sample_idx, d);
+  const int C = h->C, P = h->P, K = s1.K;
   const int rows_p = d.rows_p, Qp = d.Qp;
   const int64_t Npad = h->Npad;
   cudaStream_t s = L.stream;
@@ -552,29 +546,26 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
     staged = (L.packed_flip ^= 1);
     rg::DevBuf<uint8_t>& buf = L.packed_buf[staged];
     buf.alloc((size_t)h->bs_max * row_stride);
-    if (!L.copy_stream) RG_CUDA(cudaStreamCreateWithFlags(&L.copy_stream, cudaStreamNonBlocking));
-    if (!L.h2d_done) RG_CUDA(cudaEventCreateWithFlags(&L.h2d_done, cudaEventDisableTiming));
-    cudaStream_t cs = L.copy_stream;
+    cudaStream_t cs = L.copy_stream.ensure();
     // the buffer was last read by the relayout kernel of the block this lane ran two blocks ago
-    if (L.relayout_recorded[staged]) RG_CUDA(cudaStreamWaitEvent(cs, L.relayout_done[staged], 0));
+    if (L.relayout_done[staged]) RG_CUDA(cudaStreamWaitEvent(cs, L.relayout_done[staged], 0));
     {
       ScopedTimer t(h, "h2d", cs);
       copy_to_device(buf.p, packed, (size_t)bs * row_stride, cs);
     }
-    RG_CUDA(cudaEventRecord(L.h2d_done, cs));
-    L.h2d_recorded = true;
+    RG_CUDA(cudaEventRecord(L.h2d_done.ensure(), cs));
     RG_CUDA(cudaStreamWaitEvent(s, L.h2d_done, 0));
     packed_d = buf.p;
   }
-  resolve_lane(h, L);                      // flag of the block this lane ran before (FP64 re-solve if it was raised)
+  resolve_lane(h, s1, L);                      // flag of the block this lane ran before (FP64 re-solve if it was raised)
 
   // --- scratch
   L.gp.alloc((size_t)h->rows_p_max * (Npad / 16));
   L.zz.alloc((size_t)K * 4 * h->rows_p_max * h->rows_p_max);
-  L.cnt_part.alloc((size_t)h->nchunks * h->rows_p_max * 4);
-  L.sum_part.alloc((size_t)h->nchunks * h->rows_p_max * 2 * h->cpp);
+  L.cnt_part.alloc((size_t)s1.nchunks * h->rows_p_max * 4);
+  L.sum_part.alloc((size_t)s1.nchunks * h->rows_p_max * 2 * s1.cpp);
   L.cnt_fold.alloc((size_t)K * h->rows_p_max * 4);
-  L.sum_fold.alloc((size_t)K * h->rows_p_max * 2 * h->cpp);
+  L.sum_fold.alloc((size_t)K * h->rows_p_max * 2 * s1.cpp);
   L.mu.alloc(h->rows_p_max);
   L.inv_sd.alloc(h->rows_p_max);
   L.Bv.alloc((size_t)h->rows_p_max * C);
@@ -582,7 +573,7 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   L.Qf.alloc((size_t)K * h->rows_p_max * C);
   L.gty_f.alloc((size_t)K * h->rows_p_max * P);
   L.rhs.alloc((size_t)K * h->rows_p_max * P);
-  const int Kg = h->loocv ? 1 : K;
+  const int Kg = s1.loocv ? 1 : K;
   L.gam.alloc((size_t)Kg * h->rows_p_max * Qp);
   L.gmu.alloc((size_t)Kg * h->rows_p_max * Qp);
   L.cvec.alloc((size_t)Kg * Qp * C);
@@ -593,47 +584,43 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
   //        sparse Miss path the same pass writes the missing lists and the sample-major rows Gt (miss_gram.cu)
   {
     ScopedTimer t(h, "bed_relayout", s);
-    if (h->gram_dense) {
+    if (s1.gram_dense) {
       launch_bed_relayout(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p,
                           ref_first, L.gp.p, Npad, s);
     } else {
       L.miss_total.alloc(1);
-      L.miss_seg.alloc((size_t)h->rows_p_max * h->miss_nct);
-      L.miss_list.alloc((size_t)std::max<int64_t>(h->miss_cap, 1));
+      L.miss_seg.alloc((size_t)h->rows_p_max * s1.miss_nct);
+      L.miss_list.alloc((size_t)std::max<int64_t>(s1.miss_cap, 1));
       L.gt.alloc((size_t)Npad * (h->rows_p_max / 16));
       BedMissOut mo;
-      mo.ctile = h->miss_ctile.p; mo.nct = h->miss_nct; mo.rows_p = rows_p;
-      mo.total = L.miss_total.p; mo.cap = (unsigned long long)h->miss_cap;
+      mo.ctile = s1.miss_ctile.p; mo.nct = s1.miss_nct; mo.rows_p = rows_p;
+      mo.total = L.miss_total.p; mo.cap = (unsigned long long)s1.miss_cap;
       mo.seg = L.miss_seg.p; mo.list = L.miss_list.p; mo.gt = L.gt.p;
       launch_bed_relayout_miss(packed_d, row_stride, bs, rows_p, h->file_idx_pad.p, h->word_base.p, h->word_keep.p,
                                ref_first, L.gp.p, Npad, mo, s);
       h->launches += 1;                    // the memset of the total
     }
-    if (staged >= 0) {
-      if (!L.relayout_done[staged]) RG_CUDA(cudaEventCreateWithFlags(&L.relayout_done[staged], cudaEventDisableTiming));
-      RG_CUDA(cudaEventRecord(L.relayout_done[staged], s));
-      L.relayout_recorded[staged] = true;
-    }
+    if (staged >= 0) RG_CUDA(cudaEventRecord(L.relayout_done[staged].ensure(), s));
   }
   h->launches += 1;
 
   // --- 2. sufficient statistics: FP64 CUDA-core path (fallback) or, after the Gram, as extra tensor-core tiles
   auto snp_finalize = [&]() {
     SnpFinalizeArgs a;
-    a.bs = bs; a.rows_p = rows_p; a.C = C; a.P = P; a.K = K; a.cpp = h->cpp; a.loocv = h->loocv;
+    a.bs = bs; a.rows_p = rows_p; a.C = C; a.P = P; a.K = K; a.cpp = s1.cpp; a.loocv = s1.loocv;
     a.n_analyzed = h->n_analyzed; a.numtol = 1e-6;
-    a.cnt_fold = L.cnt_fold.p; a.sum_fold = L.sum_fold.p; a.XtX_f = h->XtX_f.p; a.XtY_f = h->XtY_f.p;
+    a.cnt_fold = L.cnt_fold.p; a.sum_fold = L.sum_fold.p; a.XtX_f = s1.XtX_f.p; a.XtY_f = s1.XtY_f.p;
     a.mu = L.mu.p; a.inv_sd = L.inv_sd.p; a.Bv = L.Bv.p; a.Af = L.Af.p; a.Qf = L.Qf.p;
-    a.gty_f = L.gty_f.p; a.rhs = L.rhs.p; a.err_slot = h->err_slot.p;
+    a.gty_f = L.gty_f.p; a.rhs = L.rhs.p; a.err_slot = s1.err_slot.p;
     a.err_base = (long long)block_id * h->bs_max;
     launch_l0_snp_finalize(a, s);
     h->launches += 1;
   };
-  if (!h->stats_tc) {
+  if (!s1.stats_tc) {
     ScopedTimer t(h, "l0_stats", s);
-    launch_l0_stats(L.gp.p, Npad, h->xy.p, h->cpp, h->chunks.p, h->nchunks, rows_p, L.cnt_part.p,
+    launch_l0_stats(L.gp.p, Npad, s1.xy.p, s1.cpp, s1.chunks.p, s1.nchunks, rows_p, L.cnt_part.p,
                     L.sum_part.p, s);
-    launch_l0_fold_reduce(L.cnt_part.p, L.sum_part.p, rows_p, h->cpp, h->fold_chunks.p, K,
+    launch_l0_fold_reduce(L.cnt_part.p, L.sum_part.p, rows_p, s1.cpp, s1.fold_chunks.p, K,
                           L.cnt_fold.p, L.sum_fold.p, s);
     snp_finalize();
     h->launches += 2;
@@ -641,56 +628,56 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
 
   // --- 3. exact integer Grams on the tensor cores
   {
-    const rg_ctx::TileList& tl =
-        cached_tiles(h->tile_lists, rows_p, [&](std::vector<int2>& tiles) { gram_tile_list(2 * rows_p, tiles); });
+    const TileList& tl =
+        cached_tiles(s1.tile_lists, rows_p, [&](std::vector<int2>& tiles) { gram_tile_list(2 * rows_p, tiles); });
     const int64_t zz_stride = (int64_t)4 * rows_p * rows_p;
     ScopedTimer t(h, "gram_wgmma", s);
-    if (h->gram_dense) {
-      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p, K,
+    if (s1.gram_dense) {
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, s1.fold_k.p, K,
                      L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s);
       h->launches += 1;
     } else {
       // the Miss rows: the device picks the sparse sums or the dense tiles from the block's missing-call count
-      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p, K,
-                     L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, h->miss_cap, rows_p / 128);
-      launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, h->miss_nct, h->miss_fold_ct.p, L.miss_list.p, K,
-                         L.miss_total.p, h->miss_cap, L.zz.p, zz_stride, s);
+      launch_gram_gp(gp_map(h, L, rows_p), nullptr, rows_p, kZLevel0, tl.buf.p, tl.count, s1.fold_k.p, K,
+                     L.zz.p, 2 * rows_p, zz_stride, kZScaleGram, s, 256, L.miss_total.p, s1.miss_cap, rows_p / 128);
+      launch_miss_sparse(L.gt.p, rows_p, L.miss_seg.p, s1.miss_nct, s1.miss_fold_ct.p, L.miss_list.p, K,
+                         L.miss_total.p, s1.miss_cap, L.zz.p, zz_stride, s);
       h->launches += 2;
     }
-    L.last_gram_dense = h->gram_dense;
+    L.last_gram_dense = s1.gram_dense;
   }
-  if (h->stats_tc) {
+  if (s1.stats_tc) {
     // Z [X | Y]-digits: one more column tile per row tile of the same kernel, then the FP64 Horner
     ScopedTimer t(h, "l0_stats", s);
-    const int stat_bn = (h->stat_drows % 256 == 0) ? 256 : 128;
-    const rg_ctx::TileList& tl = cached_tiles(h->stat_tile_lists, rows_p, [&](std::vector<int2>& tiles) {
-      stat_tile_list(2 * rows_p, h->stat_drows, stat_bn, tiles);
+    const int stat_bn = (s1.stat_drows % 256 == 0) ? 256 : 128;
+    const TileList& tl = cached_tiles(s1.stat_tile_lists, rows_p, [&](std::vector<int2>& tiles) {
+      stat_tile_list(2 * rows_p, s1.stat_drows, stat_bn, tiles);
     });
-    L.tstat.alloc((size_t)K * 2 * h->rows_p_max * h->stat_drows);
-    const int64_t tfs = (int64_t)2 * rows_p * h->stat_drows;
-    launch_gram_gp(gp_map(h, L, rows_p), &h->tmD, rows_p, kZLevel0, tl.buf.p, tl.count, h->fold_k.p,
-                   K, L.tstat.p, h->stat_drows, tfs, kZScaleStat, s, stat_bn);
-    launch_l0_stats_finish(L.tstat.p, h->stat_drows, tfs, L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, rows_p,
-                           h->cpp, C + P, K, h->xy_scale.p, L.cnt_fold.p, L.sum_fold.p, s);
+    L.tstat.alloc((size_t)K * 2 * h->rows_p_max * s1.stat_drows);
+    const int64_t tfs = (int64_t)2 * rows_p * s1.stat_drows;
+    launch_gram_gp(gp_map(h, L, rows_p), &s1.tmD, rows_p, kZLevel0, tl.buf.p, tl.count, s1.fold_k.p,
+                   K, L.tstat.p, s1.stat_drows, tfs, kZScaleStat, s, stat_bn);
+    launch_l0_stats_finish(L.tstat.p, s1.stat_drows, tfs, L.zz.p, 2 * rows_p, (int64_t)4 * rows_p * rows_p, rows_p,
+                           s1.cpp, C + P, K, s1.xy_scale.p, L.cnt_fold.p, L.sum_fold.p, s);
     snp_finalize();
     h->launches += 2;
   }
 
   // --- 4./5. ridge systems -> coefficients -> out-of-fold predictions, standardised into W
-  const int mx_n = (!h->loocv && h->solver_mixed) ? MixedSolver::dim_for(bs) : 0;
+  const int mx_n = (!s1.loocv && s1.solver_mixed) ? MixedSolver::dim_for(bs) : 0;
   L.last_mx_n = mx_n;
   if (mx_n > 0) {
-    enqueue_solve_mixed(h, L, d, mx_n, s);
-    enqueue_predict(h, L, d, L.mx_x.p, (int64_t)mx_pp(P) * mx_n, mx_n, 0, s);
+    enqueue_solve_mixed(h, s1, L, d, mx_n, s);
+    enqueue_predict(h, s1, L, d, L.mx_x.p, (int64_t)mx_pp(P) * mx_n, mx_n, 0, s);
     // the flag travels to pinned host memory behind the block; it is read when this lane is next used or at a sync
-    RG_CUDA(cudaMemcpyAsync(L.mx_fail_host, L.mx_fail.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(L.mx_fail_host.p, L.mx_fail.p, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaEventRecord(L.mx_ev, s));
     L.mx_pending = true; L.mx_bs = bs; L.mx_block_id = block_id;
-    h->mx_blocks += 1;
+    s1.mx_blocks += 1;
     return;
   }
-  enqueue_solve_f64(h, L, d, s);
-  if (!h->loocv) enqueue_predict(h, L, d, L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.nC, s);
+  enqueue_solve_f64(h, s1, L, d, s);
+  if (!s1.loocv) enqueue_predict(h, s1, L, d, L.cm.p, (int64_t)d.n_aug * d.nC, d.nC, d.nC, s);
 }
 
 
@@ -699,11 +686,12 @@ static void l0_block_bed(rg_ctx* h, const uint8_t* packed, int64_t row_stride, i
 // tensor pipe, batched Cholesky, out-of-fold (or closed-form leave-one-out) predictions, standardisation into W.
 static void l0_block_dense(rg_ctx* h, const uint8_t* probs, const uint8_t* miss, const double* G64, int64_t n_file, int bs,
                            const int32_t* sample_idx, int ref_first, int block_id) {
+  Step1State& s1 = step1(h);
   RG_CHECK(n_file > 0, "bad sample count of the genotype file");
   BlockDims d;
-  rg_ctx::Lane& L = l0_begin_block(h, bs, block_id, sample_idx, d);
-  resolve_lane(h, L);
-  const int C = h->C, P = h->P, K = h->K, R = h->R;
+  Step1State::Lane& L = l0_begin_block(h, s1, bs, block_id, sample_idx, d);
+  resolve_lane(h, s1, L);
+  const int C = h->C, P = h->P, K = s1.K, R = s1.R;
   const int64_t Npad = h->Npad;
   cudaStream_t s = L.stream;
   L.last_pred_i8 = 0; L.last_mx_n = 0;     // dense FP64 prediction and Cholesky
@@ -733,34 +721,34 @@ static void l0_block_dense(rg_ctx* h, const uint8_t* probs, const uint8_t* miss,
     }
     launch_dense_from_dosage(pd, md, n_file, bs, h->file_idx_pad.p, ref_first, L.gd.p, Npad, s);
   }
-  launch_dense_prepare(L.gd.p, Npad, bs, h->file_idx_pad.p, h->xy.p, h->cpp, C, h->n_analyzed, 1e-6, L.mu.p, L.inv_sd.p,
-                       h->err_slot.p, (long long)block_id * h->bs_max, s);
+  launch_dense_prepare(L.gd.p, Npad, bs, h->file_idx_pad.p, s1.xy.p, s1.cpp, C, h->n_analyzed, 1e-6, L.mu.p, L.inv_sd.p,
+                       s1.err_slot.p, (long long)block_id * h->bs_max, s);
   // --- per-chunk G G^T (DMMA) and G Y, summed per fold in a fixed order by the assembler
-  const int nC = d.nC, nch = h->nchunks;
+  const int nC = d.nC, nch = s1.nchunks;
   const int64_t part_stride = (int64_t)nC * nC;
   L.dpart.alloc((size_t)nch * round_up(h->bs_max, 64) * round_up(h->bs_max, 64));
   L.dpart_y.alloc((size_t)P * nch * h->bs_max);
-  launch_l1_gram(L.gd.p, Npad, bs, h->chunks.p, nch, L.dpart.p, part_stride, nC, s);
+  launch_l1_gram(L.gd.p, Npad, bs, s1.chunks.p, nch, L.dpart.p, part_stride, nC, s);
   for (int p = 0; p < P; ++p)
-    launch_l1_xty(L.gd.p, Npad, h->xy.p, h->cpp, C + p, h->chunks.p, nch, L.dpart_y.p + (size_t)p * nch * bs, bs, s);
-  ensure_f64_systems(h, L, d, s);
+    launch_l1_xty(L.gd.p, Npad, s1.xy.p, s1.cpp, C + p, s1.chunks.p, nch, L.dpart_y.p + (size_t)p * nch * bs, bs, s);
+  ensure_f64_systems(h, s1, L, d, s);
   const int64_t cm_stride = (int64_t)d.n_aug * nC;
-  launch_dense_assemble(L.dpart.p, part_stride, nC, L.dpart_y.p, (int64_t)nch * bs, h->fold_chunks.p, K, R, h->lambda.p, bs, nC,
-                        P, L.cm.p, cm_stride, h->loocv, s);
-  if (h->loocv) launch_dense_loocv_fill(L.gd.p, Npad, bs, nC, L.cm.p, cm_stride, nC + d.Ppad, R, s);
-  launch_chol_factor(L.cm.p, cm_stride, nC, d.n_aug, d.nmat, L.inv.p, h->err_slot.p,
+  launch_dense_assemble(L.dpart.p, part_stride, nC, L.dpart_y.p, (int64_t)nch * bs, s1.fold_chunks.p, K, R, s1.lambda.p, bs, nC,
+                        P, L.cm.p, cm_stride, s1.loocv, s);
+  if (s1.loocv) launch_dense_loocv_fill(L.gd.p, Npad, bs, nC, L.cm.p, cm_stride, nC + d.Ppad, R, s);
+  launch_chol_factor(L.cm.p, cm_stride, nC, d.n_aug, d.nmat, L.inv.p, s1.err_slot.p,
                      (long long)(1ll << 40) + (long long)block_id * 1024, s);
   h->launches += 5 + P + chol_num_launches(nC);
   L.part.alloc((size_t)d.ntiles_s * d.Qp * 2);
   L.mean_invsd.alloc((size_t)2 * d.Qp);
-  if (h->loocv) {
-    enqueue_loocv_predict(h, L, d, s);
+  if (s1.loocv) {
+    enqueue_loocv_predict(h, s1, L, d, s);
     return;
   }
   launch_chol_backsolve(L.cm.p, cm_stride, nC, P, d.nmat, L.inv.p, s);
-  launch_dense_predict(L.gd.p, Npad, bs, L.cm.p, cm_stride, nC, nC, R, P, h->tile_fold.p, h->mask.p, h->W_tab.p, d.col0, s);
-  const int nparts = launch_l0_colsum(h->W_tab.p, Npad, d.col0, P, d.Q, d.Qp, L.part.p, s);
-  launch_l0_standardize(L.part.p, nparts, d.Qp, d.Q, P, h->neff.p, L.mean_invsd.p, h->W_tab.p, Npad, d.col0, h->is_real.p, s);
+  launch_dense_predict(L.gd.p, Npad, bs, L.cm.p, cm_stride, nC, nC, R, P, s1.tile_fold.p, s1.mask.p, s1.W_tab.p, d.col0, s);
+  const int nparts = launch_l0_colsum(s1.W_tab.p, Npad, d.col0, P, d.Q, d.Qp, L.part.p, s);
+  launch_l0_standardize(L.part.p, nparts, d.Qp, d.Q, P, s1.neff.p, L.mean_invsd.p, s1.W_tab.p, Npad, d.col0, s1.is_real.p, s);
   h->launches += 6;
 }
 
@@ -787,123 +775,123 @@ static DebugView host_view(const T* p, size_t count) {
 }
 
 // how Step 2 computed its last block, and the sums it came from
-static DebugView s2_debug_view(const rg_ctx* h, const std::string& n) {
+static DebugView s2_debug_view(const rg_ctx* h, const Step2State& s2, const std::string& n) {
   if (n == "s2_paths") {
-    const int64_t v[8] = {h->s2_tc ? 1 : 0, h->s2_nchunk, h->s2_chunk_len, h->s2_drows, h->nchunks, h->Npad, h->dp, h->bt_dp};
+    const int64_t v[8] = {s2.tc ? 1 : 0, s2.nchunk, s2.chunk_len, s2.drows, s2.nchunks, h->Npad, s2.dp, s2.bt_dp};
     return host_view(v, 8);
   }
-  if (n == "s2_sums") return dev_view(h->s2_sums.p, (size_t)h->s2_sums_rows * 3 * h->dp * 8);                 // [rows_p][3][dp]
-  if (n == "bt_sums") return dev_view(h->bt_sums.p, (size_t)h->bt_sums_rows * 4 * h->bt_sums_dp * 8);   // [rows_p][4][dp]
-  if (n == "bt_nnz") return dev_view(h->bt_nnz.p, (size_t)h->bt_sums_rows * 8);
-  if (n == "bt_n510") return dev_view(h->bt_n510.p, (size_t)h->bt_sums_rows * 8);
+  if (n == "s2_sums") return dev_view(s2.sums.p, (size_t)s2.sums_rows * 3 * s2.dp * 8);                 // [rows_p][3][dp]
+  if (n == "bt_sums") return dev_view(s2.dose_sums.p, (size_t)s2.dose_sums_rows * 4 * s2.dose_sums_dp * 8);   // [rows_p][4][dp]
+  if (n == "bt_nnz") return dev_view(s2.dose_nnz.p, (size_t)s2.dose_sums_rows * 8);
+  if (n == "bt_n510") return dev_view(s2.dose_n510.p, (size_t)s2.dose_sums_rows * 8);
   // the tensor sums, when the last block was a 2-bit one: its rows [rows_p][Npad/16], the digit sums
   // [s2_nchunk][3 rows_p][drows] of the planes [G; G^2; Miss], and the digit rows of F [drows][Npad] they were taken against
-  const size_t rp = (size_t)round_up(h->s2_last_bs, kRowPad);
-  if (n == "s2_gp") return dev_view(h->gp.p, rp * (h->Npad / 16) * 4);
-  if (n == "s2_T" && h->s2_tc) return dev_view(h->s2_T.p, (size_t)h->s2_nchunk * 3 * rp * h->s2_drows * 4);
-  if (n == "s2_FD" && h->s2_tc) return dev_view(h->s2_FD.p, (size_t)h->s2_drows * h->Npad);
+  const size_t rp = (size_t)round_up(s2.last_bs, kRowPad);
+  if (n == "s2_gp") return dev_view(s2.gp.p, rp * (h->Npad / 16) * 4);
+  if (n == "s2_T" && s2.tc) return dev_view(s2.T.p, (size_t)s2.nchunk * 3 * rp * s2.drows * 4);
+  if (n == "s2_FD" && s2.tc) return dev_view(s2.FD.p, (size_t)s2.drows * h->Npad);
   // GxE interaction state of the chromosome: its feature rows [Npad][nf] once rg_s2_set_interaction has run; the shape,
   // the routes [bs] and the chunk-reduced sums [bs][nf] (defined where the variant's route reads them) of the last
   // rg_s2_interaction call since then
   if (n.compare(0, 4, "int_") == 0) {
-    RG_CHECK(h->int_set, "no interaction state on this handle: " + n);
-    if (n == "int_F") return dev_view(h->int_F.p, (size_t)h->Npad * h->int_nf * 8);
-    RG_CHECK(h->int_last_bs > 0, "no rg_s2_interaction call since rg_s2_set_interaction: " + n);
-    const int bs = h->int_last_bs;
+    RG_CHECK(s2.int_set, "no interaction state on this handle: " + n);
+    if (n == "int_F") return dev_view(s2.int_F.p, (size_t)h->Npad * s2.int_nf * 8);
+    RG_CHECK(s2.int_last_bs > 0, "no rg_s2_interaction call since rg_s2_set_interaction: " + n);
+    const int bs = s2.int_last_bs;
     if (n == "int_paths") {
-      const int64_t v[8] = {h->nchunks, h->Npad, h->int_nf, h->int_nr, h->int_K, ceil_div(h->P, kIntTG),
+      const int64_t v[8] = {s2.nchunks, h->Npad, s2.int_nf, s2.int_nr, s2.int_K, ceil_div(h->P, kIntTG),
                             ceil_div(h->Npad, kIntSlab), bs};
       return host_view(v, 8);
     }
-    if (n == "int_route") return dev_view(h->int_route.p, (size_t)bs);
-    if (n == "int_sums") return dev_view(h->int_sums.p, (size_t)bs * h->int_nf * 8);
+    if (n == "int_route") return dev_view(s2.int_route.p, (size_t)bs);
+    if (n == "int_sums") return dev_view(s2.int_sums.p, (size_t)bs * s2.int_nf * 8);
   }
   throw Error{"unknown Step-2 debug buffer: " + n};
 }
 
 // shape and state of the last level-1 fit
-static DebugView l1_debug_view(const rg_ctx* h, const std::string& n) {
-  RG_CHECK(h->l1_done, "no level-1 fit on this handle: " + n);
-  const int64_t nC = h->l1_nC, P = h->P;
+static DebugView l1_debug_view(const rg_ctx* h, const Step1State& s1, const std::string& n) {
+  RG_CHECK(s1.l1_done, "no level-1 fit on this handle: " + n);
+  const int64_t nC = s1.l1_nC, P = h->P;
   if (n == "l1_dims") {
-    const int64_t v[8] = {h->B, nC, h->R1, h->K, h->l1_nmat, h->l1_n_aug, h->l1_nchunks, h->l1_chunk_len};
+    const int64_t v[8] = {s1.B, nC, s1.R1, s1.K, s1.l1_nmat, s1.l1_n_aug, s1.l1_nchunks, s1.l1_chunk_len};
     return host_view(v, 8);
   }
-  if (n == "l1_chunks") return dev_view(h->l1_chunks.p, (size_t)h->l1_nchunks * sizeof(int4));          // (t0, len, fold, 0)
-  if (n == "l1_beta" && !h->loocv) return dev_view(h->l1_beta.p, (size_t)P * h->K * h->R1 * nC * 8);    // [P][K R1][nC]
-  if (n == "l1_sums" && !h->l1_bt) return dev_view(h->l1_sums.p, (size_t)P * (kMaxRidge * 3 + 2) * 8);
-  if (n == "l1_bvec" && h->loocv) return dev_view(h->l1_bvec.p, (size_t)P * nC * 8);
-  if (n == "l1_hvec" && h->loocv) return dev_view(h->l1_hvec.p, (size_t)P * h->Npad * 8);
+  if (n == "l1_chunks") return dev_view(s1.l1_chunks.p, (size_t)s1.l1_nchunks * sizeof(int4));          // (t0, len, fold, 0)
+  if (n == "l1_beta" && !s1.loocv) return dev_view(s1.l1_beta.p, (size_t)P * s1.K * s1.R1 * nC * 8);    // [P][K R1][nC]
+  if (n == "l1_sums" && !s1.l1_bt) return dev_view(s1.l1_sums.p, (size_t)P * (kMaxRidge * 3 + 2) * 8);
+  if (n == "l1_bvec" && s1.loocv) return dev_view(s1.l1_bvec.p, (size_t)P * nC * 8);
+  if (n == "l1_hvec" && s1.loocv) return dev_view(s1.l1_hvec.p, (size_t)P * h->Npad * 8);
   throw Error{"no level-1 debug buffer " + n + " for this fit"};
 }
 
 // intermediates of the last level-0 block
-static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
-  RG_CHECK(!h->lanes.empty(), "no level-0 lane: " + n);
-  rg_ctx::Lane& L = *h->lanes[h->last_lane];
-  const int rp = h->last_rows_p;
+static DebugView l0_debug_view(rg_ctx* h, Step1State& s1, const std::string& n) {
+  RG_CHECK(!s1.lanes.empty(), "no level-0 lane: " + n);
+  Step1State::Lane& L = *s1.lanes[s1.last_lane];
+  const int rp = s1.last_rows_p;
   if (n == "gp") return dev_view(L.gp.p, (size_t)rp * (h->Npad / 16) * 4);
-  if (n == "zz") return dev_view(L.zz.p, (size_t)h->K * 4 * rp * rp * 4);
-  if (n == "tstat" && h->stats_tc) return dev_view(L.tstat.p, (size_t)h->K * 2 * rp * h->stat_drows * 4);  // [K][2 rp][drows]
-  if (n == "xyD" && h->stats_tc) return dev_view(h->xyD.p, (size_t)h->stat_drows * h->Npad);                // [drows][Npad]
+  if (n == "zz") return dev_view(L.zz.p, (size_t)s1.K * 4 * rp * rp * 4);
+  if (n == "tstat" && s1.stats_tc) return dev_view(L.tstat.p, (size_t)s1.K * 2 * rp * s1.stat_drows * 4);  // [K][2 rp][drows]
+  if (n == "xyD" && s1.stats_tc) return dev_view(s1.xyD.p, (size_t)s1.stat_drows * h->Npad);                // [drows][Npad]
   if (n == "mu") return dev_view(L.mu.p, (size_t)rp * 8);
   if (n == "inv_sd") return dev_view(L.inv_sd.p, (size_t)rp * 8);
   if (n == "Bv") return dev_view(L.Bv.p, (size_t)rp * h->C * 8);
-  if (n == "gty_f") return dev_view(L.gty_f.p, (size_t)h->K * rp * h->P * 8);
-  if (n == "rhs") return dev_view(L.rhs.p, (size_t)h->K * rp * h->P * 8);
-  if (n == "cm") return dev_view(L.cm.p, (size_t)h->last_nmat * h->last_n_aug * h->last_nC * 8);
-  if (n == "mean_invsd") return dev_view(L.mean_invsd.p, (size_t)2 * h->R * h->P * 8);
-  if (n == "wraw") return dev_view(L.wraw.p, (size_t)h->P * h->R * h->Npad * 8);
+  if (n == "gty_f") return dev_view(L.gty_f.p, (size_t)s1.K * rp * h->P * 8);
+  if (n == "rhs") return dev_view(L.rhs.p, (size_t)s1.K * rp * h->P * 8);
+  if (n == "cm") return dev_view(L.cm.p, (size_t)s1.last_nmat * s1.last_n_aug * s1.last_nC * 8);
+  if (n == "mean_invsd") return dev_view(L.mean_invsd.p, (size_t)2 * s1.R * h->P * 8);
+  if (n == "wraw") return dev_view(L.wraw.p, (size_t)h->P * s1.R * h->Npad * 8);
   if (n == "gam" || n == "gmu" || n == "cvec") {
-    const size_t Kg = h->loocv ? 1 : h->K, Qp = (size_t)round_up(h->R * h->P, predict_qt());
+    const size_t Kg = s1.loocv ? 1 : s1.K, Qp = (size_t)round_up(s1.R * h->P, predict_qt());
     const DevBuf<double>& b = n == "gam" ? L.gam : n == "gmu" ? L.gmu : L.cvec;
     return dev_view(b.p, (n == "cvec" ? Kg * Qp * h->C : Kg * rp * Qp) * 8);
   }
-  if (n == "cnt_fold") return dev_view(L.cnt_fold.p, (size_t)h->K * rp * 4 * 4);
-  if (n == "sum_fold") return dev_view(L.sum_fold.p, (size_t)h->K * rp * 2 * h->cpp * 8);
+  if (n == "cnt_fold") return dev_view(L.cnt_fold.p, (size_t)s1.K * rp * 4 * 4);
+  if (n == "sum_fold") return dev_view(L.sum_fold.p, (size_t)s1.K * rp * 2 * s1.cpp * 8);
   if (n == "paths") {
     // which kernels produced the last block: statistics on the tensor cores, INT8 prediction, mixed-solver dimension
-    const int64_t v[3] = {h->stats_tc ? 1 : 0, L.last_pred_i8, L.last_mx_n};
+    const int64_t v[3] = {s1.stats_tc ? 1 : 0, L.last_pred_i8, L.last_mx_n};
     return host_view(v, 3);
   }
   if (n == "dims") {
-    const int64_t v[8] = {h->Npad, rp, h->last_nC, h->last_n_aug, h->last_nmat, h->K, h->cpp, h->nchunks};
+    const int64_t v[8] = {h->Npad, rp, s1.last_nC, s1.last_n_aug, s1.last_nmat, s1.K, s1.cpp, s1.nchunks};
     return host_view(v, 8);
   }
   if (n == "gram_path") {
     // how the Miss rows of the last block's Gram were computed: 1 = sparse sums, 0 = dense tiles; the block's
     // missing calls (-1 when RG_B200_GRAM=dense skipped the count) and the sparse path's capacity
-    int64_t v[3] = {0, -1, h->miss_cap};
+    int64_t v[3] = {0, -1, s1.miss_cap};
     if (!L.last_gram_dense) {
       RG_CHECK(L.miss_total.p, "debug buffer not filled yet: gram_path");
       unsigned long long tot = 0;
       RG_CUDA(cudaStreamSynchronize(L.stream));
       RG_CUDA(cudaMemcpy(&tot, L.miss_total.p, sizeof(tot), cudaMemcpyDeviceToHost));
-      v[0] = (int64_t)tot <= h->miss_cap ? 1 : 0;
+      v[0] = (int64_t)tot <= s1.miss_cap ? 1 : 0;
       v[1] = (int64_t)tot;
     }
     return host_view(v, 3);
   }
-  if (n == "miss_ctile") return host_view(h->miss_ctile_host.data(), h->miss_ctile_host.size());  // (word, words, fold, 0)
+  if (n == "miss_ctile") return host_view(s1.miss_ctile_host.data(), s1.miss_ctile_host.size());  // (word, words, fold, 0)
   if (n == "miss_seg" || n == "miss_list") {
     // the relayout's missing lists of the last block (sparse path only): seg [rows_p][miss_nct] (offset, count) into
     // list; a view holds them once the block's total is within the capacity
     RG_CHECK(!L.last_gram_dense && L.miss_seg.p, "no missing lists for the last block: " + n);
-    if (n == "miss_seg") return dev_view(L.miss_seg.p, (size_t)rp * h->miss_nct * sizeof(int2));
-    return dev_view(L.miss_list.p, (size_t)std::max<int64_t>(h->miss_cap, 1) * 4);
+    if (n == "miss_seg") return dev_view(L.miss_seg.p, (size_t)rp * s1.miss_nct * sizeof(int2));
+    return dev_view(L.miss_list.p, (size_t)std::max<int64_t>(s1.miss_cap, 1) * 4);
   }
-  if (n == "pad_of") return host_view(h->pad_of.data(), h->N);
+  if (n == "pad_of") return host_view(s1.pad_of.data(), h->N);
   if (n == "zz_ref") {
     // the integer Grams recomputed on the CUDA cores from the 2-bit rows
     RG_CHECK(L.gp.p, "debug buffer not filled yet: gp");
     const size_t per = (size_t)4 * rp * rp;
     DevBuf<float> ref;
-    ref.alloc(per * h->K);
-    RG_CUDA(cudaMemsetAsync(ref.p, 0, per * h->K * 4, h->stream));
-    for (int f = 0; f < h->K; ++f)
-      launch_gram_reference(L.gp.p, h->Npad, rp, (int)h->fold_pad_start[f], (int)(h->fold_pad_start[f] + h->fold_pad_len[f]),
+    ref.alloc(per * s1.K);
+    RG_CUDA(cudaMemsetAsync(ref.p, 0, per * s1.K * 4, h->stream));
+    for (int f = 0; f < s1.K; ++f)
+      launch_gram_reference(L.gp.p, h->Npad, rp, (int)s1.fold_pad_start[f], (int)(s1.fold_pad_start[f] + s1.fold_pad_len[f]),
                             ref.p + per * f, 2 * rp, h->stream);
-    std::vector<float> v(per * h->K);
+    std::vector<float> v(per * s1.K);
     RG_CUDA(cudaMemcpyAsync(v.data(), ref.p, v.size() * 4, cudaMemcpyDeviceToHost, h->stream));
     RG_CUDA(cudaStreamSynchronize(h->stream));
     return host_view(v.data(), v.size());
@@ -914,13 +902,21 @@ static DebugView l0_debug_view(rg_ctx* h, const std::string& n) {
 static DebugView debug_view(rg_ctx* h, const std::string& n, int64_t max_bytes) {
   if (n == "pgen_rows") {
     // the rows the last rg_pgen_decode produced (Step 1: the next lane's input), cut to the caller's buffer
-    const DevBuf<uint8_t>& r = h->kind == 1 && !h->lanes.empty() ? h->lanes[h->next_lane]->packed_dev : h->pgen_rows;
+    const DevBuf<uint8_t>& r = h->s1 ? h->s1->lanes[h->s1->next_lane]->packed_dev : h->s2->pgen_rows;
     RG_CHECK(r.p, "pgen_rows: no rg_pgen_decode has filled it");
     return dev_view(r.p, std::min<size_t>(r.n, (size_t)std::max<int64_t>(max_bytes, 0)));
   }
-  if (h->kind == 2) return s2_debug_view(h, n);
-  if (n.compare(0, 3, "l1_") == 0) return l1_debug_view(h, n);
-  return l0_debug_view(h, n);
+  if (h->s2) return s2_debug_view(h, *h->s2, n);
+  if (n.compare(0, 3, "l1_") == 0) return l1_debug_view(h, *h->s1, n);
+  return l0_debug_view(h, *h->s1, n);
+}
+
+// rg_l0_status of an error-slot word; the failure it names goes to rg_last_error
+static int64_t l0_status_of(unsigned long long v) {
+  if (v == ~0ull) return 0;
+  if (v >= (1ull << 40)) set_last_error("Cholesky pivot not positive (system id " + std::to_string(v - (1ull << 40)) + ")");
+  else set_last_error("SNP has low variance (index " + std::to_string(v - 1) + ")");
+  return (int64_t)v;
 }
 
 static int64_t copy_debug_view(const DebugView& v, const std::string& n, void* out, int64_t max_bytes) {
@@ -969,9 +965,10 @@ int rg_step1_create(const rg_step1_config* cfg, const double* X, const double* Y
   RG_CHECK(cfg->n_ridge_l0 >= 1 && cfg->max_block_size >= 1 && cfg->total_blocks >= 1, "bad sizes");
   RG_CUDA(cudaSetDevice(cfg->device));
   std::unique_ptr<rg_ctx> h(new rg_ctx());
-  h->kind = 1;
+  h->s1 = std::make_unique<Step1State>();
+  Step1State& s1 = *h->s1;
   h->device = cfg->device;
-  RG_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+  h->stream.ensure();
   {
     // The CUDA driver multiplexes streams onto CUDA_DEVICE_MAX_CONNECTIONS hardware queues (default 8, read when the context
     // is created); streams that share a queue serialise behind each other, which is why more than 8 lanes do not pay at the
@@ -982,37 +979,34 @@ int rg_step1_create(const rg_step1_config* cfg, const double* X, const double* Y
     if (const char* q = getenv("CUDA_DEVICE_MAX_CONNECTIONS")) if (atoi(q) >= 16) nl = 12;
     if (const char* e = getenv("RG_B200_LANES")) nl = std::max(1, std::min(32, atoi(e)));
     for (int i = 0; i < nl; ++i) {
-      auto l = std::make_unique<rg_ctx::Lane>();
-      RG_CUDA(cudaStreamCreateWithFlags(&l->stream, cudaStreamNonBlocking));
-      RG_CUDA(cudaEventCreateWithFlags(&l->done, cudaEventDisableTiming));
-      h->lanes.push_back(std::move(l));
+      s1.lanes.push_back(std::make_unique<Step1State::Lane>());
+      s1.lanes.back()->stream.ensure();
     }
   }
   h->N = cfg->n_samples; h->C = cfg->n_cov; h->P = cfg->n_pheno;
-  h->loocv = cfg->loocv ? 1 : 0;
-  h->K = h->loocv ? 1 : cfg->n_folds;
-  h->R = cfg->n_ridge_l0; h->R1 = cfg->n_ridge_l1;
+  s1.loocv = cfg->loocv ? 1 : 0;
+  s1.K = s1.loocv ? 1 : cfg->n_folds;
+  s1.R = cfg->n_ridge_l0; s1.R1 = cfg->n_ridge_l1;
   h->bs_max = cfg->max_block_size;
   h->rows_p_max = (int)round_up(h->bs_max, kRowPad);
-  h->total_blocks = cfg->total_blocks;
-  h->B = (int64_t)h->total_blocks * h->R;
+  s1.total_blocks = cfg->total_blocks;
+  s1.B = (int64_t)s1.total_blocks * s1.R;
   h->n_analyzed = cfg->n_analyzed;
-  if (const char* e = getenv("RG_B200_SOLVER")) h->solver_mixed = std::string(e) == "f64" ? 0 : 1;
-  if (const char* e = getenv("RG_B200_MX_TOL")) h->mx_tol = (float)atof(e);
-  build_layout(h.get(), X, Y, mask, in_analysis, fold_sizes);
-  h->lambda.alloc(h->R);
-  h->neff.alloc(h->P);
-  RG_CUDA(cudaMemcpy(h->lambda.p, lambda, h->R * 8, cudaMemcpyHostToDevice));
-  RG_CUDA(cudaMemcpy(h->neff.p, neff, h->P * 8, cudaMemcpyHostToDevice));
-  h->err_slot.alloc(1);
-  RG_CUDA(cudaMemset(h->err_slot.p, 0xFF, 8));
-  h->W_owned.assign(h->P, 1);                 // storage itself is allocated on first use (rg::ensure_W)
+  if (const char* e = getenv("RG_B200_SOLVER")) s1.solver_mixed = std::string(e) == "f64" ? 0 : 1;
+  if (const char* e = getenv("RG_B200_MX_TOL")) s1.mx_tol = (float)atof(e);
+  build_layout(h.get(), s1, X, Y, mask, in_analysis, fold_sizes);
+  s1.lambda.alloc(s1.R);
+  s1.neff.alloc(h->P);
+  RG_CUDA(cudaMemcpy(s1.lambda.p, lambda, s1.R * 8, cudaMemcpyHostToDevice));
+  RG_CUDA(cudaMemcpy(s1.neff.p, neff, h->P * 8, cudaMemcpyHostToDevice));
+  s1.err_slot.alloc(1);
+  RG_CUDA(cudaMemset(s1.err_slot.p, 0xFF, 8));
+  s1.W_owned.assign(h->P, 1);                 // storage itself is allocated on first use (rg::ensure_W)
   // every level-0 kernel addresses W through this table; rg_W_attach_peer redirects a phenotype to the HBM of
   // the GPU that owns its level-1 fit (stores travel over NVLink as the tiles are produced)
-  h->W_host_tab.resize(h->P);
-  h->W_host_tab.assign(h->P, nullptr);
-  h->W_tab.alloc(h->P);
-  h->l1_select.assign(h->P, 1);
+  s1.W_host_tab.assign(h->P, nullptr);
+  s1.W_tab.alloc(h->P);
+  s1.l1_select.assign(h->P, 1);
   *out = h.release();
   RG_API_END
 }
@@ -1020,81 +1014,64 @@ int rg_step1_create(const rg_step1_config* cfg, const double* X, const double* Y
 void rg_destroy(rg_handle h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  for (void* m : h->W_peer_mapped) cudaIpcCloseMemHandle(m);
-  if (h->poll_stream) { cudaStreamSynchronize(h->poll_stream); cudaStreamDestroy(h->poll_stream); }
-  if (h->poll_host) cudaFreeHost(h->poll_host);
-  for (auto& l : h->lanes) cudaStreamSynchronize(l->stream);
-  cudaStreamSynchronize(h->stream);
-  rg::flush_timers(h);
-  for (auto& l : h->lanes) {
-    if (l->mx_ev) cudaEventDestroy(l->mx_ev);
-    if (l->h2d_done) cudaEventDestroy(l->h2d_done);
-    for (int k = 0; k < 2; ++k) if (l->relayout_done[k]) cudaEventDestroy(l->relayout_done[k]);
-    if (l->copy_stream) { cudaStreamSynchronize(l->copy_stream); cudaStreamDestroy(l->copy_stream); }
-    if (l->mx_fail_host) cudaFreeHost(l->mx_fail_host);
-    cudaEventDestroy(l->done);
-    cudaStreamDestroy(l->stream);
+  std::vector<cudaStream_t> streams{h->stream};
+  if (h->s1) {
+    streams.push_back(h->s1->poll_stream);
+    for (auto& l : h->s1->lanes) streams.insert(streams.end(), {l->stream, l->copy_stream});
   }
-  cudaStreamDestroy(h->stream);
-  if (h->s2_hd) cudaFreeHost(h->s2_hd);
-  if (h->s2_hi) cudaFreeHost(h->s2_hi);
-  if (h->s2_copy_stream) { cudaStreamSynchronize(h->s2_copy_stream); cudaStreamDestroy(h->s2_copy_stream); }
-  for (int k = 0; k < rg_ctx::kStageSlots; ++k) if (h->s2_stage_ev[k]) cudaEventDestroy(h->s2_stage_ev[k]);
-  delete h;
+  if (h->s2) streams.push_back(h->s2->copy_stream);
+  for (cudaStream_t s : streams) if (s) cudaStreamSynchronize(s);
+  rg::flush_timers(h);
+  delete h;                                 // the members release their streams, events, pinned buffers and mappings
 }
 
 int rg_W_export(rg_handle h, void* ipc_handle_64) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1 && ipc_handle_64, "bad argument");
+  RG_CHECK(h && ipc_handle_64, "bad argument");
+  Step1State& s1 = step1(h);
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t is 64 bytes");
   RG_CUDA(cudaSetDevice(h->device));
-  ensure_W(h);
+  ensure_W(h, s1);
   cudaIpcMemHandle_t mh;
-  RG_CUDA(cudaIpcGetMemHandle(&mh, h->W.p));
+  RG_CUDA(cudaIpcGetMemHandle(&mh, s1.W.p));
   memcpy(ipc_handle_64, &mh, 64);
   RG_API_END
 }
 
 int rg_W_set_owned(rg_handle h, const uint8_t* owned) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1 && owned, "bad argument");
+  RG_CHECK(h && owned, "bad argument");
+  Step1State& s1 = step1(h);
   rg::sync_lanes(h);
-  RG_CHECK(!h->W.p, "rg_W_set_owned must be called before the first block / export");
-  h->W_owned.assign(owned, owned + h->P);
-  for (int p = 0; p < h->P; ++p) h->l1_select[p] = owned[p] ? 1 : 0;
-  ensure_W(h);
+  RG_CHECK(!s1.W.p, "rg_W_set_owned must be called before the first block / export");
+  s1.W_owned.assign(owned, owned + h->P);
+  for (int p = 0; p < h->P; ++p) s1.l1_select[p] = owned[p] ? 1 : 0;
+  ensure_W(h, s1);
   RG_API_END
 }
 
 int rg_W_attach_peer(rg_handle h, const void* ipc_handle_64, const uint8_t* owned_by_peer) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1 && ipc_handle_64 && owned_by_peer, "bad argument");
+  RG_CHECK(h && ipc_handle_64 && owned_by_peer, "bad argument");
+  Step1State& s1 = step1(h);
   rg::sync_lanes(h);
-  ensure_W(h);
+  ensure_W(h, s1);
   cudaIpcMemHandle_t mh;
   memcpy(&mh, ipc_handle_64, 64);
-  void* base = nullptr;
-  RG_CUDA(cudaIpcOpenMemHandle(&base, mh, cudaIpcMemLazyEnablePeerAccess));
-  h->W_peer_mapped.push_back(base);
-  // the peer's allocation is compact over ITS owned phenotypes (rg_W_set_owned with the same mask on that rank)
-  size_t slot = 0;
-  for (int p = 0; p < h->P; ++p)
-    if (owned_by_peer[p]) {
-      h->W_host_tab[p] = static_cast<double*>(base) + (slot++) * (size_t)h->Npad * h->B;
-      h->l1_select[p] = 0;
-    }
-  RG_CUDA(cudaMemcpy(h->W_tab.p, h->W_host_tab.data(), h->P * sizeof(double*), cudaMemcpyHostToDevice));
+  s1.W_peer_mapped.emplace_back(mh);
+  attach_W(h, s1, static_cast<double*>(s1.W_peer_mapped.back().p), owned_by_peer);
   RG_API_END
 }
 
 int rg_W_attach_local(rg_handle h, rg_handle peer, const uint8_t* owned_by_peer) {
   RG_API_BEGIN
-  RG_CHECK(h && peer && h != peer && h->kind == 1 && peer->kind == 1 && owned_by_peer, "bad argument");
-  RG_CHECK(h->P == peer->P && h->Npad == peer->Npad && h->B == peer->B, "handles describe different problems");
+  RG_CHECK(h && peer && h != peer && owned_by_peer, "bad argument");
+  Step1State &s1 = step1(h), &peer1 = step1(peer);
+  RG_CHECK(h->P == peer->P && h->Npad == peer->Npad && s1.B == peer1.B, "handles describe different problems");
   RG_CUDA(cudaSetDevice(peer->device));
-  ensure_W(peer);
+  ensure_W(peer, peer1);
   rg::sync_lanes(h);
-  ensure_W(h);
+  ensure_W(h, s1);
   if (h->device != peer->device) {
     int can = 0;
     RG_CUDA(cudaDeviceCanAccessPeer(&can, h->device, peer->device));
@@ -1103,21 +1080,16 @@ int rg_W_attach_local(rg_handle h, rg_handle peer, const uint8_t* owned_by_peer)
     if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
     else RG_CUDA(e);
   }
-  size_t slot = 0;
   for (int p = 0; p < h->P; ++p)
-    if (owned_by_peer[p]) {
-      RG_CHECK(peer->W_owned[p], "the peer does not own storage for a phenotype it is said to own");
-      h->W_host_tab[p] = peer->W.p + (slot++) * (size_t)h->Npad * h->B;
-      h->l1_select[p] = 0;
-    }
-  RG_CUDA(cudaMemcpy(h->W_tab.p, h->W_host_tab.data(), h->P * sizeof(double*), cudaMemcpyHostToDevice));
+    RG_CHECK(!owned_by_peer[p] || peer1.W_owned[p], "the peer does not own storage for a phenotype it is said to own");
+  attach_W(h, s1, peer1.W.p, owned_by_peer);
   RG_API_END
 }
 
 int rg_l1_select(rg_handle h, const uint8_t* sel) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1 && sel, "bad argument");
-  h->l1_select.assign(sel, sel + h->P);
+  RG_CHECK(h && sel, "bad argument");
+  step1(h).l1_select.assign(sel, sel + h->P);
   RG_API_END
 }
 
@@ -1136,9 +1108,10 @@ int rg_fence(rg_handle h) {
   RG_CHECK(h, "null handle");
   RG_CUDA(cudaSetDevice(h->device));
   // blocks whose mixed-precision solve raised its flag are re-solved in FP64 first (host waits on those lanes' events)
-  if (h->kind == 1) for (auto& l : h->lanes) rg::resolve_lane(h, *l);
-  for (auto& l : h->lanes) {
-    RG_CUDA(cudaEventRecord(l->done, l->stream));
+  if (!h->s1) return 0;
+  for (auto& l : h->s1->lanes) rg::resolve_lane(h, *h->s1, *l);
+  for (auto& l : h->s1->lanes) {
+    RG_CUDA(cudaEventRecord(l->done.ensure(), l->stream));
     RG_CUDA(cudaStreamWaitEvent(h->stream, l->done, 0));
   }
   RG_API_END
@@ -1172,24 +1145,26 @@ int rg_l0_block_f64(rg_handle h, const double* G, int64_t n_file, int32_t bs, co
 
 int rg_l0_wait_input(rg_handle h) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1, "not a Step-1 handle");
+  RG_CHECK(h, "not a Step-1 handle");     // a null handle is no Step-1 handle either
+  Step1State& s1 = step1(h);
   RG_CUDA(cudaSetDevice(h->device));
-  rg_ctx::Lane& L = *h->lanes[h->last_lane];
-  if (L.h2d_recorded) RG_CUDA(cudaEventSynchronize(L.h2d_done));
+  Step1State::Lane& L = *s1.lanes[s1.last_lane];
+  if (L.h2d_done) RG_CUDA(cudaEventSynchronize(L.h2d_done));
   RG_API_END
 }
 
 int rg_l0_load_W(rg_handle h, int32_t block_id, int32_t ph, const double* in) {
   RG_API_BEGIN
   RG_CHECK(h && in, "null argument");
-  RG_CHECK(h->kind == 1 && block_id >= 0 && block_id < h->total_blocks && ph >= 0 && ph < h->P, "bad index");
+  Step1State& s1 = step1(h);
+  RG_CHECK(block_id >= 0 && block_id < s1.total_blocks && ph >= 0 && ph < h->P, "bad index");
   RG_CUDA(cudaSetDevice(h->device));
-  std::vector<double> tmp((size_t)h->Npad * h->R, 0.0);
-  for (int r = 0; r < h->R; ++r)
-    for (int64_t s = 0; s < h->N; ++s) tmp[(size_t)r * h->Npad + h->pad_of[s]] = in[(size_t)r * h->N + s];
-  ensure_W(h);
-  RG_CHECK(h->W_host_tab[ph] != nullptr, "this rank holds no storage for that phenotype (rg_W_set_owned)");
-  double* dst = h->W_host_tab[ph] + (size_t)block_id * h->R * h->Npad;
+  std::vector<double> tmp((size_t)h->Npad * s1.R, 0.0);
+  for (int r = 0; r < s1.R; ++r)
+    for (int64_t s = 0; s < h->N; ++s) tmp[(size_t)r * h->Npad + s1.pad_of[s]] = in[(size_t)r * h->N + s];
+  ensure_W(h, s1);
+  RG_CHECK(s1.W_host_tab[ph] != nullptr, "this rank holds no storage for that phenotype (rg_W_set_owned)");
+  double* dst = s1.W_host_tab[ph] + (size_t)block_id * s1.R * h->Npad;
   RG_CUDA(cudaMemcpyAsync(dst, tmp.data(), tmp.size() * 8, cudaMemcpyHostToDevice, h->stream));
   RG_CUDA(cudaStreamSynchronize(h->stream));
   RG_API_END
@@ -1205,47 +1180,45 @@ int64_t rg_l0_status(rg_handle h) {
   }
   rg::flush_timers(h);
   try { rg::pgen_check_errors(h); } catch (const rg::Error& e) { rg::set_last_error(e.msg); return (int64_t)1 << 41; }
+  if (!h->s1) return 0;
   unsigned long long v = 0;
-  cudaMemcpy(&v, h->err_slot.p, 8, cudaMemcpyDeviceToHost);
-  if (v == ~0ull) return 0;
-  if (v >= (1ull << 40)) {
-    rg::set_last_error("Cholesky pivot not positive (system id " + std::to_string(v - (1ull << 40)) + ")");
-    return (int64_t)v;
-  }
-  rg::set_last_error("SNP has low variance (index " + std::to_string(v - 1) + ")");
-  return (int64_t)v;
+  cudaMemcpy(&v, h->s1->err_slot.p, 8, cudaMemcpyDeviceToHost);
+  return rg::l0_status_of(v);
 }
 
 int64_t rg_l0_poll_status(rg_handle h) {
-  if (!h || h->kind != 1 || !h->err_slot.p) return -1;
-  cudaSetDevice(h->device);
-  if (!h->poll_stream && cudaStreamCreateWithFlags(&h->poll_stream, cudaStreamNonBlocking) != cudaSuccess) return -1;
-  if (!h->poll_host && cudaHostAlloc((void**)&h->poll_host, 8, cudaHostAllocDefault) != cudaSuccess) return -1;
-  if (cudaMemcpyAsync(h->poll_host, h->err_slot.p, 8, cudaMemcpyDeviceToHost, h->poll_stream) != cudaSuccess ||
-      cudaStreamSynchronize(h->poll_stream) != cudaSuccess) {
-    rg::set_last_error(std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError()));
+  if (!h) return -1;
+  unsigned long long v = 0;
+  try {
+    Step1State& s1 = step1(h);
+    cudaSetDevice(h->device);
+    s1.poll_host.alloc(1);
+    const cudaStream_t ps = s1.poll_stream.ensure();
+    if (cudaMemcpyAsync(s1.poll_host.p, s1.err_slot.p, 8, cudaMemcpyDeviceToHost, ps) != cudaSuccess ||
+        cudaStreamSynchronize(ps) != cudaSuccess)
+      throw rg::Error{std::string("CUDA error: ") + cudaGetErrorString(cudaGetLastError())};
+    v = *s1.poll_host.p;
+  } catch (const rg::Error& e) {
+    rg::set_last_error(e.msg);
     return -1;
   }
-  const unsigned long long v = *h->poll_host;
-  if (v == ~0ull) return 0;
-  if (v >= (1ull << 40)) rg::set_last_error("Cholesky pivot not positive (system id " + std::to_string(v - (1ull << 40)) + ")");
-  else rg::set_last_error("SNP has low variance (index " + std::to_string(v - 1) + ")");
-  return (int64_t)v;
+  return rg::l0_status_of(v);
 }
 
 int rg_l0_fetch_W(rg_handle h, int32_t block_id, int32_t ph, double* out) {
   RG_API_BEGIN
   RG_CHECK(h && out, "null argument");
-  RG_CHECK(h->kind == 1 && block_id >= 0 && block_id < h->total_blocks && ph >= 0 && ph < h->P, "bad index");
+  Step1State& s1 = step1(h);
+  RG_CHECK(block_id >= 0 && block_id < s1.total_blocks && ph >= 0 && ph < h->P, "bad index");
   rg::sync_lanes(h);
-  std::vector<double> tmp((size_t)h->Npad * h->R);
-  ensure_W(h);
-  RG_CHECK(h->W_host_tab[ph] != nullptr, "this rank holds no storage for that phenotype (rg_W_set_owned)");
-  const double* src = h->W_host_tab[ph] + (size_t)block_id * h->R * h->Npad;   // local or peer-mapped
+  std::vector<double> tmp((size_t)h->Npad * s1.R);
+  ensure_W(h, s1);
+  RG_CHECK(s1.W_host_tab[ph] != nullptr, "this rank holds no storage for that phenotype (rg_W_set_owned)");
+  const double* src = s1.W_host_tab[ph] + (size_t)block_id * s1.R * h->Npad;   // local or peer-mapped
   RG_CUDA(cudaMemcpyAsync(tmp.data(), src, tmp.size() * 8, cudaMemcpyDeviceToHost, h->stream));
   RG_CUDA(cudaStreamSynchronize(h->stream));
-  for (int r = 0; r < h->R; ++r)
-    for (int64_t s = 0; s < h->N; ++s) out[(size_t)r * h->N + s] = tmp[(size_t)r * h->Npad + h->pad_of[s]];
+  for (int r = 0; r < s1.R; ++r)
+    for (int64_t s = 0; s < h->N; ++s) out[(size_t)r * h->N + s] = tmp[(size_t)r * h->Npad + s1.pad_of[s]];
   RG_API_END
 }
 
@@ -1265,10 +1238,11 @@ int64_t rg_debug_fetch(rg_handle h, const char* name, void* out, int64_t max_byt
 
 int rg_l0_solver_stats(rg_handle h, int64_t* mixed_blocks, int64_t* f64_fallbacks) {
   RG_API_BEGIN
-  RG_CHECK(h && h->kind == 1, "not a Step-1 handle");
+  RG_CHECK(h, "not a Step-1 handle");     // a null handle is no Step-1 handle either
+  Step1State& s1 = step1(h);
   rg::sync_lanes(h);
-  if (mixed_blocks) *mixed_blocks = h->mx_blocks;
-  if (f64_fallbacks) *f64_fallbacks = h->mx_fallbacks;
+  if (mixed_blocks) *mixed_blocks = s1.mx_blocks;
+  if (f64_fallbacks) *f64_fallbacks = s1.mx_fallbacks;
   RG_API_END
 }
 
@@ -1299,12 +1273,10 @@ int rg_dbg_mixed_solve(int32_t device, int32_t n, int32_t K, int32_t R, int32_t 
   RG_CUDA(cudaMemcpy(dl.p, lambda, R * 8, cudaMemcpyHostToDevice));
   for (int f = 0; f < K; ++f)
     RG_CUDA(cudaMemcpy(db.p + (size_t)f * Pp * n, b + (size_t)f * P * n, (size_t)P * n * 8, cudaMemcpyHostToDevice));
-  cudaStream_t st;
-  RG_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  mx.solve(dA.p, dl.p, db.p, dx.p, dr.p, P, steps, (float)tol, dfail.p, st);
+  rg::Stream st;
+  mx.solve(dA.p, dl.p, db.p, dx.p, dr.p, P, steps, (float)tol, dfail.p, st.ensure());
   cudaError_t e = cudaGetLastError();                        // a launch the device refused (shared memory, grid)
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaStreamDestroy(st);
   RG_CHECK(e == cudaSuccess, std::string("mixed solver kernels failed: ") + cudaGetErrorString(e));
   for (int m = 0; m < nmat; ++m)
     RG_CUDA(cudaMemcpy(x_out + (size_t)m * P * n, dx.p + (size_t)m * Pp * n, (size_t)P * n * 8, cudaMemcpyDeviceToHost));
