@@ -343,6 +343,8 @@ int rg_s2_block_bed_bt(rg_handle h, const uint8_t* packed, int64_t row_stride, i
  * rg_s2_firth -- approximate Firth test for selected (variant, trait) pairs of the resident block; replaces
  * fit_firth_logistic_snp_fast + fit_firth_pseudo / fit_firth (src/Step2_Models.cpp:1158-1252, 1527-1737).
  * beta is reported on the original allele coding; status != 0 in the low 4 bits = did not converge.
+ * The resident block (here and for rg_s2_spa) is that of the last block call if it was a binary-trait route and no
+ * rg_s2_set_chr_bt came after it; without one the call fails.
  */
 int rg_s2_firth(rg_handle h, int32_t n_sel, const int32_t* variant_idx, const int32_t* trait_idx, double* beta,
                 double* se, double* lrt, int32_t* status);

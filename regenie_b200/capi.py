@@ -522,7 +522,7 @@ class Step2:
         return status, coef, vcov
 
     def debug(self, name, dtype, count):
-        """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the last block; "s2_gp"
+        """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the resident block; "s2_gp"
         (uint32 [rows_p][Npad/16]), "s2_T" (float32 [chunk][3 rows_p][drows]) and "s2_FD" (int8 [drows][Npad]): the 2-bit
         rows, tensor sums and digit rows of F of the last 2-bit block.  GxE interaction: "int_F" (float64 [Npad][nf]),
         the feature rows rg_s2_set_interaction built; of the last interaction() call since then, "int_paths" (int64 x 8:

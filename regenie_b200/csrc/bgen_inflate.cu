@@ -80,7 +80,7 @@ __global__ void bgen_unpack_kernel(const uint8_t* __restrict__ raw, uint64_t raw
 
 static void bgen_inflate(rg_ctx* h, const uint8_t* comp, const uint64_t* comp_offs, int64_t n_file, int bs,
                          const uint8_t** probs_out, const uint8_t** miss_out) {
-  Step2State& s2 = step2(h);
+  Step2State::Input& in = step2(h).in;
   RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
   RG_CHECK(n_file > 0 && n_file < (1ll << 30), "bad sample count");
   for (int v = 0; v < bs; ++v) RG_CHECK(comp_offs[v + 1] >= comp_offs[v], "stream offsets must not decrease");
@@ -93,31 +93,31 @@ static void bgen_inflate(rg_ctx* h, const uint8_t* comp, const uint64_t* comp_of
   const uint64_t base = comp_offs[0], total = comp_offs[bs] - base;
   std::vector<uint64_t> rel(bs + 1);
   for (int v = 0; v <= bs; ++v) rel[v] = comp_offs[v] - base;
-  if ((size_t)total > s2.inflate_comp.n) s2.inflate_comp.alloc((size_t)(total + total / 4 + 4096));   // grows rarely
-  s2.inflate_offs.alloc((size_t)h->bs_max + 1);
-  s2.inflate_raw.alloc((size_t)h->bs_max * raw_stride);
-  s2.inflate_status.alloc((size_t)h->bs_max);
-  s2.probs_dev.alloc((size_t)h->bs_max * n_file * 2);
-  s2.miss_dev.alloc((size_t)h->bs_max * n_file);
-  copy_to_device(s2.inflate_comp.p, comp + base, (size_t)total, s);
-  RG_CUDA(cudaMemcpyAsync(s2.inflate_offs.p, rel.data(), rel.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+  if ((size_t)total > in.inflate_comp.n) in.inflate_comp.alloc((size_t)(total + total / 4 + 4096));   // grows rarely
+  in.inflate_offs.alloc((size_t)h->bs_max + 1);
+  in.inflate_raw.alloc((size_t)h->bs_max * raw_stride);
+  in.inflate_status.alloc((size_t)h->bs_max);
+  in.probs_dev.alloc((size_t)h->bs_max * n_file * 2);
+  in.miss_dev.alloc((size_t)h->bs_max * n_file);
+  copy_to_device(in.inflate_comp.p, comp + base, (size_t)total, s);
+  RG_CUDA(cudaMemcpyAsync(in.inflate_offs.p, rel.data(), rel.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
   const char* mode_env = getenv("RG_B200_INFLATE");          // read per call: the bench times both kernels in one process
   const bool use_window = mode_env && std::string(mode_env) == "window";
   if (use_window) {
     ensure_dyn_smem(reinterpret_cast<const void*>(bgen_inflate_window_kernel), kWindowSmem);
     bgen_inflate_window_kernel<<<(unsigned)ceil_div(bs, kWindowWarps), kWindowWarps * 32, kWindowSmem, s>>>(
-        s2.inflate_comp.p, s2.inflate_offs.p, s2.inflate_raw.p, raw_stride, raw_len, bs, s2.inflate_status.p);
+        in.inflate_comp.p, in.inflate_offs.p, in.inflate_raw.p, raw_stride, raw_len, bs, in.inflate_status.p);
   } else {
     bgen_inflate_kernel<<<(unsigned)ceil_div(bs, kInflateWarps), kInflateWarps * 32, 0, s>>>(
-        s2.inflate_comp.p, s2.inflate_offs.p, s2.inflate_raw.p, raw_stride, raw_len, bs, s2.inflate_status.p);
+        in.inflate_comp.p, in.inflate_offs.p, in.inflate_raw.p, raw_stride, raw_len, bs, in.inflate_status.p);
   }
   RG_CUDA(cudaGetLastError());
   const unsigned chunks = (unsigned)std::min<int64_t>(64, ceil_div(n_file, 1024));
-  bgen_unpack_kernel<<<dim3(chunks, (unsigned)bs), 256, 0, s>>>(s2.inflate_raw.p, raw_stride, (uint32_t)n_file, bs,
-                                                               s2.probs_dev.p, s2.miss_dev.p, s2.inflate_status.p);
+  bgen_unpack_kernel<<<dim3(chunks, (unsigned)bs), 256, 0, s>>>(in.inflate_raw.p, raw_stride, (uint32_t)n_file, bs,
+                                                               in.probs_dev.p, in.miss_dev.p, in.inflate_status.p);
   RG_CUDA(cudaGetLastError());
   std::vector<int32_t> st(bs);
-  RG_CUDA(cudaMemcpyAsync(st.data(), s2.inflate_status.p, (size_t)bs * 4, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaMemcpyAsync(st.data(), in.inflate_status.p, (size_t)bs * 4, cudaMemcpyDeviceToHost, s));
   RG_CUDA(cudaStreamSynchronize(s));
   h->launches += 2;
   for (int v = 0; v < bs; ++v) {
@@ -128,8 +128,8 @@ static void bgen_inflate(rg_ctx* h, const uint8_t* comp, const uint64_t* comp_of
     throw Error{"corrupt zlib stream in the bgen file at variant " + std::to_string(v) + " of the block (inflate status " +
                 std::to_string(st[v]) + ")."};
   }
-  *probs_out = s2.probs_dev.p;
-  *miss_out = s2.miss_dev.p;
+  *probs_out = in.probs_dev.p;
+  *miss_out = in.miss_dev.p;
 }
 
 }  // namespace rg

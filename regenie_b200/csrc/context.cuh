@@ -146,76 +146,87 @@ struct Step1State {
   int next_lane = 0, last_lane = 0;
 };
 
-// The state only a Step-2 handle has.  bt_: binary traits (rg_s2_set_chr_bt); dose_: 4-plane sums of the dosage and
-// 2-bit binary-trait routes; int_ / firth_: GxE, Firth and SPA; no prefix: quantitative traits and the shared inputs.
+// What rg_s2_set_chr / rg_s2_set_chr_bt build for one trait kind: the chromosome's feature rows F and, unless
+// RG_B200_S2_STATS=f64 was set at that call (tc), their digit rows for the tensor-core statistics of 2-bit blocks.
+struct S2Chr {
+  bool set = false, tc = false;      // set: the kind's chromosome call has run
+  int dp = 0, ncol = 0, col_male = -1;   // F [Npad][dp], ncol columns used; chrX: the male indicator's column (-1: none)
+  int drows = 0, nchunk = 0;
+  int64_t chunk_len = 0;             // samples per tensor-core chunk (the last one may be shorter)
+  DevBuf<double> F, Fscale;
+  DevBuf<uint8_t> FD;                // [drows][Npad] digit rows of F
+  DevBuf<int2> fold_k;               // the tensor-core sample chunks
+  CUtensorMap tmD;
+};
+struct S2QtChr : S2Chr { DevBuf<double> YtX, scf, male_tot; };
+struct S2BtChr : S2Chr { DevBuf<double> w, gs, xw, off, coltot, xwy, phat; DevBuf<int8_t> ym; };
+// The block the last block call left in the input, sum and output buffers, for rg_s2_firth / rg_s2_spa /
+// rg_s2_interaction and the sums hooks of rg_debug_fetch.  A block call replaces it; a chromosome call of its kind ends it.
+struct S2Block {
+  enum Kind { none, qt, bt } kind = none;
+  int bs = 0, rows_p = 0, dp = 0;
+  bool dz = false, dose = false;     // dz / the 4-plane sums hold the block's genotype words / sums
+};
+// The state only a Step-2 handle has.
 struct Step2State {
-  int strict = 0, dp = 0;
+  int strict = 0;
   std::vector<double> Xh;            // [N x C] host copy
   DevBuf<int4> chunks;               // [nchunks] sample chunks of the f64 reductions: (t0, len, 0, 0)
   int nchunks = 0;
-  DevBuf<double> F, part, sums, maskcount, YtX, XmX, scf;
-  DevBuf<double> out_d;              // packed f64 outputs
-  DevBuf<int32_t> out_i;             // packed i32 outputs
-  PinnedBuf<double> out_hd;          // pinned mirrors of the two output buffers (+ the INFO block)
-  PinnedBuf<int32_t> out_hi;
-  // 2-bit rows of the block: host rows copied to the device, the padded rows and their tensor maps keyed by rows_p
-  DevBuf<uint8_t> packed_dev;
-  DevBuf<uint32_t> gp;
-  std::map<int, CUtensorMap> gmaps;
-  // statistics on the tensor cores (bed / pgen input): the tiles Z F-digits keyed by rows_p * 4096 + drows / 256
-  std::map<int, TileList> stat_tile_lists;
-  bool tc = false;
-  int drows = 0, nchunk = 0, ncol = 0;
-  int64_t chunk_len = 0;                   // samples per tensor-core chunk (the last one may be shorter)
-  DevBuf<uint8_t> FD;                      // [drows][Npad] digit rows of F
-  DevBuf<double> Fscale;
-  DevBuf<float> T;                         // [chunk][3 rows_p][drows]
-  DevBuf<int2> fold_k;
+  DevBuf<double> maskcount, XmX;
   DevBuf<uint8_t> ones;
-  CUtensorMap tmD;
-  // chrX: male indicator of every sample (empty = none), F column of it, per-block non-PAR flags
-  std::vector<uint8_t> male;
-  int col_male = -1, bt_col_male = -1;
+  std::vector<uint8_t> male;         // chrX: male indicator of every sample (empty = none), per-block non-PAR flags
   DevBuf<uint8_t> nonpar;
   bool nonpar_set = false;
-  DevBuf<double> male_tot;
-  int bt_dp = 0, bt_ncol = 0;              // bt_ncol: used feature columns of the bt_dp padded ones
-  int fcols = 0;                           // the same for the quantitative-trait feature rows (dp)
-  bool chr_set = false, bt_chr_set = false;   // rg_s2_set_chr / rg_s2_set_chr_bt has run
-  int last_bs = 0;                         // variants resident in dz (for rg_s2_firth)
-  // padded rows of the sums the last block left, and the row width of dose_sums (rg_debug_fetch "s2_sums" / "bt_sums")
-  int sums_rows = 0, dose_sums_rows = 0, dose_sums_dp = 0;
-  DevBuf<uint8_t> probs_dev, miss_dev;
-  DevBuf<uint8_t> inflate_comp, inflate_raw;      // rg_bgen_inflate: compressed streams, inflated payloads
-  DevBuf<uint64_t> inflate_offs;
-  DevBuf<int32_t> inflate_status;
-  DevBuf<uint8_t> pgen_in, pgen_rows;             // rg_pgen_decode: records in, 2-bit rows out
-  DevBuf<uint32_t> dz;               // [rows_p][Npad] d | e << 10 | missing << 31
-  bool dz_qt = false;                // dz holds the words of the resident quantitative-trait block of this chromosome
-  // 4-plane sums of a block of dosages or of 2-bit hard calls (the binary-trait routes and the quantitative-trait dosage
-  // route): chunk partials, [rows_p][4][dp] sums, non-zero and hom-alt counts; the INFO scores of the dosage routes
-  DevBuf<double> dose_part, dose_sums, dose_nnz, dose_n510, dose_info;
-  DevBuf<int2> dose_cnt_part;        // [chunk][rows_p] non-zero / hom-alt counts of the dosage statistics kernel
-  DevBuf<double> qt_info_sums;       // [rows_p][dp] INFO sums of the quantitative-trait dosage route
-  // GxE interaction tests (rg_s2_set_interaction / rg_s2_interaction, csrc/s2_interaction.cu)
-  bool int_set = false;
-  DevBuf<int8_t> int_route;
-  int int_K = 0, int_nr = 0, int_nf = 0;
-  int int_last_bs = 0;               // variants of the last rg_s2_interaction since rg_s2_set_interaction (0: none)
-  DevBuf<double> int_F, int_E, int_part, int_sums, int_var, int_meat, int_out;
-  DevBuf<uint8_t> int_pow2;
-  DevBuf<int32_t> int_status;
-  // binary traits: the chromosome's state, the per-variant outputs Firth and SPA read back, and their selections
-  DevBuf<double> bt_F, bt_w, bt_gs, bt_xw, bt_off, bt_coltot, bt_xwy;
-  DevBuf<double> bt_xtwg, bt_mu, firth_gvec, firth_out, bt_den, bt_phat;
-  DevBuf<int8_t> bt_ym, firth_cflag;
-  DevBuf<int32_t> firth_sel, firth_status;
+  S2QtChr qt;
+  S2BtChr bt;
+  S2Block block;
+  struct Input {
+    DevBuf<uint8_t> packed_dev, probs_dev, miss_dev;   // host rows / probabilities / ploidy bytes copied to the device
+    DevBuf<uint32_t> gp;                            // the padded 2-bit rows and their tensor maps keyed by rows_p
+    std::map<int, CUtensorMap> gmaps;
+    DevBuf<uint8_t> inflate_comp, inflate_raw;      // rg_bgen_inflate: compressed streams, inflated payloads
+    DevBuf<uint64_t> inflate_offs;
+    DevBuf<int32_t> inflate_status;
+    DevBuf<uint8_t> pgen_in, pgen_rows;             // rg_pgen_decode: records in, 2-bit rows out
+    DevBuf<uint32_t> dz;                            // [rows_p][Npad] d | e << 10 | missing << 31
+  } in;
+  struct Sums {
+    // 3-plane sums [rows_p][3][dp] of the quantitative-trait finish, from FP64 chunk partials or the tensor digit sums
+    DevBuf<double> part, s3;
+    DevBuf<float> T;                 // [chunk][3 rows_p][drows]
+    std::map<int, TileList> tiles;   // the tiles Z F-digits, keyed by rows_p * 4096 + drows / 256
+    // 4-plane sums [rows_p][4][dp] of dosages or 2-bit binary-trait calls, with their chunk partials and non-zero /
+    // hom-alt counts; [rows_p][dp] INFO sums of the quantitative-trait dosage route
+    DevBuf<double> part4, s4, nnz, n510, qt_info;
+    DevBuf<int2> cnt_part;
+  } sums;
+  struct Outputs {
+    DevBuf<double> d; DevBuf<int32_t> i;          // packed f64 / i32 outputs
+    PinnedBuf<double> hd; PinnedBuf<int32_t> hi;  // their pinned mirrors (+ the INFO block)
+    DevBuf<double> xtwg, mu, den, info;   // of the binary-trait finish, read back by Firth and SPA; INFO scores
+  } out;
+  struct Selections {                // rg_s2_firth / rg_s2_spa: (variant, trait) indices of a batch, scratch, results
+    DevBuf<int32_t> idx, status;
+    DevBuf<double> gvec, out;
+    DevBuf<int8_t> cflag;
+  } sel;
+  struct Gxe {                       // rg_s2_set_interaction / rg_s2_interaction, csrc/s2_interaction.cu
+    bool set = false;
+    int K = 0, nr = 0, nf = 0, last_bs = 0;   // last_bs: variants of the last rg_s2_interaction since the set call
+    DevBuf<double> F, E, part, sums, var, meat, out;
+    DevBuf<uint8_t> pow2;
+    DevBuf<int8_t> route;
+    DevBuf<int32_t> status;
+  } gxe;
   // rg_s2_stage: input bytes of the NEXT block travel on a copy stream while the current block computes
   static constexpr int kStageSlots = 4;
-  DevBuf<uint8_t> stage[kStageSlots];
-  Event stage_ev[kStageSlots];
-  bool stage_pending[kStageSlots] = {false, false, false, false};
-  Stream copy_stream;
+  struct Staging {
+    DevBuf<uint8_t> buf[kStageSlots];
+    Event ev[kStageSlots];
+    bool pending[kStageSlots] = {false, false, false, false};
+    Stream copy_stream;
+  } stage;
 };
 
 }  // namespace rg

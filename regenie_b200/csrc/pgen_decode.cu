@@ -115,8 +115,8 @@ static void pgen_decode(rg_ctx* h, const rg_pgen_block* b, const uint8_t** rows_
   // where the rows go: Step 1 - the input buffer and stream of the lane the next rg_l0_block_bed call takes
   Step1State::Lane* L = h->s1 ? h->s1->lanes[h->s1->next_lane].get() : nullptr;
   const cudaStream_t s = L ? L->stream : h->stream;
-  rg::DevBuf<uint8_t>& rows = L ? L->packed_dev : h->s2->pgen_rows;
-  rg::DevBuf<uint8_t>& in = L ? L->pgen_in : h->s2->pgen_in;
+  rg::DevBuf<uint8_t>& rows = L ? L->packed_dev : h->s2->in.pgen_rows;
+  rg::DevBuf<uint8_t>& in = L ? L->pgen_in : h->s2->in.pgen_in;
   const uint32_t n = (uint32_t)b->n_file;
   const uint32_t words = (uint32_t)round_up(ceil_div(n, 16), 4);          // rows are multiples of 16 bytes
   const size_t stride = (size_t)words * 4;

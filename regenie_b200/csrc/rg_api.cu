@@ -774,37 +774,39 @@ static DebugView host_view(const T* p, size_t count) {
   return v;
 }
 
-// how Step 2 computed its last block, and the sums it came from
+// how Step 2 computed its resident block (digit rows of its trait kind, else the quantitative one's) and its sums
 static DebugView s2_debug_view(const rg_ctx* h, const Step2State& s2, const std::string& n) {
+  const S2Block& b = s2.block;
+  const S2Chr& c = b.kind == S2Block::bt ? static_cast<const S2Chr&>(s2.bt) : s2.qt;
   if (n == "s2_paths") {
-    const int64_t v[8] = {s2.tc ? 1 : 0, s2.nchunk, s2.chunk_len, s2.drows, s2.nchunks, h->Npad, s2.dp, s2.bt_dp};
+    const int64_t v[8] = {c.tc ? 1 : 0, c.nchunk, c.chunk_len, c.drows, s2.nchunks, h->Npad, s2.qt.dp, s2.bt.dp};
     return host_view(v, 8);
   }
-  if (n == "s2_sums") return dev_view(s2.sums.p, (size_t)s2.sums_rows * 3 * s2.dp * 8);                 // [rows_p][3][dp]
-  if (n == "bt_sums") return dev_view(s2.dose_sums.p, (size_t)s2.dose_sums_rows * 4 * s2.dose_sums_dp * 8);   // [rows_p][4][dp]
-  if (n == "bt_nnz") return dev_view(s2.dose_nnz.p, (size_t)s2.dose_sums_rows * 8);
-  if (n == "bt_n510") return dev_view(s2.dose_n510.p, (size_t)s2.dose_sums_rows * 8);
-  // the tensor sums, when the last block was a 2-bit one: its rows [rows_p][Npad/16], the digit sums
-  // [s2_nchunk][3 rows_p][drows] of the planes [G; G^2; Miss], and the digit rows of F [drows][Npad] they were taken against
-  const size_t rp = (size_t)round_up(s2.last_bs, kRowPad);
-  if (n == "s2_gp") return dev_view(s2.gp.p, rp * (h->Npad / 16) * 4);
-  if (n == "s2_T" && s2.tc) return dev_view(s2.T.p, (size_t)s2.nchunk * 3 * rp * s2.drows * 4);
-  if (n == "s2_FD" && s2.tc) return dev_view(s2.FD.p, (size_t)s2.drows * h->Npad);
+  // [rows_p][3][dp] of a quantitative-trait block, [rows_p][4][dp] and counts of a dosage or binary-trait block
+  if (n == "s2_sums") return dev_view(b.kind == S2Block::qt ? s2.sums.s3.p : nullptr, (size_t)b.rows_p * 3 * b.dp * 8);
+  if (n == "bt_sums") return dev_view(b.dose ? s2.sums.s4.p : nullptr, (size_t)b.rows_p * 4 * b.dp * 8);
+  if (n == "bt_nnz") return dev_view(b.dose ? s2.sums.nnz.p : nullptr, (size_t)b.rows_p * 8);
+  if (n == "bt_n510") return dev_view(b.dose ? s2.sums.n510.p : nullptr, (size_t)b.rows_p * 8);
+  // the tensor sums, when the block is a 2-bit one: its rows [rows_p][Npad/16], the digit sums
+  // [nchunk][3 rows_p][drows] of the planes [G; G^2; Miss], and the digit rows of F [drows][Npad] they were taken against
+  if (n == "s2_gp") return dev_view(s2.in.gp.p, (size_t)b.rows_p * (h->Npad / 16) * 4);
+  if (n == "s2_T" && c.tc) return dev_view(s2.sums.T.p, (size_t)c.nchunk * 3 * b.rows_p * c.drows * 4);
+  if (n == "s2_FD" && c.tc) return dev_view(c.FD.p, (size_t)c.drows * h->Npad);
   // GxE interaction state of the chromosome: its feature rows [Npad][nf] once rg_s2_set_interaction has run; the shape,
   // the routes [bs] and the chunk-reduced sums [bs][nf] (defined where the variant's route reads them) of the last
   // rg_s2_interaction call since then
   if (n.compare(0, 4, "int_") == 0) {
-    RG_CHECK(s2.int_set, "no interaction state on this handle: " + n);
-    if (n == "int_F") return dev_view(s2.int_F.p, (size_t)h->Npad * s2.int_nf * 8);
-    RG_CHECK(s2.int_last_bs > 0, "no rg_s2_interaction call since rg_s2_set_interaction: " + n);
-    const int bs = s2.int_last_bs;
+    const Step2State::Gxe& g = s2.gxe;
+    RG_CHECK(g.set, "no interaction state on this handle: " + n);
+    if (n == "int_F") return dev_view(g.F.p, (size_t)h->Npad * g.nf * 8);
+    RG_CHECK(g.last_bs > 0, "no rg_s2_interaction call since rg_s2_set_interaction: " + n);
     if (n == "int_paths") {
-      const int64_t v[8] = {s2.nchunks, h->Npad, s2.int_nf, s2.int_nr, s2.int_K, ceil_div(h->P, kIntTG),
-                            ceil_div(h->Npad, kIntSlab), bs};
+      const int64_t v[8] = {s2.nchunks, h->Npad, g.nf, g.nr, g.K, ceil_div(h->P, kIntTG), ceil_div(h->Npad, kIntSlab),
+                            g.last_bs};
       return host_view(v, 8);
     }
-    if (n == "int_route") return dev_view(s2.int_route.p, (size_t)bs);
-    if (n == "int_sums") return dev_view(s2.int_sums.p, (size_t)bs * s2.int_nf * 8);
+    if (n == "int_route") return dev_view(g.route.p, (size_t)g.last_bs);
+    if (n == "int_sums") return dev_view(g.sums.p, (size_t)g.last_bs * g.nf * 8);
   }
   throw Error{"unknown Step-2 debug buffer: " + n};
 }
@@ -902,7 +904,7 @@ static DebugView l0_debug_view(rg_ctx* h, Step1State& s1, const std::string& n) 
 static DebugView debug_view(rg_ctx* h, const std::string& n, int64_t max_bytes) {
   if (n == "pgen_rows") {
     // the rows the last rg_pgen_decode produced (Step 1: the next lane's input), cut to the caller's buffer
-    const DevBuf<uint8_t>& r = h->s1 ? h->s1->lanes[h->s1->next_lane]->packed_dev : h->s2->pgen_rows;
+    const DevBuf<uint8_t>& r = h->s1 ? h->s1->lanes[h->s1->next_lane]->packed_dev : h->s2->in.pgen_rows;
     RG_CHECK(r.p, "pgen_rows: no rg_pgen_decode has filled it");
     return dev_view(r.p, std::min<size_t>(r.n, (size_t)std::max<int64_t>(max_bytes, 0)));
   }
@@ -1019,7 +1021,7 @@ void rg_destroy(rg_handle h) {
     streams.push_back(h->s1->poll_stream);
     for (auto& l : h->s1->lanes) streams.insert(streams.end(), {l->stream, l->copy_stream});
   }
-  if (h->s2) streams.push_back(h->s2->copy_stream);
+  if (h->s2) streams.push_back(h->s2->stage.copy_stream);
   for (cudaStream_t s : streams) if (s) cudaStreamSynchronize(s);
   rg::flush_timers(h);
   delete h;                                 // the members release their streams, events, pinned buffers and mappings
