@@ -392,6 +392,53 @@ typedef struct rg_s2_int_opts {
  */
 int rg_s2_interaction(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, double* coef, double* vcov);
 
+/* ------------------------------------------------------------------ Step 2 (BT): GxE interaction tests */
+/*
+ * Per-chromosome state of the interaction tests of binary traits with a quantitative variable E (--interaction VAR, E
+ * kept as a covariate).  Call it after rg_s2_set_chr_bt; the next rg_s2_set_chr_bt clears it.  As in the reference, E and
+ * E^2 join the covariates of a binary-trait run (src/Pheno.cpp:91-95, :1073-1076), so the X of rg_step2_create must be
+ * the basis of [covariates, E, E^2].
+ *   E       [N]     pheno_data.interaction_cov (raw values; only the analysed samples are read)
+ *   offset  [P][N]  m_ests.offset_nullreg: linear predictor of each trait's null logistic fit with its LOCO offset
+ *                   (src/Step1_Models.cpp:63, :135)
+ */
+typedef struct rg_s2_int_bt_chr {
+  const double* E;
+  const double* offset;
+} rg_s2_int_bt_chr;
+int rg_s2_set_interaction_bt(rg_handle h, const rg_s2_int_bt_chr* st);
+
+/*
+ * rg_s2_interaction_bt -- the logistic interaction model of every (variant, trait) pair of the block left resident by
+ * the last rg_s2_block_bed_bt / rg_s2_block_bgen8_bt call (get_interaction_terms + apply_interaction_tests_bt,
+ * src/Interaction.cpp:44-92, :441-678): H = [G_res / scale_fac, resid(E o G) / scf_i] in the minor-allele coding,
+ * fit_logistic from beta = 0 with offset_nullreg (check_hs_dev on, then off), V = (H^T W H)^-1, and the HC3 sandwich when
+ * robust SEs are forced, or unless no_robust, for traits with MAC > rare_mac where either Wald p-value is below 0.05.
+ * opts.force_hc4 is not used for binary traits.  Outputs are host arrays, variant-major:
+ *   status [bs][P]     0 = no interaction rows (variant or trait ignored, or resid(E o G) or G_res has sd < numtol),
+ *                      1 = robust (HC3) SEs, 3 = model-based SEs, -1 = H^T W H near-singular or a negative robust
+ *                      variance, -2 = the logistic regression failed
+ *   coef   [bs][P][2]  (beta_G, beta_GxE) on the scale of the printed rows (divided by scale_fac, scf_i), sign-corrected
+ *                      for flipped alleles
+ *   vcov   [bs][P][4]  their 2 x 2 covariance (row-major), on the same scale
+ * ADD-INT_SNP and ADD-INT_SNPxVAR are beta / sqrt(vcov diagonal) Wald tests, ADD-INT_2DF is coef^T vcov^-1 coef (2 df).
+ */
+int rg_s2_interaction_bt(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, double* coef, double* vcov);
+
+/*
+ * rg_s2_interaction_firth -- the Firth fallback of the interaction tests (--firth, for pairs whose GxE Wald p-value is
+ * at most pThresh; apply_interaction_tests_firth, src/Interaction.cpp:680-863) for selected (variant, trait) pairs.
+ * Needs rg_s2_interaction_bt on the resident block and the null-Firth offsets (rg_s2_bt_chr.firth_offset).  Three
+ * penalised fits (fit_firth_nr, src/Step2_Models.cpp:1267-1383, with the offsets): both columns from 0, G dropped from
+ * (0, beta_GxE), GxE dropped from (beta_G, 0).  Outputs per pair, host arrays:
+ *   coef [n][2], se [n][2]  of the full fit, on the printed scale, sign-corrected for flipped alleles
+ *   lrt  [n][3]             ADD-INT_2DF = dev0 - dev (2 df), ADD-INT_SNP and ADD-INT_SNPxVAR = dev_dropped - dev (1 df)
+ *   status [n]              0 = rows, 1 / 2 / 3 = the full / G-dropped / GxE-dropped fit failed, 4 = a negative LRT,
+ *                           5 = the variant has no interaction rows; any non-zero status means no rows for the pair
+ */
+int rg_s2_interaction_firth(rg_handle h, int32_t n_sel, const int32_t* variant_idx, const int32_t* trait_idx,
+                            double* coef, double* se, double* lrt, int32_t* status);
+
 /* ------------------------------------------------------------------ PGEN records (SURVEY 8 (f)3) */
 /*
  * rg_pgen_decode -- the variant records of one block of a PLINK 2 .pgen (hard calls), decoded ON THE DEVICE into

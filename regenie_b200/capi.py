@@ -77,7 +77,7 @@ EXPORTS = [
     "rg_last_error", "rg_version", "rg_device_count", "rg_step1_create", "rg_destroy", "rg_sync",
     "rg_l0_block_bed", "rg_l0_status", "rg_l0_fetch_W", "rg_l1_fit", "rg_loco", "rg_step2_create",
     "rg_s2_set_chr", "rg_s2_block_bed", "rg_W_info", "rg_debug_fetch", "rg_launch_count", "rg_stream",
-    "rg_set_timing", "rg_get_timing", "rg_fence", "rg_s2_set_chr_bt", "rg_s2_block_bgen8_bt", "rg_s2_block_bgen8", "rg_s2_firth", "rg_l1_fit_bt", "rg_W_set_owned", "rg_W_export", "rg_W_attach_peer", "rg_l1_select", "rg_s2_set_sex", "rg_s2_set_non_par", "rg_l0_load_W", "rg_s2_spa", "rg_s2_block_bed_bt", "rg_prs", "rg_bgen_inflate", "rg_s2_set_interaction", "rg_s2_interaction",
+    "rg_set_timing", "rg_get_timing", "rg_fence", "rg_s2_set_chr_bt", "rg_s2_block_bgen8_bt", "rg_s2_block_bgen8", "rg_s2_firth", "rg_l1_fit_bt", "rg_W_set_owned", "rg_W_export", "rg_W_attach_peer", "rg_l1_select", "rg_s2_set_sex", "rg_s2_set_non_par", "rg_l0_load_W", "rg_s2_spa", "rg_s2_block_bed_bt", "rg_prs", "rg_bgen_inflate", "rg_s2_set_interaction", "rg_s2_interaction", "rg_s2_set_interaction_bt", "rg_s2_interaction_bt", "rg_s2_interaction_firth",
     "rg_l0_solver_stats", "rg_dbg_mixed_solve", "rg_l0_wait_input", "rg_l0_block_dosage_u8", "rg_l0_block_f64", "rg_W_attach_local",
     "rg_s2_stage", "rg_host_alloc", "rg_host_free", "rg_pgen_decode", "rg_warmup", "rg_l0_poll_status",
 ]
@@ -308,6 +308,10 @@ class S2IntOpts(C.Structure):
                 ("force_hc4", C.c_int32), ("no_robust", C.c_int32)]
 
 
+class S2IntBtChr(C.Structure):
+    _fields_ = [("E", C.c_void_p), ("offset", C.c_void_p)]
+
+
 class Step2:
     """Host-side mirror of the Step-2 QT call sequence of Data::test_snps_fast (src/Data.cpp:2230-2383)."""
 
@@ -520,6 +524,48 @@ class Step2:
         o = S2IntOpts(float(rare_mac), float(min_mac), int(force_robust), int(force_hc4), int(no_robust))
         check(L.rg_s2_interaction(self.h, C.byref(o), _ptr(status), _ptr(coef), _ptr(vcov)))
         return status, coef, vcov
+
+    # ---- GxE interaction tests (binary traits)
+    def set_interaction_bt(self, E, offset):
+        """rg_s2_set_interaction_bt after set_chr_bt.  E [N]; offset [N x P], the linear predictor of each trait's null
+        logistic fit (offset_nullreg)."""
+        L = lib()
+        L.rg_s2_set_interaction_bt.argtypes = [C.c_void_p, C.c_void_p]
+        E = np.ascontiguousarray(E, dtype=np.float64)
+        off = _f64(offset)
+        if E.shape != (self.N,) or off.shape != (self.N, self.P):
+            raise ValueError("set_interaction_bt: E must have %d entries and offset shape (%d, %d)" % (self.N, self.N, self.P))
+        st = S2IntBtChr(E.ctypes.data, off.ctypes.data)
+        check(L.rg_s2_set_interaction_bt(self.h, C.byref(st)))
+
+    def interaction_bt(self, rare_mac=1000.0, min_mac=5.0, force_robust=False, no_robust=False):
+        """rg_s2_interaction_bt on the resident binary-trait block: (status [bs, P], coef [bs, P, 2], vcov [bs, P, 2, 2]).
+        Raises ValueError, without calling the library, when no block call has succeeded on this handle."""
+        if self.last_bs is None:
+            raise ValueError("interaction_bt() needs a block call first")
+        L = lib()
+        L.rg_s2_interaction_bt.argtypes = [C.c_void_p] * 5
+        bs, P = self.last_bs, self.P
+        status = np.empty((bs, P), dtype=np.int32)
+        coef, vcov = np.empty((bs, P, 2)), np.empty((bs, P, 2, 2))
+        o = S2IntOpts(float(rare_mac), float(min_mac), int(force_robust), 0, int(no_robust))
+        check(L.rg_s2_interaction_bt(self.h, C.byref(o), _ptr(status), _ptr(coef), _ptr(vcov)))
+        return status, coef, vcov
+
+    def interaction_firth(self, variant_idx, trait_idx):
+        """rg_s2_interaction_firth for the pairs (variant_idx[k], trait_idx[k]) of the resident block: (coef [n, 2],
+        se [n, 2], lrt [n, 3] = (2DF, SNP, SNPxVAR), status [n])."""
+        L = lib()
+        L.rg_s2_interaction_firth.argtypes = [C.c_void_p, C.c_int32] + [C.c_void_p] * 6
+        vi = np.ascontiguousarray(variant_idx, dtype=np.int32).reshape(-1)
+        ti = np.ascontiguousarray(trait_idx, dtype=np.int32).reshape(-1)
+        if len(vi) != len(ti):
+            raise ValueError("interaction_firth: %d variant indices, %d trait indices" % (len(vi), len(ti)))
+        n = len(vi)
+        coef, se, lrt = np.empty((n, 2)), np.empty((n, 2)), np.empty((n, 3))
+        status = np.empty(n, dtype=np.int32)
+        check(L.rg_s2_interaction_firth(self.h, n, _ptr(vi), _ptr(ti), _ptr(coef), _ptr(se), _ptr(lrt), _ptr(status)))
+        return coef, se, lrt, status
 
     def debug(self, name, dtype, count):
         """rg_debug_fetch: "s2_paths" (int64 x 8), "s2_sums", "bt_sums", "bt_nnz", "bt_n510" of the resident block; "s2_gp"

@@ -159,7 +159,11 @@ struct S2Chr {
   CUtensorMap tmD;
 };
 struct S2QtChr : S2Chr { DevBuf<double> YtX, scf, male_tot; };
-struct S2BtChr : S2Chr { DevBuf<double> w, gs, xw, off, coltot, xwy, phat; DevBuf<int8_t> ym; };
+struct S2BtChr : S2Chr {
+  DevBuf<double> w, gs, xw, off, coltot, xwy, phat;
+  DevBuf<int8_t> ym;
+  bool firth = false;                // off holds the null-Firth offsets (rg_s2_bt_chr.firth_offset was given)
+};
 // The block the last block call left in the input, sum and output buffers, for rg_s2_firth / rg_s2_spa /
 // rg_s2_interaction and the sums hooks of rg_debug_fetch.  A block call replaces it; a chromosome call of its kind ends it.
 struct S2Block {
@@ -181,6 +185,7 @@ struct Step2State {
   S2QtChr qt;
   S2BtChr bt;
   S2Block block;
+  int64_t block_serial = 0;          // block calls so far: tells whether a result belongs to the resident block
   struct Input {
     DevBuf<uint8_t> packed_dev, probs_dev, miss_dev;   // host rows / probabilities / ploidy bytes copied to the device
     DevBuf<uint32_t> gp;                            // the padded 2-bit rows and their tensor maps keyed by rows_p
@@ -219,6 +224,15 @@ struct Step2State {
     DevBuf<int8_t> route;
     DevBuf<int32_t> status;
   } gxe;
+  struct GxeBt {                     // rg_s2_set_interaction_bt / rg_s2_interaction_bt / _firth, csrc/s2_interaction_bt.cu
+    bool set = false;
+    int nf = 0;
+    int64_t wald_serial = -1;        // block_serial of the block the last rg_s2_interaction_bt ran on
+    DevBuf<double> F, E, off, part, sums, var, H, out;
+    DevBuf<uint8_t> pow2;
+    DevBuf<int8_t> route;
+    DevBuf<int32_t> status, sel;
+  } gxe_bt;
   // rg_s2_stage: input bytes of the NEXT block travel on a copy stream while the current block computes
   static constexpr int kStageSlots = 4;
   struct Staging {

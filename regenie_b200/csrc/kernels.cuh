@@ -391,6 +391,15 @@ struct SpaArgs {
 void launch_s2_spa(const SpaArgs& a, cudaStream_t s);
 
 // ---- s2_interaction.cu
+// near-singular check and inverse of a symmetric 2 x 2 (SelfAdjointEigenSolver + eigenvalues().minCoeff() < numtol)
+__device__ inline bool int_inv2(double a11, double a12, double a22, double numtol, double* z) {
+  const double hm = 0.5 * (a11 + a22), hd = 0.5 * (a11 - a22);
+  const double lmin = hm - sqrt(hd * hd + a12 * a12);
+  if (!(lmin >= numtol)) return false;
+  const double det = a11 * a22 - a12 * a12;
+  z[0] = a22 / det; z[1] = -a12 / det; z[2] = a11 / det;
+  return true;
+}
 constexpr int kIntTG = 8;            // traits per CTA of the meat kernel (blockIdx.z = trait group)
 constexpr int64_t kIntSlab = 16384;  // samples per host slab of the feature rows (rg_s2_set_interaction)
 struct S2IntArgs {
@@ -414,5 +423,50 @@ struct S2IntArgs {
   int8_t* route;                     // [bs] 0 none, 1 robust, 2 HLM (written by the first kernel)
 };
 void launch_s2_interaction(const S2IntArgs& a, const uint8_t* pow2, double* part, cudaStream_t s);
+// sums[v][f] = sum over the samples of g_v^(1 or 2) Fint[i][f] (pow2[f]) for the variants with route[v] == 1 (the robust
+// columns [0, nr) of s2_int_sums_kernel; nr = nf for the binary-trait feature rows).  g is the mean-imputed genotype:
+// missing calls take 2 af_all[v] when mu is null, else mu[v], with non-missing calls flipped to 2 - g when flags[v] & 8.
+void launch_s2_int_sums(const uint32_t* dz, int64_t npad, const double* af_all, const double* mu, const int32_t* flags,
+                        int bs, const int8_t* route, int nr, const double* Fint, int nf, const uint8_t* pow2,
+                        const int4* chunks, int nchunks, double* part, double* sums, cudaStream_t s);
+
+// ---- s2_interaction_bt.cu
+constexpr int kIntBtTG = 4;          // traits per CTA of the logistic kernel (blockIdx.y = trait group)
+constexpr int kIntBtBatch = 128;     // variants (Wald) or pairs (Firth) whose H columns are materialised at a time
+struct S2IntBtArgs {
+  int bs, C, P, nf, nchunks, var_stride;
+  int force_robust, no_robust;
+  long long n_analyzed;
+  double rare_mac, min_mac, numtol;
+  int64_t npad;
+  const uint32_t* dz;                // [rows_p][Npad] genotype words of the resident block
+  const double* Fint;                // [Npad][nf] X_c, E X_c (times g), 1, E, E^2 (times g^2); zero outside the analysis
+  const double* E;                   // [Npad]
+  const int8_t* ym;                  // [P][Npad] 0 masked, 1 control, 2 case
+  const double* off;                 // [P][Npad] offset of the fits (offset_nullreg, or the null-Firth offset)
+  const int4* chunks;
+  const double *af_all, *mu, *mac;
+  const int32_t* flags;
+  int8_t* route;                     // [bs] 1 = the variant is tested
+  double* sums;                      // [bs][nf]
+  double* var;                       // [bs][var_stride]: ok, scale_fac, scf_i, X^T G [C], X^T (E o G) [C]
+  double* H;                         // [kIntBtBatch][2][Npad] the H columns of a batch
+  int v0, nb;                        // the batch: variants v0 .. v0 + nb (Wald)
+  // Wald outputs [bs][P]
+  int32_t* status;
+  double *coef, *vcov;               // [bs][P][2], [bs][P][4]
+  // Firth: pair k of the batch is (sel_var[k], sel_trait[k]); H slot k holds its variant's columns
+  const int32_t *sel_var, *sel_trait;
+  int niter;
+  double tol, maxstep;
+  double *f_coef, *f_se, *f_lrt;     // [nb][2], [nb][2], [nb][3]
+  int32_t* f_status;                 // [nb]
+};
+// route, per-variant sums, scales and residualisation coefficients of every variant of the block
+void launch_s2_int_bt_prep(const S2IntBtArgs& a, const uint8_t* pow2, double* part, cudaStream_t s);
+// H columns of the batch, then the logistic fits of its variants (every trait)
+void launch_s2_int_bt_wald(const S2IntBtArgs& a, cudaStream_t s);
+// H columns of the batch's pairs, then the three Firth fits of each pair
+void launch_s2_int_bt_firth(const S2IntBtArgs& a, cudaStream_t s);
 
 }  // namespace rg

@@ -220,6 +220,7 @@ static std::pair<Step2State&, Chr&> s2_block_begin(rg_ctx* h, Chr Step2State::*k
   RG_CHECK(bs > 0 && bs <= h->bs_max, "block size out of range");
   RG_CHECK(c.set, std::string(std::is_same<Chr, S2BtChr>::value ? "rg_s2_set_chr_bt" : "rg_s2_set_chr") + " has not been called");
   s2.block = S2Block();
+  ++s2.block_serial;
   RG_CUDA(cudaSetDevice(h->device));
   s2_wait_stage(h, s2, in, h->stream);
   s2_wait_stage(h, s2, in2, h->stream);
@@ -328,7 +329,10 @@ static void s2_set_chr_bt(rg_ctx* h, const rg_s2_bt_chr* st) {
   upload(b.xw, xw, h->stream); upload(b.ym, ym, h->stream); upload(b.phat, phat, h->stream);
   s2_build_digits(h, s2, b);                                         // for rg_s2_block_bed_bt
   RG_CUDA(cudaStreamSynchronize(h->stream));
+  b.firth = st->firth_offset != nullptr;
   b.set = true;
+  s2.gxe_bt.set = false;                                             // rg_s2_set_interaction_bt follows, per chromosome
+  s2.gxe_bt.wald_serial = -1;
 }
 
 // the per-variant buffers of the binary-trait finish (S2BtFinalizeArgs), which rg_s2_firth / rg_s2_spa read back
@@ -586,6 +590,122 @@ static void s2_interaction(rg_ctx* h, const rg_s2_int_opts* o, int32_t* status, 
   RG_CUDA(cudaStreamSynchronize(s));
 }
 
+// ---------------------------------------------------------------- GxE interaction tests (binary traits)
+// Feature rows [Npad][2 C + 2] of the per-variant sums: X_c, E X_c (times g), 1, E^2 (times g^2), zero outside the
+// analysis; X is the covariate basis of rg_step2_create, which spans E and E^2 as well.
+static void s2_set_interaction_bt(rg_ctx* h, const rg_s2_int_bt_chr* st) {
+  Step2State& s2 = step2(h);
+  RG_CHECK(s2.bt.set, "rg_s2_set_interaction_bt needs a Step-2 handle after rg_s2_set_chr_bt");
+  RG_CUDA(cudaSetDevice(h->device));
+  const int64_t N = h->N, Npad = h->Npad;
+  const int C = h->C, P = h->P, nf = 2 * C + 2;
+  auto& g = s2.gxe_bt;
+  std::vector<double> E(Npad, 0.0), off((size_t)P * Npad, 0.0);
+  std::vector<uint8_t> pow2(nf, 0);
+  pow2[2 * C] = pow2[2 * C + 1] = 1;
+  for (int64_t s = 0; s < N; ++s) E[s] = h->in_analysis[s] ? st->E[s] : 0.0;
+  for (int p = 0; p < P; ++p)
+    for (int64_t s = 0; s < N; ++s) off[(size_t)p * Npad + s] = st->offset[(size_t)p * N + s];
+  upload(g.E, E, h->stream); upload(g.off, off, h->stream); upload(g.pow2, pow2, h->stream);
+  g.F.alloc((size_t)Npad * nf);
+  std::vector<double> F((size_t)kIntSlab * nf);
+  for (int64_t s0 = 0; s0 < Npad; s0 += kIntSlab) {
+    const int64_t ns = std::min(kIntSlab, Npad - s0);
+    RG_CUDA(cudaStreamSynchronize(h->stream));                       // the previous slab's upload has finished
+    std::fill(F.begin(), F.end(), 0.0);
+    for (int64_t s = s0; s < std::min(s0 + ns, N); ++s) {
+      if (!h->in_analysis[s]) continue;
+      const double e = E[s];
+      double* r = &F[(size_t)(s - s0) * nf];
+      for (int c = 0; c < C; ++c) { r[c] = s2.Xh[(size_t)c * N + s]; r[C + c] = e * r[c]; }
+      r[2 * C] = 1.0; r[2 * C + 1] = e * e;
+    }
+    RG_CUDA(cudaMemcpyAsync(g.F.p + (size_t)s0 * nf, F.data(), (size_t)ns * nf * 8, cudaMemcpyHostToDevice, h->stream));
+  }
+  RG_CUDA(cudaStreamSynchronize(h->stream));
+  g.nf = nf;
+  g.wald_serial = -1;
+  g.set = true;
+}
+
+// the arguments both binary-trait interaction calls share
+static S2IntBtArgs s2_int_bt_args(rg_ctx* h, Step2State& s2) {
+  const rg_s2_out d = s2_out_at(h, s2.out.d.p, s2.out.i.p);
+  auto& g = s2.gxe_bt;
+  S2IntBtArgs a{};
+  a.bs = s2.block.bs; a.C = h->C; a.P = h->P; a.nf = g.nf; a.nchunks = s2.nchunks; a.var_stride = 3 + 2 * h->C;
+  a.n_analyzed = h->n_analyzed; a.numtol = 1e-6; a.npad = h->Npad;
+  a.dz = s2.in.dz.p; a.Fint = g.F.p; a.E = g.E.p; a.ym = s2.bt.ym.p; a.chunks = s2.chunks.p;
+  a.af_all = d.af_all; a.mu = s2.out.mu.p; a.mac = d.mac; a.flags = d.flags;
+  g.var.alloc((size_t)h->bs_max * a.var_stride);
+  g.H.alloc((size_t)kIntBtBatch * 2 * h->Npad);
+  a.route = g.route.p; a.sums = g.sums.p; a.var = g.var.p; a.H = g.H.p;
+  return a;
+}
+
+static void s2_interaction_bt(rg_ctx* h, const rg_s2_int_opts* o, int32_t* status, double* coef, double* vcov) {
+  Step2State& s2 = step2(h);
+  auto& g = s2.gxe_bt;
+  RG_CHECK(g.set, "rg_s2_interaction_bt needs rg_s2_set_interaction_bt");
+  RG_CHECK(s2.block.kind == S2Block::bt && s2.block.dz,
+           "rg_s2_interaction_bt needs the block of the last rg_s2_block_bed_bt / rg_s2_block_bgen8_bt call on the "
+           "current chromosome");
+  RG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  const int bs = s2.block.bs, P = h->P;
+  g.route.alloc(h->bs_max); g.sums.alloc((size_t)h->bs_max * g.nf);
+  g.part.alloc((size_t)s2.nchunks * round_up(h->bs_max, 16) * g.nf);
+  g.out.alloc((size_t)h->bs_max * P * 6); g.status.alloc((size_t)h->bs_max * P);
+  S2IntBtArgs a = s2_int_bt_args(h, s2);
+  a.off = g.off.p;
+  a.rare_mac = o->rare_mac; a.min_mac = o->min_mac; a.force_robust = o->force_robust; a.no_robust = o->no_robust;
+  a.status = g.status.p; a.coef = g.out.p; a.vcov = g.out.p + (size_t)bs * P * 2;
+  launch_s2_int_bt_prep(a, g.pow2.p, g.part.p, s);
+  h->launches += 4;
+  for (int v0 = 0; v0 < bs; v0 += kIntBtBatch) {
+    a.v0 = v0; a.nb = std::min(kIntBtBatch, bs - v0);
+    launch_s2_int_bt_wald(a, s);
+    h->launches += 2;
+  }
+  RG_CUDA(cudaMemcpyAsync(status, a.status, (size_t)bs * P * 4, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaMemcpyAsync(coef, a.coef, (size_t)bs * P * 2 * 8, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaMemcpyAsync(vcov, a.vcov, (size_t)bs * P * 4 * 8, cudaMemcpyDeviceToHost, s));
+  RG_CUDA(cudaStreamSynchronize(s));
+  g.wald_serial = s2.block_serial;
+}
+
+static void s2_interaction_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* coef,
+                                 double* se, double* lrt, int32_t* status) {
+  Step2State& s2 = step2(h);
+  auto& g = s2.gxe_bt;
+  RG_CHECK(s2.block.kind == S2Block::bt && g.set && g.wald_serial == s2.block_serial,
+           "rg_s2_interaction_firth needs rg_s2_interaction_bt on the resident binary-trait block");
+  RG_CHECK(s2.bt.firth, "rg_s2_interaction_firth needs the null-Firth offsets (rg_s2_bt_chr.firth_offset)");
+  for (int k = 0; k < n_sel; ++k)
+    RG_CHECK(var_idx[k] >= 0 && var_idx[k] < s2.block.bs && trait_idx[k] >= 0 && trait_idx[k] < h->P, "selection out of range");
+  RG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t s = h->stream;
+  S2IntBtArgs a = s2_int_bt_args(h, s2);
+  a.off = s2.bt.off.p; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;    // niter_max_firth, numtol_firth, maxstep
+  g.sel.alloc(2 * kIntBtBatch + kIntBtBatch);
+  g.out.alloc(7 * kIntBtBatch);
+  a.sel_var = g.sel.p; a.sel_trait = g.sel.p + kIntBtBatch; a.f_status = g.sel.p + 2 * kIntBtBatch;
+  a.f_coef = g.out.p; a.f_se = g.out.p + 2 * kIntBtBatch; a.f_lrt = g.out.p + 4 * kIntBtBatch;
+  for (int o = 0; o < n_sel; o += kIntBtBatch) {
+    const int nb = std::min(kIntBtBatch, n_sel - o);
+    a.nb = nb;
+    RG_CUDA(cudaMemcpyAsync(g.sel.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+    RG_CUDA(cudaMemcpyAsync(g.sel.p + kIntBtBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+    launch_s2_int_bt_firth(a, s);
+    h->launches += 2;
+    RG_CUDA(cudaMemcpyAsync(coef + 2 * o, a.f_coef, nb * 2 * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(se + 2 * o, a.f_se, nb * 2 * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(lrt + 3 * o, a.f_lrt, nb * 3 * 8, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaMemcpyAsync(status + o, a.f_status, nb * 4, cudaMemcpyDeviceToHost, s));
+    RG_CUDA(cudaStreamSynchronize(s));
+  }
+}
+
 extern "C" {
 
 int rg_s2_set_interaction(rg_handle h, const rg_s2_int_chr* st) {
@@ -599,6 +719,31 @@ int rg_s2_interaction(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, 
   RG_API_BEGIN
   RG_CHECK(h && opts && status && coef && vcov, "null argument");
   s2_interaction(h, opts, status, coef, vcov);
+  RG_CUDA(cudaGetLastError());
+  RG_API_END
+}
+
+int rg_s2_set_interaction_bt(rg_handle h, const rg_s2_int_bt_chr* st) {
+  RG_API_BEGIN
+  RG_CHECK(h && st && st->E && st->offset, "null argument");
+  s2_set_interaction_bt(h, st);
+  RG_API_END
+}
+
+int rg_s2_interaction_bt(rg_handle h, const rg_s2_int_opts* opts, int32_t* status, double* coef, double* vcov) {
+  RG_API_BEGIN
+  RG_CHECK(h && opts && status && coef && vcov, "null argument");
+  s2_interaction_bt(h, opts, status, coef, vcov);
+  RG_CUDA(cudaGetLastError());
+  RG_API_END
+}
+
+int rg_s2_interaction_firth(rg_handle h, int32_t n_sel, const int32_t* variant_idx, const int32_t* trait_idx, double* coef,
+                            double* se, double* lrt, int32_t* status) {
+  RG_API_BEGIN
+  RG_CHECK(h && (n_sel == 0 || (variant_idx && trait_idx && coef && se && lrt && status)), "null argument");
+  RG_CHECK(n_sel >= 0, "n_sel < 0");
+  if (n_sel > 0) s2_interaction_firth(h, n_sel, variant_idx, trait_idx, coef, se, lrt, status);
   RG_CUDA(cudaGetLastError());
   RG_API_END
 }

@@ -12,7 +12,8 @@
 // The meat sum_i e_i^2 / (1 - h_i)^2 H_i H_i^T needs the leverages h_i and residuals e_i, which are nonlinear in the
 // samples: one pass per robust variant (per 8 traits) with a fixed-order block reduction per sample chunk
 // (s2_int_meat_kernel).  A first kernel fixes each variant's route, so the sums kernel forms only the columns that route
-// reads and ignored variants do no work.
+// reads and ignored variants do no work.  The binary-trait tests (s2_interaction_bt.cu) run the same sums kernel on their
+// own feature rows, with the genotype in the block's minor-allele coding (launch_s2_int_sums).
 #include "kernels.cuh"
 
 namespace rg {
@@ -33,7 +34,9 @@ __device__ __forceinline__ bool int_needs(int8_t route, int f, int nr) { return 
 // part[chunk][v][f] = sum over the chunk's samples of g_v(i)^(1 or 2) F[i][f], for the (v, f) the route of v reads; a
 // CTA whose variants need none of its columns returns at once
 __global__ void __launch_bounds__(kIntThreads) s2_int_sums_kernel(const uint32_t* __restrict__ dz, int64_t npad,
-                                                                  const double* __restrict__ af_all, int bs,
+                                                                  const double* __restrict__ af_all,
+                                                                  const double* __restrict__ mu,
+                                                                  const int32_t* __restrict__ flags, int bs,
                                                                   const int8_t* __restrict__ route, int nr,
                                                                   const double* __restrict__ F, int nf,
                                                                   const uint8_t* __restrict__ pow2, const int4* chunks,
@@ -56,8 +59,15 @@ __global__ void __launch_bounds__(kIntThreads) s2_int_sums_kernel(const uint32_t
     for (int k = threadIdx.x; k < kIntVT * kIntSub; k += kIntThreads) {
       const int v = k / kIntSub, j = k % kIntSub;
       double g = 0.0;
-      if (v0 + v < bs && route[v0 + v] > 0 && j < len)
-        g = int_g(dz[(int64_t)(v0 + v) * npad + ch.x + o + j], 2.0 * af_all[v0 + v]);
+      if (v0 + v < bs && route[v0 + v] > 0 && j < len) {
+        const uint32_t w = dz[(int64_t)(v0 + v) * npad + ch.x + o + j];
+        if (!mu) {
+          g = int_g(w, 2.0 * af_all[v0 + v]);
+        } else {                                                     // binary traits: minor-allele coding
+          g = int_g(w, mu[v0 + v]);
+          if ((flags[v0 + v] & 8) && !(w >> 31)) g = 2.0 - g;
+        }
+      }
       gs[v][j] = g;
     }
     __syncthreads();
@@ -102,16 +112,6 @@ __global__ void s2_int_route_kernel(S2IntArgs a) {
     r = (a.K > 0 && !a.no_robust && !a.force_robust && rare) ? 2 : 1;
   }
   a.route[v] = r;
-}
-
-// near-singular check and inverse of a symmetric 2 x 2 (SelfAdjointEigenSolver + eigenvalues().minCoeff() < numtol)
-__device__ bool int_inv2(double a11, double a12, double a22, double numtol, double* z) {
-  const double hm = 0.5 * (a11 + a22), hd = 0.5 * (a11 - a22);
-  const double lmin = hm - sqrt(hd * hd + a12 * a12);
-  if (!(lmin >= numtol)) return false;
-  const double det = a11 * a22 - a12 * a12;
-  z[0] = a22 / det; z[1] = -a12 / det; z[2] = a11 / det;
-  return true;
 }
 
 // per variant: for robust variants b = X^T G, a = X^T (E o G), the two scales, Z = (H^T H)^-1 and
@@ -280,15 +280,22 @@ __global__ void s2_int_robust_kernel(S2IntArgs a) {
 
 }  // namespace
 
+void launch_s2_int_sums(const uint32_t* dz, int64_t npad, const double* af_all, const double* mu, const int32_t* flags,
+                        int bs, const int8_t* route, int nr, const double* Fint, int nf, const uint8_t* pow2,
+                        const int4* chunks, int nchunks, double* part, double* sums, cudaStream_t s) {
+  const int bs_pad = (int)round_up(bs, kIntVT);
+  dim3 g1((unsigned)ceil_div(nf, kIntThreads), nchunks, bs_pad / kIntVT);
+  s2_int_sums_kernel<<<g1, kIntThreads, 0, s>>>(dz, npad, af_all, mu, flags, bs, route, nr, Fint, nf, pow2, chunks, bs_pad,
+                                                part);
+  const int64_t per = (int64_t)bs * nf;
+  s2_int_reduce_kernel<<<(unsigned)ceil_div(per, 256), 256, 0, s>>>(part, nchunks, (int64_t)bs_pad * nf, route, bs, nf, nr,
+                                                                    sums);
+}
+
 void launch_s2_interaction(const S2IntArgs& a, const uint8_t* pow2, double* part, cudaStream_t s) {
-  const int bs_pad = (int)round_up(a.bs, kIntVT);
   s2_int_route_kernel<<<(unsigned)ceil_div(a.bs, 128), 128, 0, s>>>(a);
-  dim3 g1((unsigned)ceil_div(a.nf, kIntThreads), a.nchunks, bs_pad / kIntVT);
-  s2_int_sums_kernel<<<g1, kIntThreads, 0, s>>>(a.dz, a.npad, a.af_all, a.bs, a.route, a.nr, a.Fint, a.nf, pow2, a.chunks,
-                                                bs_pad, part);
-  const int64_t per = (int64_t)a.bs * a.nf;
-  s2_int_reduce_kernel<<<(unsigned)ceil_div(per, 256), 256, 0, s>>>(part, a.nchunks, (int64_t)bs_pad * a.nf, a.route, a.bs,
-                                                                    a.nf, a.nr, a.sums);
+  launch_s2_int_sums(a.dz, a.npad, a.af_all, nullptr, nullptr, a.bs, a.route, a.nr, a.Fint, a.nf, pow2, a.chunks, a.nchunks,
+                     part, a.sums, s);
   s2_int_finish_kernel<<<(unsigned)ceil_div(a.bs, 64), 64, 0, s>>>(a);
   s2_int_meat_kernel<<<dim3(a.nchunks, a.bs, (unsigned)ceil_div(a.P, kIntTG)), 256, 0, s>>>(a);
   s2_int_robust_kernel<<<(unsigned)ceil_div(a.bs * a.P, 128), 128, 0, s>>>(a);
