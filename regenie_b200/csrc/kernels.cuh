@@ -295,6 +295,85 @@ void launch_l1_loocv_chr_pred(const double* W, int64_t ldw, int B, int nC, const
 void launch_l0_std_reduce_only(const double* part, int ntiles, int Qp, int Q, int P, const double* neff,
                                double* mean_invsd, cudaStream_t s);
 
+// ---- Step 2: device helpers of the per-variant kernels
+// The genotype word dz of one (variant, sample), DESIGN.md "Step-2 genotype words": d = dosage x 255 (0..510) in bits
+// 0-9, e = 4 p0 + p1 in bits 10-20 (8-bit dosages; 0 for hard calls), or the missing bit 31 alone.
+constexpr uint32_t kDzMissing = 0x80000000u;
+__device__ __forceinline__ uint32_t dz_word(uint32_t d, uint32_t e) { return d | (e << 10); }
+__device__ __forceinline__ bool dz_missing(uint32_t w) { return (w & kDzMissing) != 0u; }
+__device__ __forceinline__ uint32_t dz_d(uint32_t w) { return w & 0x3FFu; }
+__device__ __forceinline__ uint32_t dz_e(uint32_t w) { return (w >> 10) & 0x7FFu; }
+
+// The genotype value of a word has two arithmetic forms: Firth and SPA divide d by 255 (s2_sel_g), the GxE kernels
+// multiply it by 1 / 255 (int_g).  They differ by one ulp on 48 of the 511 codes (never on the hard calls 0, 255, 510),
+// so one form for both would change the results of the other on fractional dosages.
+// Both: the value in the minor-allele coding (flip: 2 - g), and mu for a missing call.
+__device__ __forceinline__ double s2_sel_g(uint32_t w, double mu, bool flip) {
+  return dz_missing(w) ? mu : (flip ? 2.0 - (double)dz_d(w) / 255.0 : (double)dz_d(w) / 255.0);
+}
+__device__ __forceinline__ double int_g(uint32_t w, double mu, bool flip = false) {
+  if (dz_missing(w)) return mu;
+  const double g = (double)dz_d(w) * (1.0 / 255.0);
+  return flip ? 2.0 - g : g;
+}
+
+constexpr double kNumtolEps = 10.0 * 2.220446049250313e-16;   // numtol_eps, src/Regenie.hpp:225
+__device__ __forceinline__ double get_pvec(double eta) {      // src/Step1_Models.cpp:1797-1804
+  if (eta > 30.0) return 1.0 / (1.0 + kNumtolEps);
+  if (eta < -30.0) return kNumtolEps / (1.0 + kNumtolEps);
+  return 1.0 - 1.0 / (exp(eta) + 1.0);
+}
+
+// Fixed-order sum of v over a CTA of kWarps warps (lanes by shuffles, then the warps in ascending order), so the totals do
+// not depend on timing; every thread receives them.  sh holds kWarps * K doubles.
+template <int kWarps, int K>
+__device__ __forceinline__ void cta_sum(double (&v)[K], double* sh) {
+#pragma unroll
+  for (int k = 0; k < K; ++k)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __syncthreads();
+  if (lane == 0)
+#pragma unroll
+    for (int k = 0; k < K; ++k) sh[warp * K + k] = v[k];
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double s = 0.0;
+    for (int w = 0; w < kWarps; ++w) s += sh[w * K + k];
+    v[k] = s;
+  }
+}
+
+// N, MAC and AF of column c of a variant's sums (compute_mac / compute_aaf_info, src/Geno.cpp:3077-3148), and INFO when
+// info is not null.  S1, S2, Se are in units of 1 / k (k = 1: dosage units), Sm counts the missing calls and n is the
+// column's total over the analysed samples.  Non-PAR chrX (cm >= 0, the column of the same samples' males, *n_male
+// their total): males are coded 0/2 but count half towards the allele count (src/Geno.cpp:2447-2462).
+struct S2Count { double ns, mac; };
+__device__ __forceinline__ S2Count s2_count(const double* S1, const double* S2, const double* Sm, const double* Se, int c,
+                                            double n, int cm, const double* n_male, double k, int32_t* ns_out, double* mac_out,
+                                            double* af_out, double* info) {
+  const double ns = n - Sm[c];
+  const double tp = S1[c] * k;
+  double mac;
+  if (cm >= 0) {
+    const double macr = tp - 0.5 * S1[cm] * k;
+    mac = fmin(macr, 2.0 * ns - (*n_male - Sm[cm]) - macr);
+  } else {
+    mac = fmin(tp, 2.0 * ns - tp);
+  }
+  *ns_out = (int)ns;
+  *mac_out = mac;
+  const double af = tp / (2.0 * ns);
+  *af_out = af;
+  if (info) {                                                        // 1 - sum(4 p0 + p1 - g^2) / (2 n af (1 - af))
+    const double num = Se[c] * k - S2[c] * (k * k);
+    *info = (af == 0.0 || af == 1.0) ? 1.0 : 1.0 - num / (2.0 * ns * af * (1.0 - af));
+  }
+  return {ns, mac};
+}
+
 // ---- s2_kernels.cu
 struct S2FinalizeArgs {
   int bs, C, P, dp, strict;
@@ -348,45 +427,71 @@ void launch_s2_bt_finalize(const S2BtFinalizeArgs& a, cudaStream_t s);
 // integer-unit sums [rows][4][dp] -> dosage-unit [rows][3][dp] (S1, S2, Sm) + [rows][dp] (Se)
 void launch_dosage_scale(const double* sums4, int rows_p, int dp, double* sums3, double* se, cudaStream_t s);
 
-// ---- s2_firth.cu
-struct FirthArgs {
-  int n_sel, C, P, dp, niter;
-  double tol, maxstep;
-  int64_t npad;
-  const int32_t *sel_var, *sel_trait;
-  const uint32_t* dz;
-  const double* F;
-  const double *w, *gs, *xw, *off;   // [P][Npad], xw [P][C][Npad]
-  const int8_t* ym;                  // [P][Npad] 0 masked, 1 control, 2 case
-  const double* xtwg;                // [bs][P][C]
-  const double* mu;                  // [bs] imputed mean (after flip)
-  const double* mac;                 // [bs][P]
-  const int32_t* flags;              // [bs]
-  double* gvec;                      // [n_sel][Npad] scratch
-  int8_t* cflag;                     // [n_sel][Npad] scratch
-  double *beta, *se, *lrt;
-  int32_t* status;
-};
-void launch_s2_firth(const FirthArgs& a, cudaStream_t s);
-
-// ---- s2_spa.cu
-struct SpaArgs {
+// ---- s2_firth.cu / s2_spa.cu: one CTA per selected (variant, trait) of the resident binary-trait block
+struct S2SelArgs {
   int n_sel, C, P, dp, niter;
   double tol;
   int64_t npad;
   const int32_t *sel_var, *sel_trait;
   const uint32_t* dz;
-  const double* F;
-  const double *w, *gs, *xw, *phat;  // [P][Npad], xw [P][C][Npad]
-  const int8_t* ym;
+  const double* F;                   // [Npad][dp] binary-trait feature rows (column 0: in the analysis)
+  const double *w, *gs, *xw;         // [P][Npad], xw [P][C][Npad]
+  const int8_t* ym;                  // [P][Npad] 0 masked, 1 control, 2 case
   const double* xtwg;                // [bs][P][C]
-  const double* mu;                  // [bs]
-  const double *stat, *den;          // [bs][P] score statistic and its denominator G'WG
-  const int32_t* flags;
+  const double* mu;                  // [bs] imputed mean (after flip)
+  const int32_t* flags;              // [bs]
   double* gvec;                      // [n_sel][Npad] scratch
-  int8_t* cflag;                     // [n_sel][Npad] scratch (active-set flags)
+  int8_t* cflag;                     // [n_sel][Npad] scratch (carrier / active-set flags)
+  int32_t* status;                   // [n_sel]
+};
+// What both kernels read first for selection blockIdx.x: the pair's rows, the variant's coding and X^T W g, which goes
+// to the kernel's own array v (a member array would put the whole struct in local memory)
+struct S2Sel {
+  int C;
+  int64_t npad;
+  int i, ph;                         // variant, trait
+  bool flip, sparse;                 // flags bits 3 and 2
+  double mu;
+  const uint32_t* drow;
+  const double *w, *gs, *xw;
+  const int8_t* ym;
+  double* gv;
+  int8_t* cf;
+  double* v;                         // [C]
+  __device__ __forceinline__ S2Sel(const S2SelArgs& a, double (&vr)[kMaxCov]) : C(a.C), npad(a.npad), v(vr) {
+    const int sel = blockIdx.x;
+    i = a.sel_var[sel]; ph = a.sel_trait[sel];
+    const int flags = a.flags[i];
+    flip = flags & 8; sparse = flags & 4;
+    mu = a.mu[i];
+    drow = a.dz + (int64_t)i * a.npad;
+    w = a.w + (int64_t)ph * a.npad; gs = a.gs + (int64_t)ph * a.npad; xw = a.xw + (int64_t)ph * a.C * a.npad;
+    ym = a.ym + (int64_t)ph * a.npad;
+    gv = a.gvec + (int64_t)sel * a.npad; cf = a.cflag + (int64_t)sel * a.npad;
+    for (int c = 0; c < a.C; ++c) v[c] = a.xtwg[((int64_t)i * a.P + ph) * a.C + c];
+  }
+  // the genotype g of sample t (0 outside the analysis) and its residual r = g w - sum_c xw_c v_c
+  __device__ __forceinline__ double gres(const S2SelArgs& a, int64_t t, double& g) const {
+    g = s2_sel_g(drow[t], mu, flip);
+    if (a.F[t * a.dp] == 0.0) g = 0.0;
+    double r = g * w[t];
+    for (int c = 0; c < C; ++c) r -= xw[(int64_t)c * npad + t] * v[c];
+    return r;
+  }
+};
+
+struct FirthArgs : S2SelArgs {
+  double maxstep;
+  const double* off;                 // [P][Npad]
+  const double* mac;                 // [bs][P]
+  double *beta, *se, *lrt;
+};
+void launch_s2_firth(const FirthArgs& a, cudaStream_t s);
+
+struct SpaArgs : S2SelArgs {
+  const double* phat;                // [P][Npad]
+  const double *stat, *den;          // [bs][P] score statistic and its denominator G'WG
   double* pval;                      // [n_sel] sum of the two tail probabilities
-  int32_t* status;
 };
 void launch_s2_spa(const SpaArgs& a, cudaStream_t s);
 

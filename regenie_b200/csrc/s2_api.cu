@@ -431,45 +431,52 @@ static void s2_block_bed_bt(rg_ctx* h, const uint8_t* packed, int64_t row_stride
   s2_copy_out(h, s2, bs, out, nullptr, nullptr, s);
 }
 
-// Firth and SPA on (variant, trait) selections of the block left resident by a binary-trait route, kSelBatch at a time.
-// `batch(s2, o, nb)` fills its kernel's arguments for selections o .. o + nb (uploaded to sel.idx), launches the kernel and
-// queues the copies of its results; the batch is complete when this returns to the loop.
-constexpr int kSelBatch = 256;
+// The selection loop of rg_s2_firth, rg_s2_spa and rg_s2_interaction_firth on the resident binary-trait block: batches of
+// len (variant, trait) selections, whose indices go up to idx[0, len) and idx[len, 2 len).  `batch(s2, o, nb)` launches
+// its kernels for selections o .. o + nb and queues the copies of their results; the batch is complete when this returns
+// to the loop.
 template <typename Batch>
-static void s2_selections(rg_ctx* h, const char* call, int n_sel, const int32_t* var_idx, const int32_t* trait_idx,
-                          Batch&& batch) {
+static void s2_selections(rg_ctx* h, const char* call, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, int len,
+                          DevBuf<int32_t>& idx, Batch&& batch) {
   Step2State& s2 = step2(h);
   RG_CHECK(s2.block.kind == S2Block::bt, std::string(call) + " needs a resident binary-trait block");
   RG_CUDA(cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   for (int k = 0; k < n_sel; ++k)
     RG_CHECK(var_idx[k] >= 0 && var_idx[k] < s2.block.bs && trait_idx[k] >= 0 && trait_idx[k] < h->P, "selection out of range");
-  s2.sel.gvec.alloc((size_t)kSelBatch * h->Npad); s2.sel.cflag.alloc((size_t)kSelBatch * h->Npad);
-  s2.sel.idx.alloc(2 * kSelBatch); s2.sel.status.alloc(kSelBatch); s2.sel.out.alloc(3 * kSelBatch);
-  for (int o = 0; o < n_sel; o += kSelBatch) {
-    const int nb = std::min(kSelBatch, n_sel - o);
-    RG_CUDA(cudaMemcpyAsync(s2.sel.idx.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
-    RG_CUDA(cudaMemcpyAsync(s2.sel.idx.p + kSelBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+  idx.alloc(2 * len);
+  for (int o = 0; o < n_sel; o += len) {
+    const int nb = std::min(len, n_sel - o);
+    RG_CUDA(cudaMemcpyAsync(idx.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+    RG_CUDA(cudaMemcpyAsync(idx.p + len, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
     batch(s2, o, nb);
-    h->launches += 1;
     RG_CUDA(cudaStreamSynchronize(s));
   }
 }
 
+// Firth and SPA: kSelBatch selections at a time.  The arguments both kernels read for a batch of nb, with its scratch and
+// result buffers.
+constexpr int kSelBatch = 256;
+static void s2_sel_args(rg_ctx* h, Step2State& s2, int nb, int niter, double tol, S2SelArgs& a) {
+  s2.sel.gvec.alloc((size_t)kSelBatch * h->Npad); s2.sel.cflag.alloc((size_t)kSelBatch * h->Npad);
+  s2.sel.status.alloc(kSelBatch); s2.sel.out.alloc(3 * kSelBatch);
+  a.n_sel = nb; a.C = h->C; a.P = h->P; a.dp = s2.bt.dp; a.niter = niter; a.tol = tol;
+  a.npad = h->Npad; a.sel_var = s2.sel.idx.p; a.sel_trait = s2.sel.idx.p + kSelBatch;
+  a.dz = s2.in.dz.p; a.F = s2.bt.F.p; a.w = s2.bt.w.p; a.gs = s2.bt.gs.p; a.xw = s2.bt.xw.p; a.ym = s2.bt.ym.p;
+  a.xtwg = s2.out.xtwg.p; a.mu = s2.out.mu.p; a.flags = s2_out_at(h, s2.out.d.p, s2.out.i.p).flags;
+  a.gvec = s2.sel.gvec.p; a.cflag = s2.sel.cflag.p; a.status = s2.sel.status.p;
+}
+
 static void s2_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* beta, double* se,
                      double* lrt, int32_t* status) {
-  s2_selections(h, "rg_s2_firth", n_sel, var_idx, trait_idx, [&](Step2State& s2, int o, int nb) {
+  s2_selections(h, "rg_s2_firth", n_sel, var_idx, trait_idx, kSelBatch, step2(h).sel.idx, [&](Step2State& s2, int o, int nb) {
     cudaStream_t s = h->stream;
-    const rg_s2_out d = s2_out_at(h, s2.out.d.p, s2.out.i.p);
     FirthArgs a;
-    a.n_sel = nb; a.C = h->C; a.P = h->P; a.dp = s2.bt.dp; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;
-    a.npad = h->Npad; a.sel_var = s2.sel.idx.p; a.sel_trait = s2.sel.idx.p + kSelBatch;
-    a.dz = s2.in.dz.p; a.F = s2.bt.F.p; a.w = s2.bt.w.p; a.gs = s2.bt.gs.p; a.xw = s2.bt.xw.p; a.off = s2.bt.off.p;
-    a.ym = s2.bt.ym.p; a.xtwg = s2.out.xtwg.p; a.mu = s2.out.mu.p; a.mac = d.mac; a.flags = d.flags;
-    a.gvec = s2.sel.gvec.p; a.cflag = s2.sel.cflag.p;
+    s2_sel_args(h, s2, nb, 250, 2.5e-4, a);
+    a.maxstep = 5.0; a.off = s2.bt.off.p; a.mac = s2_out_at(h, s2.out.d.p, s2.out.i.p).mac;
     a.beta = s2.sel.out.p; a.se = s2.sel.out.p + kSelBatch; a.lrt = s2.sel.out.p + 2 * kSelBatch;
-    a.status = s2.sel.status.p;
     launch_s2_firth(a, s);
+    h->launches += 1;
     RG_CUDA(cudaMemcpyAsync(beta + o, a.beta, nb * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(se + o, a.se, nb * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(lrt + o, a.lrt, nb * 8, cudaMemcpyDeviceToHost, s));
@@ -478,16 +485,14 @@ static void s2_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t
 }
 
 static void s2_spa(rg_ctx* h, int n_sel, const int32_t* var_idx, const int32_t* trait_idx, double* pval, int32_t* status) {
-  s2_selections(h, "rg_s2_spa", n_sel, var_idx, trait_idx, [&](Step2State& s2, int o, int nb) {
+  s2_selections(h, "rg_s2_spa", n_sel, var_idx, trait_idx, kSelBatch, step2(h).sel.idx, [&](Step2State& s2, int o, int nb) {
     cudaStream_t s = h->stream;
-    const rg_s2_out d = s2_out_at(h, s2.out.d.p, s2.out.i.p);
     SpaArgs a;
-    a.n_sel = nb; a.C = h->C; a.P = h->P; a.dp = s2.bt.dp; a.niter = 1000; a.tol = 1.220703125e-4;   // eps^(1/4), src/Regenie.hpp:330
-    a.npad = h->Npad; a.sel_var = s2.sel.idx.p; a.sel_trait = s2.sel.idx.p + kSelBatch;
-    a.dz = s2.in.dz.p; a.F = s2.bt.F.p; a.w = s2.bt.w.p; a.gs = s2.bt.gs.p; a.xw = s2.bt.xw.p; a.phat = s2.bt.phat.p;
-    a.ym = s2.bt.ym.p; a.xtwg = s2.out.xtwg.p; a.mu = s2.out.mu.p; a.stat = d.stat; a.den = s2.out.den.p; a.flags = d.flags;
-    a.gvec = s2.sel.gvec.p; a.cflag = s2.sel.cflag.p; a.pval = s2.sel.out.p; a.status = s2.sel.status.p;
+    s2_sel_args(h, s2, nb, 1000, 1.220703125e-4, a);                  // eps^(1/4), src/Regenie.hpp:330
+    a.phat = s2.bt.phat.p; a.stat = s2_out_at(h, s2.out.d.p, s2.out.i.p).stat; a.den = s2.out.den.p;
+    a.pval = s2.sel.out.p;
     launch_s2_spa(a, s);
+    h->launches += 1;
     RG_CUDA(cudaMemcpyAsync(pval + o, a.pval, nb * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(status + o, a.status, nb * 4, cudaMemcpyDeviceToHost, s));
   });
@@ -681,29 +686,20 @@ static void s2_interaction_firth(rg_ctx* h, int n_sel, const int32_t* var_idx, c
   RG_CHECK(s2.block.kind == S2Block::bt && g.set && g.wald_serial == s2.block_serial,
            "rg_s2_interaction_firth needs rg_s2_interaction_bt on the resident binary-trait block");
   RG_CHECK(s2.bt.firth, "rg_s2_interaction_firth needs the null-Firth offsets (rg_s2_bt_chr.firth_offset)");
-  for (int k = 0; k < n_sel; ++k)
-    RG_CHECK(var_idx[k] >= 0 && var_idx[k] < s2.block.bs && trait_idx[k] >= 0 && trait_idx[k] < h->P, "selection out of range");
-  RG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t s = h->stream;
-  S2IntBtArgs a = s2_int_bt_args(h, s2);
-  a.off = s2.bt.off.p; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;    // niter_max_firth, numtol_firth, maxstep
-  g.sel.alloc(2 * kIntBtBatch + kIntBtBatch);
-  g.out.alloc(7 * kIntBtBatch);
-  a.sel_var = g.sel.p; a.sel_trait = g.sel.p + kIntBtBatch; a.f_status = g.sel.p + 2 * kIntBtBatch;
-  a.f_coef = g.out.p; a.f_se = g.out.p + 2 * kIntBtBatch; a.f_lrt = g.out.p + 4 * kIntBtBatch;
-  for (int o = 0; o < n_sel; o += kIntBtBatch) {
-    const int nb = std::min(kIntBtBatch, n_sel - o);
-    a.nb = nb;
-    RG_CUDA(cudaMemcpyAsync(g.sel.p, var_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
-    RG_CUDA(cudaMemcpyAsync(g.sel.p + kIntBtBatch, trait_idx + o, nb * 4, cudaMemcpyHostToDevice, s));
+  s2_selections(h, "rg_s2_interaction_firth", n_sel, var_idx, trait_idx, kIntBtBatch, g.sel, [&](Step2State&, int o, int nb) {
+    cudaStream_t s = h->stream;
+    S2IntBtArgs a = s2_int_bt_args(h, s2);
+    a.off = s2.bt.off.p; a.niter = 250; a.tol = 2.5e-4; a.maxstep = 5.0;    // niter_max_firth, numtol_firth, maxstep
+    g.out.alloc(7 * kIntBtBatch); g.status.alloc(kIntBtBatch);
+    a.sel_var = g.sel.p; a.sel_trait = g.sel.p + kIntBtBatch; a.nb = nb;
+    a.f_coef = g.out.p; a.f_se = g.out.p + 2 * kIntBtBatch; a.f_lrt = g.out.p + 4 * kIntBtBatch; a.f_status = g.status.p;
     launch_s2_int_bt_firth(a, s);
     h->launches += 2;
     RG_CUDA(cudaMemcpyAsync(coef + 2 * o, a.f_coef, nb * 2 * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(se + 2 * o, a.f_se, nb * 2 * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(lrt + 3 * o, a.f_lrt, nb * 3 * 8, cudaMemcpyDeviceToHost, s));
     RG_CUDA(cudaMemcpyAsync(status + o, a.f_status, nb * 4, cudaMemcpyDeviceToHost, s));
-    RG_CUDA(cudaStreamSynchronize(s));
-  }
+  });
 }
 
 extern "C" {

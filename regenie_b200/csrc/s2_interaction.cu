@@ -24,10 +24,6 @@ constexpr int kIntVT = 16;       // variants per CTA of the sums kernel
 constexpr int kIntSub = 256;     // samples staged in shared memory at a time
 constexpr int kIntThreads = 128;
 
-__device__ __forceinline__ double int_g(uint32_t w, double mu) {
-  return (w >> 31) ? mu : (double)(w & 1023u) * (1.0 / 255.0);
-}
-
 // the feature columns a variant's route reads: robust columns [0, nr), HLM columns [nr, nf)
 __device__ __forceinline__ bool int_needs(int8_t route, int f, int nr) { return route == (f < nr ? 1 : 2); }
 
@@ -61,12 +57,8 @@ __global__ void __launch_bounds__(kIntThreads) s2_int_sums_kernel(const uint32_t
       double g = 0.0;
       if (v0 + v < bs && route[v0 + v] > 0 && j < len) {
         const uint32_t w = dz[(int64_t)(v0 + v) * npad + ch.x + o + j];
-        if (!mu) {
-          g = int_g(w, 2.0 * af_all[v0 + v]);
-        } else {                                                     // binary traits: minor-allele coding
-          g = int_g(w, mu[v0 + v]);
-          if ((flags[v0 + v] & 8) && !(w >> 31)) g = 2.0 - g;
-        }
+        if (!mu) g = int_g(w, 2.0 * af_all[v0 + v]);
+        else g = int_g(w, mu[v0 + v], flags[v0 + v] & 8);            // binary traits: minor-allele coding
       }
       gs[v][j] = g;
     }

@@ -10,57 +10,27 @@ namespace rg {
 
 constexpr int kSpaThreads = 512;
 
-template <int K>
-__device__ __forceinline__ void spa_block_sum(double (&v)[K], double* sh) {
-#pragma unroll
-  for (int k = 0; k < K; ++k)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0)
-#pragma unroll
-    for (int k = 0; k < K; ++k) sh[warp * K + k] = v[k];
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    double s = 0.0;
-    for (int wq = 0; wq < kSpaThreads / 32; ++wq) s += sh[wq * K + k];
-    v[k] = s;
-  }
-}
-
 __global__ void __launch_bounds__(kSpaThreads)
 s2_spa_kernel(SpaArgs a) {
   __shared__ double sh[(kSpaThreads / 32) * 6];
-  const int sel = blockIdx.x;
-  const int i = a.sel_var[sel], ph = a.sel_trait[sel];
-  const int C = a.C, P = a.P;
-  const int64_t npad = a.npad;
-  const uint32_t* drow = a.dz + (int64_t)i * npad;
-  const double* w = a.w + (int64_t)ph * npad;
-  const double* gsq = a.gs + (int64_t)ph * npad;
-  const double* phat = a.phat + (int64_t)ph * npad;
-  const double* xw = a.xw + (int64_t)ph * C * npad;
-  const int8_t* ym = a.ym + (int64_t)ph * npad;
-  double* gv = a.gvec + (int64_t)sel * npad;
-  int8_t* inS = a.cflag + (int64_t)sel * npad;
-  const int flags = a.flags[i];
-  const bool flip = flags & 8, fast = flags & 4;
-  const double mu = a.mu[i];
-  const double stat = a.stat[(int64_t)i * P + ph], denum = a.den[(int64_t)i * P + ph];
-  const double c = sqrt(denum);
   double v[kMaxCov];
-  for (int cc = 0; cc < C; ++cc) v[cc] = a.xtwg[((int64_t)i * P + ph) * C + cc];
+  const S2Sel sp(a, v);
+  const int64_t npad = a.npad;
+  const double* gsq = sp.gs;
+  const double* phat = a.phat + (int64_t)sp.ph * npad;
+  const int8_t* ym = sp.ym;
+  double* gv = sp.gv;
+  int8_t* inS = sp.cf;
+  const bool fast = sp.sparse;
+  const int64_t ip = (int64_t)sp.i * a.P + sp.ph;
+  const double stat = a.stat[ip], denum = a.den[ip];
+  const double c = sqrt(denum);
 
   // ---- Gmod = Gres / Gamma^{1/2} on the masked samples, the active set, and the constants a, b, d, K' limits
   double s5[5] = {0, 0, 0, 0, 0};      // a, neg, pos, sum_S gres^2, sum_S gmu
   for (int64_t t = threadIdx.x; t < npad; t += kSpaThreads) {
-    const uint32_t dv = drow[t];
-    double g = (dv & 0x80000000u) ? mu : (flip ? 2.0 - (double)(dv & 0x3FFu) / 255.0 : (double)(dv & 0x3FFu) / 255.0);
-    if (a.F[t * a.dp] == 0.0) g = 0.0;
-    double r = g * w[t];
-    for (int cc = 0; cc < C; ++cc) r -= xw[(int64_t)cc * npad + t] * v[cc];
+    double g;
+    const double r = sp.gres(a, t, g);
     const bool m = ym[t] != 0;
     const double gm = m ? r / gsq[t] : 0.0;
     gv[t] = gm;
@@ -72,7 +42,7 @@ s2_spa_kernel(SpaArgs a) {
     s5[2] += fmax(gm, 0.0);
     if (s_in && fast) { s5[3] += r * r; s5[4] += gmu; }
   }
-  spa_block_sum<5>(s5, sh);
+  cta_sum<kSpaThreads / 32>(s5, sh);
   const double va = s5[0], vb = denum - s5[3], vd = s5[4];
   int status = 0;
   double ptot = 0.0;
@@ -94,7 +64,7 @@ s2_spa_kernel(SpaArgs a) {
       s[2] += (gm * gm * gsv * gsv / (c * c) * e) / (den * den);
       if (want_k) s[0] += log(1.0 - p + p * exp(tc * gm));
     }
-    spa_block_sum<4>(s, sh);
+    cta_sum<kSpaThreads / 32>(s, sh);
     if (fast) {
       k0 = s[0] - t * vd / c + t * t / 2.0 / denum * vb;
       k1 = s[1] - vd / c + t / denum * vb;
@@ -151,8 +121,8 @@ s2_spa_kernel(SpaArgs a) {
   }
   if (status == 0 && !(ptot <= 1.0)) status = 5;
   if (threadIdx.x == 0) {
-    a.pval[sel] = ptot;
-    a.status[sel] = status | (fast ? 256 : 0);
+    a.pval[blockIdx.x] = ptot;
+    a.status[blockIdx.x] = status | (fast ? 256 : 0);
   }
 }
 
