@@ -7,6 +7,10 @@
 //   rgb200_hostprobe bgen-probs FILE FIRST N OUT            raw probability + ploidy bytes of N variants
 //   rgb200_hostprobe bgen-info FILE [--ref-first]           variant-level INFO (info1) of every variant
 //   rgb200_hostprobe rows (--bed|--pgen) PREFIX OUT          every variant as PLINK 1 2-bit rows
+//   rgb200_hostprobe counts CLASSES OUT (--bed PREFIX|--bgen FILE) [--ref-first] [--remove F]
+//                    genotype counts of every variant (host/counts.hpp), int64 [variants][T][6].  CLASSES: a line
+//                    "T binary male non_par", then cls [T][kept samples], male [kept samples] if male = 1 and
+//                    non_par [variants] if non_par = 1, one byte each
 //   rgb200_hostprobe prep OUT (--bed|--pgen|--bgen) X --phenoFile F [--covarFile F] [--bt] [--step2] [--strict]
 //                    [--remove F] [--keep F] [--apply-rint] [--catCovarList a,b] [--phenoColList a,b] [--covarColList a,b]
 //                    [--cv K] [--bsize B] [--null-eta]
@@ -27,6 +31,7 @@
 #include "../../csrc/pgen_core.h"
 #include "../bgen.hpp"
 #include "../bt_null.hpp"
+#include "../counts.hpp"
 #include "../data.hpp"
 #include "../output.hpp"
 #include "../pgen.hpp"
@@ -106,6 +111,63 @@ int cmd_rows(char** argv) {
   std::ofstream f(argv[4], std::ios::binary);
   f.write(reinterpret_cast<const char*>(rows.data()), (std::streamsize)rows.size());
   std::cout << g.snps.size() << " " << g.row_stride << " " << g.keys.size() << "\n";
+  return 0;
+}
+
+// the hard-call counter on the rows of a .bed, or the dosage counter on the probability pairs of a .bgen
+int cmd_counts(int argc, char** argv) {
+  std::string bed, bgen, remove;
+  bool ref_first = false;
+  for (int i = 4; i < argc; ++i) {
+    const std::string a = argv[i];
+    if (a == "--bed") bed = argv[++i];
+    else if (a == "--bgen") bgen = argv[++i];
+    else if (a == "--remove") remove = argv[++i];
+    else if (a == "--ref-first") ref_first = true;
+    else throw Fail("probe: unknown option " + a);
+  }
+  BedFile g;
+  BgenFile gg;
+  const auto rem = read_id_list(remove, 2);
+  if (!bgen.empty()) gg.open(bgen, "", ref_first, {}, {}, rem, {}, {}, "", true);
+  else g.open(bed, ref_first, {}, {}, rem, {});
+  const std::vector<int32_t>& sidx = bgen.empty() ? g.sample_idx : gg.sample_idx;
+  const size_t M = bgen.empty() ? g.snps.size() : gg.snps.size(), N = sidx.size();
+  const size_t n_file = bgen.empty() ? g.keys_file.size() : gg.n_file;
+  ClassTable ct;
+  int binary = 0, has_male = 0, has_np = 0;
+  std::ifstream f(argv[2], std::ios::binary);
+  f >> ct.T >> binary >> has_male >> has_np;
+  f.get();
+  ct.binary = binary != 0;
+  auto bytes = [&](std::vector<uint8_t>& v, size_t n) {
+    v.resize(n);
+    f.read(reinterpret_cast<char*>(v.data()), (std::streamsize)n);
+  };
+  std::vector<uint8_t> non_par;
+  bytes(ct.cls, (size_t)ct.T * N);
+  if (has_male) bytes(ct.male, N);
+  if (has_np) bytes(non_par, M);
+  if (!f) throw Fail("probe: class file too short");
+  const uint8_t* np = has_np ? non_par.data() : nullptr;
+  std::vector<long> out(M * ct.T * 6);
+  if (!bgen.empty()) {
+    std::vector<uint8_t> probs(M * n_file * 2), pm(M * n_file);
+    gg.read_block(0, M, probs.data(), pm.data(), 4);
+    dosage_counts(ct, ref_first, n_file, sidx, probs.data(), pm.data(), M, np, out.data(), 4);
+  } else {
+    std::vector<uint8_t> rows(M * g.row_stride);
+    g.read_rows(0, M, rows.data());
+    HardCallCounts hc;
+    hc.init(ct, ref_first, n_file, sidx);
+    hc.count(rows.data(), g.row_stride, (int)M, np, out.data(), 4);
+  }
+  std::ofstream o(argv[3], std::ios::binary);
+  for (long x : out) {
+    const int64_t v = x;
+    o.write(reinterpret_cast<const char*>(&v), sizeof(v));
+  }
+  std::cout << M << " " << N << " " << n_file << "\n";
   return 0;
 }
 
@@ -376,6 +438,7 @@ int main(int argc, char** argv) {
     if (c == "bgen-info" && argc >= 3) return cmd_bgen_info(argc, argv);
     if (c == "rows" && argc == 5) return cmd_rows(argv);
     if (c == "pgen-rows" && argc == 5) return cmd_pgen_rows(argv);
+    if (c == "counts" && argc >= 6) return cmd_counts(argc, argv);
     if (c == "prep" && argc >= 3) return cmd_prep(argc, argv);
     if (c == "cat" && argc == 3) return cmd_cat(argv);
     if (c == "pred-file" && argc >= 4) return cmd_pred_file(argc, argv);

@@ -676,7 +676,7 @@ def check_htp_bgen_chrx(run, read, tmp_path, golden_dir):
 def check_htp_bgen(run, read, tmp_path, golden_dir, bt=False):
     """--htp on dosages: the thresholded genotype counts of each trait's samples (cases / controls for a binary trait) against
     oracle.step2.genocounts on the float dosages (update_genocounts, src/Geno.cpp:2986-3018), INFO= in the Info column, same
-    variants as the native file.  The driver forms the counts on the host from the inflated bytes (BgenFile::trait_counts)."""
+    variants as the native file.  The driver forms the counts on the host from the inflated bytes (host/counts.cpp)."""
     from oracle import bgen as obgen, prep, step2
     d = golden_dir
     keys = ["_".join(l.split()[:2]) for l in open(d + "/example.fam")]

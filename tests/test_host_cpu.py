@@ -11,6 +11,7 @@ dumps with the numpy restatement in oracle/ and with the reference's fixtures:
   * .loco / .prs writers and readers, plain and --gz                                  (src/Data.cpp:1795-1982)
   * .regenie rows + LOG10P vs scipy                                                   (src/Step2_Models.cpp:2502-2540)
   * .regenie.ids                                                                      (src/Pheno.cpp:1538-1576)
+  * --no-split / --htp genotype counts vs oracle/plink.py and oracle/bgen.py           (update_genocounts src/Geno.cpp:2986-3018)
 """
 import gzip
 import math
@@ -546,3 +547,93 @@ def test_variant_level_info_matches_the_oracle_formula(tmp_path, ref_first):
         lo = min(lo, want)
     assert lo < 0.8                                                  # the file really has low-INFO variants
     assert probe("inflate-bgen", f, "window").stdout.splitlines()[-1].split()[:4] == ["variants", str(M), "bad", "0"]
+
+
+# ------------------------------------------------------------------------------------------- genotype counts (--no-split, --htp)
+def _counts_fileset(tmp_path, kind):
+    """239 samples (a partial last word of 32 and a partial last byte), 5 % missing calls, a remove list of 17 samples, a
+    male vector and non-PAR flags.  On the .bgen every third male call of a non-PAR variant is set to dosage exactly 1
+    (p1 + 2 hom = 255, for either allele order) or to a pair with p0 + p1 = 255."""
+    import helpers
+    from regenie_b200 import synth
+    M, N = 48, 239
+    rng = np.random.default_rng(17)
+    male = rng.random(N) < 0.5
+    non_par = rng.random(M) < 0.5
+    removed = np.sort(rng.choice(N, 17, replace=False))
+    pfx = str(tmp_path / "c")
+    if kind == "bed":
+        g = synth.genotypes(N, M, seed=17, miss=0.05)
+        with open(pfx + ".bed", "wb") as fh:
+            fh.write(b"\x6c\x1b\x01" + synth.pack_bed(g).tobytes())
+        with open(pfx + ".bim", "w") as fh:
+            fh.write("".join("1 rs%d 0 %d A G\n" % (v, 1000 + v) for v in range(M)))
+        with open(pfx + ".fam", "w") as fh:
+            fh.write("".join("F%d I%d 0 0 1 -9\n" % (s, s) for s in range(N)))
+        ids = ["F%d I%d" % (s, s) for s in removed]
+        bim = plink.read_bim(pfx + ".bim")
+        raw = plink.read_bed_rows(pfx + ".bed", N, bim.offset)
+        geno = lambda rf: plink.decode_bed(raw, N, ref_first=rf)
+    else:
+        probs, miss = helpers.synthetic_dosage_probs(M, N, seed=17, miss_rate=0.05)
+        one = [(p0, 255 - 2 * p0) for p0 in range(128)]                                   # ref-last dosage 1
+        one += [(x, 2 * x - 255) for x in range(128, 256)]                                # --ref-first dosage 1
+        one += [(p0, 255 - p0) for p0 in range(0, 256, 5)]                                # p0 + p1 = 255
+        vs, ss = np.nonzero(non_par[:, None] & male[None, :])
+        for k, (v, s) in enumerate(zip(vs[::3], ss[::3])):
+            probs[v, s] = one[k % len(one)]
+        f = pfx + ".bgen"
+        helpers.write_bgen(f, probs, miss, [1] * M, range(1, M + 1), ["v%d" % v for v in range(M)])
+        ids = ["s%d s%d" % (s, s) for s in removed]
+        geno = lambda rf: np.stack([obgen.dosage(p0, p1, m, rf)[0] for *_, p0, p1, m in obgen.Bgen(f).variants()])
+    with open(pfx + ".remove", "w") as fh:
+        fh.write("\n".join(ids) + "\n")
+    kept = np.setdiff1d(np.arange(N), removed)
+    return (["--" + kind, pfx if kind == "bed" else pfx + ".bgen", "--remove", pfx + ".remove"], geno, kept, male[kept],
+            non_par, N)
+
+
+@pytest.mark.parametrize("ref_first", [False, True])
+@pytest.mark.parametrize("cfg", ["nosplit", "qt", "bt"])
+@pytest.mark.parametrize("kind", ["bed", "bgen"])
+def test_genotype_counts_match_numpy(tmp_path, kind, cfg, ref_first):
+    """host/counts.cpp: the hard-call counter on the 2-bit rows and the dosage counter on the probability pairs against
+    oracle/plink.decode_bed and oracle/bgen.dosage.  --no-split's table: the analysed samples as one column, no male rule;
+    --htp's: one column per trait, cases and controls apart for a binary trait, the male rule on non-PAR variants (a male
+    call with g >= 1 is alt, any other male call ref; update_genocounts, src/Geno.cpp:2986-3018)."""
+    args, geno, kept, male, non_par, n_file = _counts_fileset(tmp_path, kind)
+    M, N = len(non_par), len(kept)
+    assert n_file % 32 != 0 and N < n_file
+    rng = np.random.default_rng(3)
+    T, binary, rule = {"nosplit": (1, False, False), "qt": (2, False, True), "bt": (3, True, True)}[cfg]
+    cls = rng.integers(0, 3 if binary else 2, (T, N)).astype(np.uint8)
+    with open(tmp_path / "cls.bin", "wb") as fh:
+        fh.write(b"%d %d %d %d\n" % (T, binary, rule, rule))
+        fh.write(cls.tobytes() + (male.astype(np.uint8).tobytes() + non_par.astype(np.uint8).tobytes() if rule else b""))
+    out = probe("counts", tmp_path / "cls.bin", tmp_path / "out.bin", *args, *(["--ref-first"] if ref_first else [])).stdout.split()
+    assert [int(x) for x in out] == [M, N, n_file]
+    got = np.fromfile(tmp_path / "out.bin", dtype=np.int64).reshape(M, T, 6)
+
+    g = geno(ref_first)[:, kept]
+    ok = g >= 0
+    alt, het = ok & (g >= 1.5), ok & (g >= 0.5) & (g < 1.5)
+    xm = ok & non_par[:, None] & male[None, :] & rule
+    alt, het = np.where(xm, g >= 1, alt), het & ~xm
+    ref = ok & ~alt & ~het
+    want = np.zeros((M, T, 6), dtype=np.int64)
+    for t in range(T):
+        for k, c in enumerate((2, 1) if binary else (1,)):
+            sel = cls[t] == c
+            want[:, t, 3 * k:3 * k + 3] = np.stack([(x & sel).sum(1) for x in (ref, het, alt)], axis=1)
+    assert np.array_equal(got, want)
+    assert (~ok).any() and ((g == 1) & ~ok).sum() == 0
+    if cfg == "nosplit":
+        # N_RA of the --no-split row: the het count is the analysed non-missing calls minus N_RR and N_AA
+        assert np.array_equal(got[:, 0, 1], (ok & (cls[0] == 1)).sum(1) - got[:, 0, 0] - got[:, 0, 2])
+    if rule:
+        if kind == "bed":
+            assert (xm & (g == 1)).any()                                                 # heterozygous males, counted as alt
+        else:
+            assert (xm & (g == 1.0)).any()                                               # dosage exactly 1 in the float expression
+            if ref_first:                                                                # ... and pairs at 255 / 255 that it puts below 1
+                assert (xm & (g < 1) & (g > 1 - 1e-12)).any()
