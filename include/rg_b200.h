@@ -213,7 +213,8 @@ int rg_s2_set_chr(rg_handle h, const double* res, const double* scf_sv);
 /*
  * chrX: rg_s2_set_sex gives the male indicator of every sample (params.sex == 1; NULL = forget it) and takes
  * effect at the next rg_s2_set_chr / rg_s2_set_chr_bt; rg_s2_set_non_par flags the variants of the NEXT block
- * call that lie in the non-PAR part of chrX (in_non_par, src/Geno.cpp:2802-2814).  For those variants males
+ * call that lie in the non-PAR part of chrX (in_non_par, src/Geno.cpp:2802-2814); that call is refused, and the
+ * flags dropped, when n is below its variant count.  For those variants males
  * count half towards the allele count and MAC = min(mac, 2 N - N_males - mac) (src/Geno.cpp:2447-2462,
  * compute_mac :3077-3108), which decides the --minMAC filter; A1FREQ, N and the test itself are unchanged.
  */

@@ -180,7 +180,8 @@ struct Step2State {
   DevBuf<double> maskcount, XmX;
   DevBuf<uint8_t> ones;
   std::vector<uint8_t> male;         // chrX: male indicator of every sample (empty = none), per-block non-PAR flags
-  DevBuf<uint8_t> nonpar;
+  DevBuf<uint8_t> nonpar;             // allocated for bs_max flags at least; nonpar_n of them were given
+  int32_t nonpar_n = 0;
   bool nonpar_set = false;
   S2QtChr qt;
   S2BtChr bt;

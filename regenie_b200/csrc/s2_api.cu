@@ -155,7 +155,7 @@ static void s2_set_chr(rg_ctx* h, const double* res, const double* scf_sv) {
 static const uint8_t* take_non_par(rg_ctx* h, Step2State& s2, int bs) {
   if (!s2.nonpar_set) return nullptr;
   s2.nonpar_set = false;
-  RG_CHECK((int)s2.nonpar.n >= bs, "rg_s2_set_non_par was given fewer flags than the block has variants");
+  RG_CHECK(s2.nonpar_n >= bs, "rg_s2_set_non_par was given fewer flags than the block has variants");
   return s2.nonpar.p;
 }
 
@@ -769,6 +769,7 @@ int rg_s2_set_non_par(rg_handle h, const uint8_t* flags, int32_t n) {
   s2.nonpar.alloc(std::max<size_t>((size_t)n, (size_t)h->bs_max));
   RG_CUDA(cudaMemcpyAsync(s2.nonpar.p, flags, n, cudaMemcpyHostToDevice, h->stream));
   RG_CUDA(cudaStreamSynchronize(h->stream));
+  s2.nonpar_n = n;
   s2.nonpar_set = true;
   RG_API_END
 }

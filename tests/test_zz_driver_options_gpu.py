@@ -142,8 +142,6 @@ def test_htp_output_binary_traits(tmp_path, golden_dir, extra):
     helpers.check_htp_bt(run, read, tmp_path, golden_dir, extra, numbers=True)
 
 
-@pytest.mark.xfail(strict=False, reason="--htp on chromosome X was written after the GPU budget of round 2 was spent: the counts are "
-                   "formed on the host and are green on the mock ABI; not yet run on hardware")
 def test_htp_output_on_chromosome_x(tmp_path, golden_dir):
     def read(path):
         return open(path).read()
