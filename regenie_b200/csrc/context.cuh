@@ -288,6 +288,9 @@ inline Step2State& step2(rg_ctx* h) {
   return *h->s2;
 }
 void ensure_W(rg_ctx* h, Step1State& s1);
+// chunk table of the sample-axis reductions: every fold of the padded layout cut into chunks of at most len samples,
+// (start, length, fold, 0) in fold order, and fold_chunks[f] = [first, last) chunk of fold f
+void fold_chunk_table(const Step1State& s1, int64_t len, std::vector<int4>& chunks, std::vector<int2>& fold_chunks);
 // buf = v, allocated to fit and copied on stream s (v stays alive until s has read it)
 template <class T>
 void upload(DevBuf<T>& buf, const std::vector<T>& v, cudaStream_t s) {

@@ -192,11 +192,6 @@ void launch_dense_from_f64(const double* G, int64_t n_file, int bs, const int32_
 void launch_dense_prepare(double* gd, int64_t npad, int bs, const int32_t* file_idx_pad, const double* xy, int cpp, int C,
                           long long n_analyzed, double numtol, double* mu, double* inv_sd, unsigned long long* err_slot,
                           long long err_base, cudaStream_t s);
-void launch_dense_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y, int64_t part_y_stride,
-                           const int2* fold_chunks, int K, int R, const double* lambda, int bs, int nC, int P, double* cm,
-                           int64_t cm_stride, int loocv, cudaStream_t s);
-void launch_dense_loocv_fill(const double* gd, int64_t npad, int bs, int nC, double* cm, int64_t cm_stride, int row0, int R,
-                             cudaStream_t s);
 void launch_dense_predict(const double* gd, int64_t npad, int bs, const double* cm, int64_t cm_stride, int ldc, int nC, int R,
                           int P, const int32_t* tile_fold, const uint8_t* mask, double* const* W, int col0, cudaStream_t s);
 
@@ -253,8 +248,9 @@ void launch_l1_gram(const double* W, int64_t ldw, int B, const int4* chunks, int
                     int64_t part_stride, int ldp, cudaStream_t s);
 void launch_l1_xty(const double* W, int64_t ldw, const double* xy, int cpp, int ycol, const int4* chunks,
                    int nchunks, double* part_y, int B, cudaStream_t s);
-void launch_l1_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y,
-                        const int2* fold_chunks, int K, int R1, const double* tau, int B, int nC, double* cm,
+// the fold systems of level 1 (P = 1) and of the dense level-0 route; every caller with loocv = 1 passes K = 1
+void launch_l1_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y, int64_t part_y_stride,
+                        int P, const int2* fold_chunks, int K, int R1, const double* tau, int B, int nC, double* cm,
                         int64_t cm_stride, int loocv, cudaStream_t s);
 void launch_l1_pred_sums(const double* W, int64_t ldw, int B, int R1, const double* beta, int ldb,
                          const int32_t* tile_fold, const double* xy, int cpp, int ycol, double* part_out,
@@ -344,6 +340,38 @@ __device__ __forceinline__ void cta_sum(double (&v)[K], double* sh) {
     for (int w = 0; w < kWarps; ++w) s += sh[w * K + k];
     v[k] = s;
   }
+}
+
+// A CTA's fixed-order reduction has two forms: cta_sum (Step 2) adds the lanes of each warp by shuffles and then the
+// warps in order, cta_tree (the Step-1 FP64 kernels) halves a shared-memory tree, sh[t] op sh[t + o] for o = kThreads / 2
+// .. 1.  They pair the values differently, so one form for both would change the last bits of the other step's results.
+// cta_tree: v[k] of every thread combined by kOp (sum or fmax) over a CTA of kThreads threads (128 or 256); every thread
+// receives the totals.  sh holds K * kThreads doubles.  It starts with a barrier, so a caller may loop over it.
+enum class CtaOp { kSum, kMax };
+template <int kThreads, CtaOp kOp = CtaOp::kSum, int K>
+__device__ __forceinline__ void cta_tree(double (&v)[K], double* sh) {
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < K; ++k) sh[k * kThreads + threadIdx.x] = v[k];
+  __syncthreads();
+  for (int o = kThreads / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        double* r = sh + k * kThreads + threadIdx.x;
+        *r = kOp == CtaOp::kMax ? fmax(r[0], r[o]) : r[0] + r[o];
+      }
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) v[k] = sh[k * kThreads];
+}
+template <int kThreads, CtaOp kOp = CtaOp::kSum>
+__device__ __forceinline__ double cta_tree(double v, double* sh) {
+  double a[1] = {v};
+  cta_tree<kThreads, kOp>(a, sh);
+  return a[0];
 }
 
 // N, MAC and AF of column c of a variant's sums (compute_mac / compute_aaf_info, src/Geno.cpp:3077-3148), and INFO when

@@ -6,7 +6,8 @@
 //   Data::calc_cv_matrices          src/Data.cpp:729-776    (per-fold G G^T and G Y on the FP64 tensor pipe: l1_gram_kernel)
 //   ridge_level_0                   src/Step1_Models.cpp:458-613 (batched Cholesky, chol.cu)
 // G~ is kept as [bs][Npad] FP64 in the padded fold layout (row = SNP, contiguous over samples), i.e. exactly the
-// "N x B column-major" shape of the level-1 predictors, so the level-1 Gram / X^T y kernels serve unchanged.
+// "N x B column-major" shape of the level-1 predictors, so level 1's Gram, X^T y, fold-system assembler and LOOCV
+// sample-row fill serve unchanged (l1_kernels.cu, loocv_kernels.cu).
 #include "kernels.cuh"
 
 namespace rg {
@@ -44,17 +45,6 @@ __global__ void dense_from_f64_kernel(const double* __restrict__ G, int64_t n_fi
   gd[(int64_t)row * npad + t] = fi >= 0 ? G[(int64_t)row * n_file + fi] : 0.0;
 }
 
-__device__ __forceinline__ double block_sum_256(double v, double* red) {
-  __syncthreads();
-  red[threadIdx.x] = v;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  return red[0];
-}
-
 // One CTA per SNP row: mean over analysed, non-missing samples; impute; project out the covariate basis; scale to unit
 // sd with the N_analyzed - C divisor; flag sd < numtol like the reference's throw (src/Data.cpp:203-209).  A flagged
 // row (constant, or missing everywhere) is zeroed, so the block's predictors stay finite while the error is reported.
@@ -71,8 +61,8 @@ dense_prepare_kernel(double* __restrict__ gd, int64_t npad, const int32_t* __res
   double tot = 0.0, cnt = 0.0;
   for (int64_t t = threadIdx.x; t < npad; t += 256)
     if (file_idx_pad[t] >= 0 && g[t] != -3.0) { tot += g[t]; cnt += 1.0; }
-  tot = block_sum_256(tot, red);
-  cnt = block_sum_256(cnt, red);
+  tot = cta_tree<256>(tot, red);
+  cnt = cta_tree<256>(cnt, red);
   const double mean = tot / cnt;
   for (int64_t t = threadIdx.x; t < npad; t += 256)
     if (g[t] == -3.0) g[t] = mean;
@@ -80,7 +70,7 @@ dense_prepare_kernel(double* __restrict__ gd, int64_t npad, const int32_t* __res
   for (int c = 0; c < C; ++c) {
     double s = 0.0;
     for (int64_t t = threadIdx.x; t < npad; t += 256) s += g[t] * xy[t * cpp + c];
-    s = block_sum_256(s, red);
+    s = cta_tree<256>(s, red);
     if (threadIdx.x == 0) bc[c] = s;
   }
   __syncthreads();
@@ -92,7 +82,7 @@ dense_prepare_kernel(double* __restrict__ gd, int64_t npad, const int32_t* __res
     g[t] = v;
     ss += v * v;
   }
-  ss = block_sum_256(ss, red);
+  ss = cta_tree<256>(ss, red);
   const double sd = sqrt(ss) / sqrt((double)(n_analyzed - C));
   const bool low = !(sd >= numtol);
   if (threadIdx.x == 0) {
@@ -101,65 +91,6 @@ dense_prepare_kernel(double* __restrict__ gd, int64_t npad, const int32_t* __res
     if (low) atomicMin(err_slot, (unsigned long long)(err_base + blockIdx.x + 1));
   }
   for (int64_t t = threadIdx.x; t < npad; t += 256) g[t] = low ? 0.0 : g[t] / sd;
-}
-
-// K*R shifted systems (row-major lower, ld = nC) + P right-hand-side rows from the chunk partials, fixed summation order.
-// part: [nchunks][nC x ldp] lower tiles of G_chunk G_chunk^T; part_y: [P][nchunks][bs].  LOOCV: R systems, nothing held out.
-// grid: (ceil(nC/128), nC + P), block 128: thread = (j, row i); rows >= nC are right-hand sides.
-__global__ void dense_assemble_kernel(const double* __restrict__ part, int64_t part_stride, int ldp,
-                                      const double* __restrict__ part_y, int64_t part_y_stride,
-                                      const int2* __restrict__ fold_chunks, int K, int R, const double* __restrict__ lambda,
-                                      int bs, int nC, int P, double* __restrict__ cm, int64_t cm_stride, int loocv) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  const int i = blockIdx.y;
-  if (j >= nC) return;
-  const bool is_rhs = i >= nC;
-  if (!is_rhs && j > i) return;
-  const int p = i - nC;
-  const bool real = is_rhs ? (j < bs) : (i < bs);
-  double fold_v[kMaxFolds];
-  double tot = 0.0;
-  for (int f = 0; f < K; ++f) {
-    double s = 0.0;
-    if (real) {
-      const int2 fc = fold_chunks[f];
-      for (int c = fc.x; c < fc.y; ++c)
-        s += is_rhs ? part_y[(int64_t)p * part_y_stride + (int64_t)c * bs + j] : part[(int64_t)c * part_stride + (int64_t)i * ldp + j];
-    }
-    fold_v[f] = s;
-    tot += s;
-  }
-  const int nf = loocv ? 1 : K;
-  for (int f = 0; f < nf; ++f)
-    for (int r = 0; r < R; ++r) {
-      double v;
-      if (real) {
-        v = loocv ? tot : tot - fold_v[f];
-        if (!is_rhs && i == j) v += lambda[r];
-      } else {
-        v = (!is_rhs && i == j) ? 1.0 : 0.0;
-      }
-      cm[(int64_t)(f * R + r) * cm_stride + (int64_t)i * nC + j] = v;
-    }
-}
-
-// LOOCV: the sample vectors ride along as right-hand-side rows of the factorisation: row (row0 + t) = G~[:, t]
-// grid: (Npad/32, ceil(nC/32)), block (32, 8): transpose through shared memory
-__global__ void dense_loocv_fill_kernel(const double* __restrict__ gd, int64_t npad, int bs, int nC, double* __restrict__ cm,
-                                        int64_t cm_stride, int row0, int R) {
-  __shared__ double tl[32][33];
-  const int64_t t0 = (int64_t)blockIdx.x * 32;
-  const int i0 = blockIdx.y * 32;
-  for (int r = threadIdx.y; r < 32; r += 8) {
-    const int i = i0 + r;
-    tl[r][threadIdx.x] = (i < bs) ? gd[(int64_t)i * npad + t0 + threadIdx.x] : 0.0;
-  }
-  __syncthreads();
-  for (int r = threadIdx.y; r < 32; r += 8) {
-    const int64_t t = t0 + r;
-    const double v = tl[threadIdx.x][r];
-    for (int m = 0; m < R; ++m) cm[(int64_t)m * cm_stride + (int64_t)(row0 + t) * nC + i0 + threadIdx.x] = v;
-  }
 }
 
 // Out-of-fold predictions  pred[t][q] = mask_p(t) * sum_i G~[i][t] beta_{f(t)}[r][p][i],  q = r * P + p, written into the
@@ -219,18 +150,6 @@ void launch_dense_prepare(double* gd, int64_t npad, int bs, const int32_t* file_
                           long long err_base, cudaStream_t s) {
   dense_prepare_kernel<<<bs, 256, 0, s>>>(gd, npad, file_idx_pad, xy, cpp, C, n_analyzed, numtol, mu, inv_sd, err_slot,
                                           err_base);
-}
-void launch_dense_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y, int64_t part_y_stride,
-                           const int2* fold_chunks, int K, int R, const double* lambda, int bs, int nC, int P, double* cm,
-                           int64_t cm_stride, int loocv, cudaStream_t s) {
-  dim3 grid((unsigned)ceil_div(nC, 128), nC + P);
-  dense_assemble_kernel<<<grid, 128, 0, s>>>(part, part_stride, ldp, part_y, part_y_stride, fold_chunks, K, R, lambda, bs, nC, P,
-                                             cm, cm_stride, loocv);
-}
-void launch_dense_loocv_fill(const double* gd, int64_t npad, int bs, int nC, double* cm, int64_t cm_stride, int row0, int R,
-                             cudaStream_t s) {
-  dim3 grid((unsigned)(npad / 32), (unsigned)ceil_div(nC, 32));
-  dense_loocv_fill_kernel<<<grid, dim3(32, 8), 0, s>>>(gd, npad, bs, nC, cm, cm_stride, row0, R);
 }
 void launch_dense_predict(const double* gd, int64_t npad, int bs, const double* cm, int64_t cm_stride, int ldc, int nC, int R,
                           int P, const int32_t* tile_fold, const uint8_t* mask, double* const* W, int col0, cudaStream_t s) {

@@ -27,13 +27,8 @@ l0_xy_digits_kernel(const double* __restrict__ xy, int cpp, int ncol, int64_t np
   }
   double mx = 0.0;
   for (int64_t t = threadIdx.x; t < npad; t += 256) mx = fmax(mx, fabs(xy[t * cpp + c]));
-  red[threadIdx.x] = mx;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + o]);
-    __syncthreads();
-  }
-  const double s = red[0] > 0.0 ? red[0] : 1.0;
+  mx = cta_tree<256, CtaOp::kMax>(mx, red);
+  const double s = mx > 0.0 ? mx : 1.0;
   if (threadIdx.x == 0) scale[c] = s;
   uint8_t* base = D + ((int64_t)(c / kStatQ) * 128 + (c % kStatQ) * kLimbs) * npad;
   for (int64_t t = threadIdx.x; t < npad; t += 256) {

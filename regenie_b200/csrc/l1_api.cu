@@ -19,14 +19,8 @@ static void l1_setup_chunks(rg_ctx* h, Step1State& s1, int nC) {
   int64_t len = round_up(std::max<int64_t>(kStatChunk, ceil_div(h->Npad, max_chunks - K + 1)), 128);
   s1.l1_chunk_len = len;
   std::vector<int4> chunks;
-  std::vector<int2> fold_chunks(K);
-  for (int f = 0; f < K; ++f) {
-    fold_chunks[f].x = (int)chunks.size();
-    for (int64_t o = 0; o < s1.fold_pad_len[f]; o += len)
-      chunks.push_back(make_int4((int)(s1.fold_pad_start[f] + o),
-                                 (int)std::min<int64_t>(len, s1.fold_pad_len[f] - o), f, 0));
-    fold_chunks[f].y = (int)chunks.size();
-  }
+  std::vector<int2> fold_chunks;
+  fold_chunk_table(s1, len, chunks, fold_chunks);
   s1.l1_nchunks = (int)chunks.size();
   upload(s1.l1_chunks, chunks, s);
   upload(s1.l1_fold_chunks, fold_chunks, s);
@@ -122,7 +116,7 @@ static void l1_fit(rg_ctx* h, const double* tau_host, double* cumsum, int32_t* b
     const int ycol = h->C + p;
     launch_l1_gram(Wp, Npad, B, s1.l1_chunks.p, nch, s1.l1_part.p, part_stride, nC, s);
     launch_l1_xty(Wp, Npad, s1.xy.p, s1.cpp, ycol, s1.l1_chunks.p, nch, s1.l1_part_y.p, B, s);
-    launch_l1_assemble(s1.l1_part.p, part_stride, nC, s1.l1_part_y.p, s1.l1_fold_chunks.p, K, R1,
+    launch_l1_assemble(s1.l1_part.p, part_stride, nC, s1.l1_part_y.p, 0, 1, s1.l1_fold_chunks.p, K, R1,
                        s1.l1_tau.p + (size_t)p * R1, B, nC, s1.l1_cm.p, cm_stride, s1.loocv, s);
     if (s1.loocv) launch_l1_loocv_fill(Wp, Npad, B, nC, s1.l1_cm.p, cm_stride, nC + 64, R1, Npad, s);
     launch_chol_factor(s1.l1_cm.p, cm_stride, nC, d.n_aug, nmat, s1.l1_inv.p, s1.err_slot.p, (long long)(1ll << 41) + p * 1024, s);
@@ -237,8 +231,8 @@ void lg_factor(LgState& st, double tau) {
   launch_l1_gram(st.s1.lg_Ws.p, st.Npad, st.B, st.s1.l1_chunks.p, st.nch, st.s1.l1_part.p, st.part_stride, nC, s);
   RG_CUDA(cudaMemcpyAsync(st.s1.l1_tau.p, &tau, 8, cudaMemcpyHostToDevice, s));
   // the RHS row is (re)written by the caller after this; part_y content is irrelevant here
-  launch_l1_assemble(st.s1.l1_part.p, st.part_stride, nC, st.s1.l1_part_y.p, st.s1.lg_all_chunks.p, 1, 1, st.s1.l1_tau.p, st.B, nC,
-                     st.s1.l1_cm.p, st.cm_stride, 1, s);
+  launch_l1_assemble(st.s1.l1_part.p, st.part_stride, nC, st.s1.l1_part_y.p, 0, 1, st.s1.lg_all_chunks.p, 1, 1, st.s1.l1_tau.p,
+                     st.B, nC, st.s1.l1_cm.p, st.cm_stride, 1, s);
   h->launches += 3;
 }
 

@@ -50,36 +50,34 @@ l1_xty_kernel(const double* __restrict__ W, int64_t ldw, const double* __restric
   double s = 0.0;
   for (int t = threadIdx.x; t < ch.y; t += 128)
     s += W[(int64_t)i * ldw + ch.x + t] * xy[(int64_t)(ch.x + t) * cpp + ycol];
-  red[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = 64; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) part_y[(int64_t)blockIdx.y * B + i] = red[0];
+  s = cta_tree<128>(s, red);
+  if (threadIdx.x == 0) part_y[(int64_t)blockIdx.y * B + i] = s;
 }
 
-// Sum chunk partials per fold (fixed order), form  XtX_sum - X_folds[f] + tau_j I  and the
-// right-hand side  XtY_sum - XtY[f]  in the batched Cholesky layout (row-major lower, RHS row nC).
-// grid: (ceil(nC/32), nC) -> thread = (j, i)
+// Sum chunk partials per fold (fixed order), form  XtX_sum - X_folds[f] + tau_j I  and the P right-hand sides
+// XtY_sum - XtY[f]  in the batched Cholesky layout (row-major lower, RHS rows nC .. nC + P - 1); LOOCV (K = 1): nothing
+// is held out.  part: [nchunks][nC x ldp] lower tiles; part_y: [P][nchunks][B], right-hand side p at p * part_y_stride.
+// Level 1 (P = 1) and the dense level-0 route (P traits, tau = lambda, B = bs).
+// grid: (ceil(nC/128), nC + P), block 128: thread = (j, row i); rows >= nC are right-hand sides.
 __global__ void l1_assemble_kernel(const double* __restrict__ part, int64_t part_stride, int ldp,
-                                   const double* __restrict__ part_y, const int2* __restrict__ fold_chunks,
-                                   int K, int R1, const double* __restrict__ tau, int B, int nC,
-                                   double* __restrict__ cm, int64_t cm_stride, int loocv) {
+                                   const double* __restrict__ part_y, int64_t part_y_stride,
+                                   const int2* __restrict__ fold_chunks, int K, int R1, const double* __restrict__ tau,
+                                   int B, int nC, double* __restrict__ cm, int64_t cm_stride, int loocv) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  const int i = blockIdx.y;                 // 0..nC-1 matrix rows, nC = RHS row
+  const int i = blockIdx.y;
   if (j >= nC) return;
-  if (i < nC && j > i) return;
+  const bool is_rhs = i >= nC;
+  if (!is_rhs && j > i) return;
+  const int p = i - nC;
+  const bool real = is_rhs ? (j < B) : (i < B);
   double fold_v[kMaxFolds];
   double tot = 0.0;
-  const bool is_rhs = (i == nC);
-  const bool real = is_rhs ? (j < B) : (i < B);
   for (int f = 0; f < K; ++f) {
     double s = 0.0;
     if (real) {
       const int2 fc = fold_chunks[f];
       for (int c = fc.x; c < fc.y; ++c)
-        s += is_rhs ? part_y[(int64_t)c * B + j] : part[(int64_t)c * part_stride + (int64_t)i * ldp + j];
+        s += is_rhs ? part_y[(int64_t)p * part_y_stride + (int64_t)c * B + j] : part[(int64_t)c * part_stride + (int64_t)i * ldp + j];
     }
     fold_v[f] = s;
     tot += s;
@@ -88,7 +86,7 @@ __global__ void l1_assemble_kernel(const double* __restrict__ part, int64_t part
     for (int r = 0; r < R1; ++r) {
       double v;
       if (real) {
-        v = loocv ? tot : tot - fold_v[f];          // LOOCV: nothing is held out of X^T X
+        v = loocv ? tot : tot - fold_v[f];
         if (!is_rhs && i == j) v += tau[r];
       } else {
         v = (!is_rhs && i == j) ? 1.0 : 0.0;
@@ -178,12 +176,12 @@ void launch_l1_xty(const double* W, int64_t ldw, const double* xy, int cpp, int 
   l1_xty_kernel<<<grid, 128, 0, s>>>(W, ldw, xy, cpp, ycol, chunks, part_y, B);
 }
 
-void launch_l1_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y,
-                        const int2* fold_chunks, int K, int R1, const double* tau, int B, int nC, double* cm,
+void launch_l1_assemble(const double* part, int64_t part_stride, int ldp, const double* part_y, int64_t part_y_stride,
+                        int P, const int2* fold_chunks, int K, int R1, const double* tau, int B, int nC, double* cm,
                         int64_t cm_stride, int loocv, cudaStream_t s) {
-  dim3 grid((unsigned)ceil_div(nC, 128), nC + 1);
-  l1_assemble_kernel<<<grid, 128, 0, s>>>(part, part_stride, ldp, part_y, fold_chunks, K, R1, tau, B, nC, cm, cm_stride,
-                                          loocv);
+  dim3 grid((unsigned)ceil_div(nC, 128), nC + P);
+  l1_assemble_kernel<<<grid, 128, 0, s>>>(part, part_stride, ldp, part_y, part_y_stride, fold_chunks, K, R1, tau, B, nC,
+                                          cm, cm_stride, loocv);
 }
 
 void launch_l1_pred_sums(const double* W, int64_t ldw, int B, int R1, const double* beta, int ldb,

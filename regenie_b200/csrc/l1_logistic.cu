@@ -35,13 +35,8 @@ l1_bt_eta_kernel(const double* __restrict__ W, int64_t ldw, int B, const double*
   eta[t] = e;
   wm[t] = code ? p * (1.0 - p) : 0.0;
   resid[t] = code ? ((code == 2 ? 1.0 : 0.0) - p) : 0.0;
-  red[threadIdx.x] = code ? -2.0 * ((code == 1) ? log(1.0 - p) : log(p)) : 0.0;
-  __syncthreads();
-  for (int o = 64; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) dev_part[blockIdx.x] = red[0];
+  const double dev = cta_tree<128>(code ? -2.0 * ((code == 1) ? log(1.0 - p) : log(p)) : 0.0, red);
+  if (threadIdx.x == 0) dev_part[blockIdx.x] = dev;
 }
 
 // score = W^T resid - tau beta from the chunk partials of l1_xty; also written into the RHS row of the system.
@@ -66,7 +61,7 @@ __global__ void __launch_bounds__(128)
 l1_bt_loo_sums_kernel(const double* __restrict__ eta, const double* __restrict__ q, const double* __restrict__ wm,
                       const double* __restrict__ resid, const int8_t* __restrict__ ym, double eps,
                       double* __restrict__ fvec, double* __restrict__ part) {
-  __shared__ double red[6][128];
+  __shared__ double red[6 * 128];
   const int64_t t = blockIdx.x * 128 + threadIdx.x;
   const int8_t code = ym[t];
   double v[6] = {0, 0, 0, 0, 0, 0};
@@ -81,14 +76,9 @@ l1_bt_loo_sums_kernel(const double* __restrict__ eta, const double* __restrict__
     v[5] = -((code == 1) ? log(1.0 - p1) : log(p1));
   }
   if (fvec) fvec[t] = f;
-  for (int k = 0; k < 6; ++k) red[k][threadIdx.x] = v[k];
-  __syncthreads();
-  for (int o = 64; o > 0; o >>= 1) {
-    if (threadIdx.x < o)
-      for (int k = 0; k < 6; ++k) red[k][threadIdx.x] += red[k][threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x < 6) part[(int64_t)blockIdx.x * 6 + threadIdx.x] = red[threadIdx.x][0];
+  cta_tree<128>(v, red);
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 6; ++k) part[(int64_t)blockIdx.x * 6 + k] = v[k];
 }
 
 // per-chromosome LOO predictions: pred[t, chr] = W_chr[t] . beta_chr - (W_chr[t] . z_chr[t]) f_t   (src/Data.cpp:1560-1566)

@@ -110,7 +110,8 @@ __global__ void l0_loocv_std_apply_kernel(double* const* __restrict__ W, int64_t
 }
 
 // ---------------------------------------------------------------------------------------- level 1
-// sample rows of the R1 systems:  row (nrow0 + t) = W[t, 0:B]   (tile transpose, coalesced both ways)
+// sample rows of the R1 systems:  row (nrow0 + t) = W[t, 0:B]   (tile transpose, coalesced both ways); the dense level-0
+// route passes its G~ as W (ldw = Npad, B = bs).
 // grid: (Npad/32, ceil(nC/32)), block (32, 8); the sample axis is grid.x, like l0_loocv_fill_kernel
 __global__ void l1_loocv_fill_kernel(const double* __restrict__ W, int64_t ldw, int B, int nC,
                                      double* __restrict__ cm, int64_t cm_stride, int nrow0, int R1) {

@@ -82,22 +82,11 @@ l0_coef_i8_kernel(const double* __restrict__ cm, int64_t cm_stride, int ldc, int
   for (int c = 0; c < C; ++c) {
     double s = 0.0;
     for (int i = threadIdx.x; i < bs; i += 256) s += sg[i] * Bv[(int64_t)i * C + c];
-    red[threadIdx.x] = s;
-    __syncthreads();
-    for (int o = 128; o > 0; o >>= 1) {
-      if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-      __syncthreads();
-    }
-    if (threadIdx.x == 0) cvec[((int64_t)f * Qp + q) * C + c] = red[0];
-    __syncthreads();
+    s = cta_tree<256>(s, red);
+    if (threadIdx.x == 0) cvec[((int64_t)f * Qp + q) * C + c] = s;
   }
-  red[threadIdx.x] = mx;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) red[threadIdx.x] = fmax(red[threadIdx.x], red[threadIdx.x + o]);
-    __syncthreads();
-  }
-  const double s = red[0] > 0.0 ? red[0] : 1.0;
+  mx = cta_tree<256, CtaOp::kMax>(mx, red);
+  const double s = mx > 0.0 ? mx : 1.0;
   if (threadIdx.x == 0) scale[(int64_t)f * Qp + q] = s;
   const int g = q / kLimbQI8, qq = q % kLimbQI8;
   const int K2 = 2 * rows_p;
@@ -394,25 +383,20 @@ l0_predict_i8_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_const
 __global__ void __launch_bounds__(256)
 l0_colsum_kernel(double* const* __restrict__ W, int64_t npad, int col0, int P, int Qp,
                  double* __restrict__ part) {
-  __shared__ double r1[256], r2[256];
+  __shared__ double red[2 * 256];
   const int q = blockIdx.x, r = q / P, p = q % P;
   const int64_t t0 = (int64_t)blockIdx.y * 8192;
   const double* w = W[p] + (int64_t)(col0 + r) * npad;
-  double s1 = 0.0, s2 = 0.0;
+  double s[2] = {0.0, 0.0};
   for (int64_t t = t0 + threadIdx.x; t < min(t0 + 8192, npad); t += 256) {
     const double v = w[t];
-    s1 += v;
-    s2 = fma(v, v, s2);
+    s[0] += v;
+    s[1] = fma(v, v, s[1]);
   }
-  r1[threadIdx.x] = s1; r2[threadIdx.x] = s2;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) { r1[threadIdx.x] += r1[threadIdx.x + o]; r2[threadIdx.x] += r2[threadIdx.x + o]; }
-    __syncthreads();
-  }
+  cta_tree<256>(s, red);
   if (threadIdx.x == 0) {
-    part[((int64_t)blockIdx.y * Qp + q) * 2 + 0] = r1[0];
-    part[((int64_t)blockIdx.y * Qp + q) * 2 + 1] = r2[0];
+    part[((int64_t)blockIdx.y * Qp + q) * 2 + 0] = s[0];
+    part[((int64_t)blockIdx.y * Qp + q) * 2 + 1] = s[1];
   }
 }
 

@@ -69,6 +69,18 @@ void require_gpu(int device) {
                                  std::to_string(prop.major) + std::to_string(prop.minor));
 }
 
+void fold_chunk_table(const Step1State& s1, int64_t len, std::vector<int4>& chunks, std::vector<int2>& fold_chunks) {
+  const int K = s1.K;
+  chunks.clear();
+  fold_chunks.assign(K, make_int2(0, 0));
+  for (int f = 0; f < K; ++f) {
+    fold_chunks[f].x = (int)chunks.size();
+    for (int64_t o = 0; o < s1.fold_pad_len[f]; o += len)
+      chunks.push_back(make_int4((int)(s1.fold_pad_start[f] + o), (int)std::min<int64_t>(len, s1.fold_pad_len[f] - o), f, 0));
+    fold_chunks[f].y = (int)chunks.size();
+  }
+}
+
 // Build the padded fold layout + all device state shared by the blocks.
 static void build_layout(rg_ctx* h, Step1State& s1, const double* X, const double* Y, const uint8_t* mask,
                          const uint8_t* in_analysis, const int64_t* fold_sizes) {
@@ -159,16 +171,10 @@ static void build_layout(rg_ctx* h, Step1State& s1, const double* X, const doubl
   }
   // chunk table for the f64 reductions
   std::vector<int4> chunks;
-  std::vector<int2> fold_chunks(K), fold_k(K);
-  for (int f = 0; f < K; ++f) {
-    fold_chunks[f].x = (int)chunks.size();
-    for (int64_t o = 0; o < s1.fold_pad_len[f]; o += kStatChunk) {
-      const int len = (int)std::min<int64_t>(kStatChunk, s1.fold_pad_len[f] - o);
-      chunks.push_back(make_int4((int)(s1.fold_pad_start[f] + o), len, f, 0));
-    }
-    fold_chunks[f].y = (int)chunks.size();
+  std::vector<int2> fold_chunks, fold_k(K);
+  fold_chunk_table(s1, kStatChunk, chunks, fold_chunks);
+  for (int f = 0; f < K; ++f)
     fold_k[f] = make_int2((int)(s1.fold_pad_start[f] / 128), (int)(s1.fold_pad_len[f] / 128));
-  }
   s1.nchunks = (int)chunks.size();
 
   cudaStream_t s = h->stream;
@@ -340,27 +346,16 @@ static void enqueue_loocv_predict(rg_ctx* h, Step1State& s1, Step1State::Lane& L
   h->launches += 3;
 }
 
-// FP64 path: assemble the K*R shifted systems, batched Cholesky (DMMA), backward substitution; LOOCV predictions
-// included (they read the factorisation directly).  Solutions end up in the right-hand-side rows of L.cm.
-static void enqueue_solve_f64(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
-  const int C = h->C, P = h->P, R = s1.R;
-  ensure_f64_systems(h, s1, L, d, s);
-  AssembleArgs aa = assemble_args(h, s1, L, d);
-  aa.nC = d.nC; aa.cm = L.cm.p; aa.cm_stride = (int64_t)d.n_aug * d.nC; aa.ldc = d.nC;
-  {
-    ScopedTimer t(h, "l0_assemble", s);
-    launch_l0_assemble(aa, L.rhs.p, P, d.Ppad, d.nmat, s);
-    h->launches += 2;
-  }
-  if (s1.loocv) {
-    ScopedTimer t(h, "loocv_fill", s);
-    launch_l0_loocv_fill(L.gp.p, h->Npad, d.bs, d.nC, L.mu.p, L.inv_sd.p, L.Bv.p, C, s1.xy.p, s1.cpp, L.cm.p, aa.cm_stride,
-                         d.nC + d.Ppad, R, s);
-    h->launches += 1;
-  }
+// What both level-0 routes run once their FP64 systems are in L.cm: the batched Cholesky (DMMA), then either the LOOCV
+// predictions (they read the factorisation directly) or the backward substitution, which leaves the solutions in the
+// right-hand-side rows of L.cm.
+static void enqueue_factor_solve_f64(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
+  const int64_t cm_stride = (int64_t)d.n_aug * d.nC;
+  L.part.alloc((size_t)d.ntiles_s * d.Qp * 2);
+  L.mean_invsd.alloc((size_t)2 * d.Qp);
   {
     ScopedTimer t(h, "chol_factor", s);
-    launch_chol_factor(L.cm.p, aa.cm_stride, d.nC, d.n_aug, d.nmat, L.inv.p, s1.err_slot.p,
+    launch_chol_factor(L.cm.p, cm_stride, d.nC, d.n_aug, d.nmat, L.inv.p, s1.err_slot.p,
                        (long long)(1ll << 40) + (long long)d.block_id * 1024, s);
     h->launches += chol_num_launches(d.nC);
   }
@@ -369,11 +364,28 @@ static void enqueue_solve_f64(rg_ctx* h, Step1State& s1, Step1State::Lane& L, co
     enqueue_loocv_predict(h, s1, L, d, s);
     return;
   }
+  ScopedTimer t(h, "chol_backsolve", s);
+  launch_chol_backsolve(L.cm.p, cm_stride, d.nC, h->P, d.nmat, L.inv.p, s);
+  h->launches += 1;
+}
+
+// FP64 path of the 2-bit route: assemble the K*R shifted systems (LOOCV: with the sample rows), then factor and solve.
+static void enqueue_solve_f64(rg_ctx* h, Step1State& s1, Step1State::Lane& L, const BlockDims& d, cudaStream_t s) {
+  ensure_f64_systems(h, s1, L, d, s);
+  AssembleArgs aa = assemble_args(h, s1, L, d);
+  aa.nC = d.nC; aa.cm = L.cm.p; aa.cm_stride = (int64_t)d.n_aug * d.nC; aa.ldc = d.nC;
   {
-    ScopedTimer t(h, "chol_backsolve", s);
-    launch_chol_backsolve(L.cm.p, aa.cm_stride, d.nC, P, d.nmat, L.inv.p, s);
+    ScopedTimer t(h, "l0_assemble", s);
+    launch_l0_assemble(aa, L.rhs.p, h->P, d.Ppad, d.nmat, s);
+    h->launches += 2;
+  }
+  if (s1.loocv) {
+    ScopedTimer t(h, "loocv_fill", s);
+    launch_l0_loocv_fill(L.gp.p, h->Npad, d.bs, d.nC, L.mu.p, L.inv_sd.p, L.Bv.p, h->C, s1.xy.p, s1.cpp, L.cm.p,
+                         aa.cm_stride, d.nC + d.Ppad, s1.R, s);
     h->launches += 1;
   }
+  enqueue_factor_solve_f64(h, s1, L, d, s);
 }
 
 // Mixed path: K symmetric FP64 fold systems -> tensor-core factorisation / inverse -> FP64 refinement.  Solutions in L.mx_x.
@@ -733,23 +745,16 @@ static void l0_block_dense(rg_ctx* h, const uint8_t* probs, const uint8_t* miss,
     launch_l1_xty(L.gd.p, Npad, s1.xy.p, s1.cpp, C + p, s1.chunks.p, nch, L.dpart_y.p + (size_t)p * nch * bs, bs, s);
   ensure_f64_systems(h, s1, L, d, s);
   const int64_t cm_stride = (int64_t)d.n_aug * nC;
-  launch_dense_assemble(L.dpart.p, part_stride, nC, L.dpart_y.p, (int64_t)nch * bs, s1.fold_chunks.p, K, R, s1.lambda.p, bs, nC,
-                        P, L.cm.p, cm_stride, s1.loocv, s);
-  if (s1.loocv) launch_dense_loocv_fill(L.gd.p, Npad, bs, nC, L.cm.p, cm_stride, nC + d.Ppad, R, s);
-  launch_chol_factor(L.cm.p, cm_stride, nC, d.n_aug, d.nmat, L.inv.p, s1.err_slot.p,
-                     (long long)(1ll << 40) + (long long)block_id * 1024, s);
-  h->launches += 5 + P + chol_num_launches(nC);
-  L.part.alloc((size_t)d.ntiles_s * d.Qp * 2);
-  L.mean_invsd.alloc((size_t)2 * d.Qp);
-  if (s1.loocv) {
-    enqueue_loocv_predict(h, s1, L, d, s);
-    return;
-  }
-  launch_chol_backsolve(L.cm.p, cm_stride, nC, P, d.nmat, L.inv.p, s);
+  launch_l1_assemble(L.dpart.p, part_stride, nC, L.dpart_y.p, (int64_t)nch * bs, P, s1.fold_chunks.p, K, R, s1.lambda.p, bs,
+                     nC, L.cm.p, cm_stride, s1.loocv, s);
+  if (s1.loocv) launch_l1_loocv_fill(L.gd.p, Npad, bs, nC, L.cm.p, cm_stride, nC + d.Ppad, R, Npad, s);
+  h->launches += 5 + P;
+  enqueue_factor_solve_f64(h, s1, L, d, s);
+  if (s1.loocv) return;
   launch_dense_predict(L.gd.p, Npad, bs, L.cm.p, cm_stride, nC, nC, R, P, s1.tile_fold.p, s1.mask.p, s1.W_tab.p, d.col0, s);
   const int nparts = launch_l0_colsum(s1.W_tab.p, Npad, d.col0, P, d.Q, d.Qp, L.part.p, s);
   launch_l0_standardize(L.part.p, nparts, d.Qp, d.Q, P, s1.neff.p, L.mean_invsd.p, s1.W_tab.p, Npad, d.col0, s1.is_real.p, s);
-  h->launches += 6;
+  h->launches += 5;
 }
 
 // ---- rg_debug_fetch (test hook): a name resolves to device bytes or to a small vector built on the host

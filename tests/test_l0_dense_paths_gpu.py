@@ -2,7 +2,7 @@
 the shapes that select its chunking, tiling and solver.
 
 The route decodes the probability pairs into an FP64 [bs][Npad] matrix, imputes / residualises / scales it
-(dense_prepare), sums per-chunk Gram partials of kStatChunk = 2048 padded samples per fold (dense_assemble), factors the
+(dense_prepare), sums per-chunk Gram partials of kStatChunk = 2048 padded samples per fold (level 1's l1_assemble), factors the
 K*R shifted systems (batched Cholesky) and predicts in tiles of DQ = 25 outputs (dense_predict); LOOCV carries the samples
 as extra right-hand-side rows of the factorisation and predicts in tiles of at most 8 phenotypes (l0_loocv_pred).
 Every case asserts through the "dims" hook (Npad, rp, nC, n_aug, nmat, K, cpp, nchunks) which shape ran, and compares
@@ -200,7 +200,7 @@ def test_sixteen_folds(tmp_path, R):
 
 def test_loocv_many_chunks_two_pheno_tiles(tmp_path):
     """LOOCV at N = 66 000 (past the 65 280 padded samples that once capped a grid axis): the sample rows of
-    dense_loocv_fill span many chunks, and P = 9 runs l0_loocv_pred in two phenotype tiles (8 + 1)."""
+    l1_loocv_fill span many chunks, and P = 9 runs l0_loocv_pred in two phenotype tiles (8 + 1)."""
     c = Case(_fileset(tmp_path, 66000, P=9, seed=23), loocv=True)
     bs = 64
     probs, miss = _probs(np.random.default_rng(104), bs, c.pb.n_file)

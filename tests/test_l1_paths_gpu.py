@@ -6,7 +6,7 @@ Level 1 picks its work split from the shape of the input:
     max_chunks = max(K, 2^30 / (8 nC^2)), so a fold spans several chunks once it is longer than 2048 samples, and the
     1 GiB cap on the chunk partials sets the length once nC is large (nC = 2560: max_chunks = 20);
   * l1_pred_sums_kernel stages beta 256 columns at a time, with R1 * 256 doubles of dynamic shared memory;
-  * l1_assemble_kernel keeps one partial per fold (K <= 16);
+  * l1_assemble_kernel, which also assembles the dense level-0 route's systems, keeps one partial per fold (K <= 16);
   * l0_loocv_pred_kernel loops over tiles of 8 phenotypes; the LOOCV fill kernels put the sample axis on grid.x.
 Level 1 is fed straight through rg_l0_load_W with a synthetic W shaped like level 0's output: every case asserts
 through the "l1_dims" / "l1_chunks" hooks which split ran.  The synthetic W holds multiples of 2^-8 below 8 in
@@ -281,7 +281,7 @@ def test_chunk_length_set_by_the_partial_cap():
 def test_column_tiling_ridge_and_fold_counts(B, R, R1, K):
     """B = 5 (one partial DMMA tile), 64 (one exact tile), 65 (a tile and one column), 300 (two beta passes of 256 and
     44 columns); R1 = 2 and 8 (the smallest and largest dynamic shared memory of l1_pred_sums_kernel); K = 2 and
-    16 (the bounds of fold_v in l1_assemble_kernel).  Uneven folds."""
+    16 (the bounds of fold_v in l1_assemble_kernel, which level 0's dense route shares).  Uneven folds."""
     N = 4100
     rng = np.random.default_rng(B)
     fs = rng.multinomial(N - 150 * K, np.ones(K) / K) + 150
